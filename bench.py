@@ -1,11 +1,14 @@
 #!/usr/bin/env python
-"""bench.py — TT-SVD GElements/s on B200 (BASELINE.json metric), one JSON line on rank 0.
+"""bench.py — TT-SVD GElements/s on H100 (BASELINE.json metric), one JSON line on rank 0.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--shape 64,64,64,64,64] [--rank 32]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 ... bench.py --gpus N ...
 
 A "step" = one tnb_ttsvd_batch call per GPU: the complete TT-SVD (tn.Tensor(X[B, ...], ranks_tt=r, batch=True)) of
---per-gpu-batch dense fp32 tensors.
+--per-gpu-batch dense fp32 tensors (fewer when they do not fit in 60 % of the free device memory).
+--dump-outputs DIR writes the cores the last timed step returned as DIR/t<b>_core<k>.npy (float32); the inputs are
+seeded, so two builds run with the same arguments can be compared output for output.
 Workload: BASELINE.json configs[1] names 64^8 (2^48 elements = 1.1 PB) which cannot exist on any
 machine; the stand-in is the largest 64^d that fits one GPU, randn(64,64,64,64,64) fp32 (4 GiB),
 target TT-rank 32 (SURVEY.md §0.4 / §8d, BASELINE.md §2).  Multi-GPU: weak scaling, the batch dimension
@@ -35,11 +38,13 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-tc", action="store_true", help="generic CUDA-core kernels only (A/B runs)")
     ap.add_argument("--cpu-shape", default="32,32,32,32,32", help="bounded sample timed on the host cores")
-    ap.add_argument("--reserve-sms", type=int, default=-1, help="SMs left free by the persistent kernels (measured: no gain on B200, default 0)")
+    ap.add_argument("--reserve-sms", type=int, default=-1, help="SMs left free by the persistent kernels (default: 4 when several tensors are in flight, else 0)")
     ap.add_argument("--per-gpu-batch", type=int, default=8,
                     help="independent tensors per GPU and step, decomposed by ONE tnb_ttsvd_batch call (the library keeps "
                          "them in flight on internal streams: the latency-bound eigen chains of one tensor run beside the "
                          "bandwidth-bound Gram/projection kernels of another)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the cores of the last timed step as DIR/t<b>_core<k>.npy (float32)")
     return ap.parse_args()
 
 
@@ -74,7 +79,7 @@ def workload_config(args):
     return {"workload": f"TT-SVD randn{shape} fp32 -> TT-rank {args.rank} (stand-in for the infeasible 64^8: 1.1 PB)",
             "per_gpu_batch": max(1, args.per_gpu_batch),
             "parallelism": "batch-sharded over the GPUs (independent tensors), all-gather of the final cores",
-            "l2": "input 4 GiB >> 126 MB L2 (no flush needed)"}
+            "l2": "input 4 GiB >> 50 MB L2 (no flush needed)"}
 
 
 class CpuArm:
@@ -254,23 +259,21 @@ def algorithmic_bytes(shape, rank, esz=4):
 
 
 def tf32_peak_tflops(peaks):
-    """Dense TF32 tcgen05 peak: measured on the box by scripts/measure_tf32_peak.py when its result is committed
-    (profiles/r02_tf32_peak.json), else half the measured burst bf16 cuBLAS rate (the kernel is timed alone)."""
-    try:
-        d = json.load(open(os.path.join(REPO, "profiles", "r02_tf32_peak.json")))
-        return float(d["tf32_tflops"]), "measured TF32 tcgen05 peak (profiles/r02_tf32_peak.json: " + d.get("how", "") + ")"
-    except Exception:
-        pass
-    return float(peaks.get("bf16_tflops", 1700.0)) / 2, "TF32 dense peak taken as half the measured burst bf16 cuBLAS rate (kernel timed alone)"
+    """Dense TF32 peak: half the measured burst bf16 rate when MEASURED_PEAKS.json has one, else the H100 SXM data
+    sheet's 495 TFLOP/s (a power-limited card reaches less)."""
+    if "bf16_tflops" in peaks:
+        return float(peaks["bf16_tflops"]) / 2, "TF32 dense peak taken as half the measured burst bf16 rate"
+    return 495.0, "H100 SXM data-sheet dense TF32 (700 W card)"
 
 
-def ncu_traffic_from_profiles(kind, step):
-    """dram bytes per launch of the dominant kernels, read at run time from the committed ncu summary (never pasted)."""
-    try:
-        d = json.load(open(os.path.join(REPO, "profiles", "r02_ncu_traffic.json")))
-        return d.get(f"{kind}{step}")
-    except Exception:
-        return None
+def dump_outputs(path, cores_list):
+    """The cores a caller of the timed path receives, one float32 .npy per core (8 x 64^5 -> r 32: ~6 MB)."""
+    import numpy as np
+
+    os.makedirs(path, exist_ok=True)
+    for b, cores in enumerate(cores_list):
+        for k, c in enumerate(cores):
+            np.save(os.path.join(path, f"t{b}_core{k}.npy"), c.detach().float().cpu().numpy())
 
 
 def run_ours(args):
@@ -296,9 +299,8 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback (B200_PROFILING.md)"
-    bf16_burst = float(peaks.get("bf16_tflops", 1700.0))
+    hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+    peak_src = "measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "H100 SXM data sheet (3.35 TB/s)"
 
     # ---- the batch of this rank: PB independent tensors, decomposed by ONE library call per step (tnb_ttsvd_batch:
     # ---- the same entry point tn.Tensor(X[B, ...], ranks_tt=r, batch=True) and dist.ttsvd_batch_sharded go through)
@@ -310,7 +312,7 @@ def run_ours(args):
     PB = max(1, min(PB, int(0.6 * free_b // per_tensor)))  # bounded by free HBM (inputs + workspaces), never grown
     reserve = args.reserve_sms if args.reserve_sms >= 0 else (4 if PB > 1 else 0)
     ops.set_reserved_sms(reserve)
-    Xb = torch.empty((PB,) + shape, device=dev, dtype=torch.float32)  # PB x 4 GiB >> 126 MB L2
+    Xb = torch.empty((PB,) + shape, device=dev, dtype=torch.float32)  # PB x 4 GiB >> 50 MB L2
     for b in range(PB):
         g = torch.Generator(device=dev).manual_seed(1234 + rank_id * 16 + b)
         Xb[b].copy_(torch.randn(shape, generator=g, device=dev, dtype=torch.float32))
@@ -347,6 +349,8 @@ def run_ours(args):
     barrier()
     ms_total = e0.elapsed_time(e1)
     launches = ops.launch_count() - l0
+    if args.dump_outputs and rank_id == 0:
+        dump_outputs(args.dump_outputs, cores_list)
     clocks = sampler.stop() if rank_id == 0 else None
     t = torch.tensor([ms_total], device=dev, dtype=torch.float64)
     if world > 1:
@@ -415,7 +419,7 @@ def run_ours(args):
         rws_k, cls_k, rr_k = dims[s_k]
         if kind_k == "gram" and cls_k > 512:  # compute-bound symmetric Gram: rows*cols*(cols+1) flops on the upper triangle
             fl = rws_k * cls_k * (cls_k + 1)
-            return {"kernel": "gram_tc2_kernel, cta_group::2 (" + name_k + ")", "bound": "tensor", "achieved": fl / ms_k / 1e9,
+            return {"kernel": "gram_tc_kernel (" + name_k + ")", "bound": "tensor", "achieved": fl / ms_k / 1e9,
                     "peak": tf32_peak, "unit": "TFLOP/s", "alg_flops": fl, "peak_note": tf32_note, "ms": ms_k}
         by = rws_k * cls_k * 4 + (rws_k * rr_k * 4 if kind_k == "factor" else 0)
         return {"kernel": ("gram_tc_kernel (" + name_k + ")") if kind_k == "gram" else name_k, "bound": "hbm",
@@ -423,8 +427,6 @@ def run_ours(args):
 
     roof = kernel_roof(top_ms, top_name, top_s, top_kind)
     roof["frac"] = roof["achieved"] / roof["peak"]
-    roof["traffic"] = ncu_traffic_from_profiles(top_kind, top_s) if list(shape) == [64] * 5 and args.rank == 32 and not args.no_tc else None
-    roof["traffic_source"] = "profiles/r02_ncu_traffic.json (ncu --set full, dram__bytes_read.sum + dram__bytes_write.sum per launch)" if roof["traffic"] else None
     roof["peak_source"] = peak_src
     others = []
     for ms_k, name_k, s_k, kind_k in cand[:4]:
@@ -543,7 +545,7 @@ def run_ours(args):
         out = {
             "metric": METRIC, "value": value, "unit": "GElements/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak",
-            "vs_baseline": None, "dtype": "f32 (Gram: tcgen05 kind::tf32, fp32 TMEM accumulation; projections: 3xTF32 on tcgen05 = fp32 accuracy; Gram matrices, eigenproblems and rank rule in fp64)"
+            "vs_baseline": None, "dtype": "f32 (Gram: tf32 tensor-core MMA, fp32 accumulation; projections: 3xTF32 on the tensor cores = fp32 accuracy; Gram matrices, eigenproblems and rank rule in fp64)"
             if not args.no_tc else "f32 (fp64-accumulated Gram, fp32 projections)",
             "data": "synthetic",
             "config": workload_config(args),

@@ -1,5 +1,5 @@
 /*
- * tnb200 — B200-native (sm_100a) decomposition / rounding hot path for tntorch.
+ * tnb200 — H100-native (sm_90a) decomposition / rounding hot path for tntorch.
  *
  * C-ABI drop-in boundary.  The reference (rballester/tntorch) is 100 % Python and has no
  * FFI of its own (SURVEY.md §8b); these entry points are what a ctypes binding added to the
@@ -57,7 +57,7 @@ uint64_t tnb_launch_count(void);
 /* Number of SMs the one-CTA-per-SM kernels (tensor-core Gram, projection) leave free, so that the latency-bound
  * one-CTA kernels of another in-flight decomposition (other stream) can run beside them.  Default 0. */
 void tnb_set_reserved_sms(int32_t n);
-/* 1 if the tcgen05/TMA kernels are usable on the current device (sm_100), else 0 */
+/* 1 if the TMA tensor-core kernels are usable on the current device (sm_90), else 0 */
 int tnb_has_tensorcore_path(void);
 
 /* ------------------------------------------------------------------------------------------
@@ -179,9 +179,9 @@ int tnb_tt_sum_round(int dtype, const void* const* cores_in, int noperands, cons
 int tnb_tt_hadamard(int dtype, const void* const* cores_a, const void* const* cores_b, int ndim, const int64_t* shape,
                     const int32_t* ranks_a, const int32_t* ranks_b, void* const* cores_out, void* stream);
 
-/* Measurement helper (bench.py / profiles/, SURVEY.md §8d): dense TF32 tcgen05 peak of this GPU — one CTA per SM issuing
- * tcgen05.mma.cta_group::1.kind::tf32 M=128 N=256 K=8 back to back on shared-memory-resident tiles (no memory traffic),
- * `reps` commits of `per_commit` MMAs; best of `trials` launches timed with CUDA events.  The denominator of the
+/* Measurement helper (SURVEY.md §8d): dense TF32 peak of this GPU for the MMA the kernels use — two CTAs per SM whose
+ * warps issue mma.sync.m16n8k8 .tf32 back to back on register operands into eight accumulators (no memory traffic),
+ * `reps` x `per_commit` MMAs per accumulator; best of `trials` launches timed with CUDA events.  The denominator of the
  * tensor-bound roofline fractions. */
 int tnb_measure_tf32_peak(int32_t reps, int32_t per_commit, int32_t trials, double* tflops_host, double* ms_host, void* stream);
 
@@ -293,12 +293,12 @@ int tnb_qr_householder(const double* A, int32_t nbatch, int32_t rows, int32_t n,
 size_t tnb_gram_workspace_bytes(int dtype, int64_t rows, int64_t n);
 int tnb_gram(int dtype, const void* A, int64_t rows, int64_t n, double* G, void* workspace, size_t workspace_bytes,
              void* stream);
-/* Same Gram on the tcgen05 tensor cores: TMA-staged slabs, kind::tf32 MMA, fp32 accumulation in TMEM
+/* Same Gram on the tensor cores: TMA-staged slabs, tf32 mma.sync, fp32 accumulation in registers
  * (fp32 input only, n % 4 == 0).  Output fp64 G like tnb_gram. */
 size_t tnb_gram_tc_workspace_bytes(int64_t rows, int64_t n);
 int tnb_gram_tc_f32(const float* A, int64_t rows, int64_t n, double* G, void* workspace, size_t workspace_bytes,
                     void* stream);
-/* C (m x n) = alpha * A^T B + beta * D on the same tcgen05 kernel (A: K x m, B: K x n, row-major fp32, TF32
+/* C (m x n) = alpha * A^T B + beta * D on the same tensor-core kernel (A: K x m, B: K x n, row-major fp32, TF32
  * operands, fp32 accumulation; m, n multiples of 4, >= 32).  The Chebyshev-filter products G*Y of
  * tnb_eig_topk's subspace iteration run through this entry (G symmetric => A = G).  D may be NULL. */
 size_t tnb_atb_tc_workspace_bytes(int64_t K, int64_t m, int64_t n);
@@ -309,7 +309,7 @@ int tnb_atb_tc_f32(const float* A, int64_t K, int64_t m, const float* B, int64_t
  * blocks n x b fp32).  G stays partitioned over the shared memories of the grid for all steps; clusters of 8
  * CTAs reduce their partial tiles through distributed shared memory.  bufs = three n x b device blocks,
  * bufs[0] = Y_0 on entry; the result is left in bufs[steps % 3].  n % 256 == 0, n <= 2048, b % 4 == 0,
- * steps <= 48.  When 8-CTA clusters for all slabs cannot be co-resident (n = 2048 on B200) the partial tiles go
+ * steps <= 48.  When 8-CTA clusters for all slabs cannot be co-resident the partial tiles go
  * through L2 with a second grid barrier per step.  TNB_ERR_UNSUPPORTED outside that envelope. */
 size_t tnb_cheb_filter_workspace_bytes(int32_t n, int32_t b);
 int tnb_cheb_filter_f32(const float* G, int32_t n, int32_t b, float* buf0, float* buf1, float* buf2, int32_t steps,
@@ -318,7 +318,7 @@ int tnb_cheb_filter_f32(const float* G, int32_t n, int32_t b, float* buf0, float
 /* C (rows x r) = A (rows x n) * V (n x r), same dtype throughout (fp32: FFMA, fp32 accumulate).
  * Replaces: `M @ left` round.py:181 / einsum absorb tensor.py:2081-2083. */
 int tnb_project(int dtype, const void* A, int64_t rows, int64_t n, const void* V, int32_t r, void* C, void* stream);
-/* The same projection on the tcgen05 tensor cores at fp32 accuracy (3xTF32 split: A_hi V_hi + A_hi V_lo + A_lo V_hi),
+/* The same projection on the tensor cores at fp32 accuracy (3xTF32 split: A_hi V_hi + A_hi V_lo + A_lo V_hi),
  * fp32 only, r <= 64, n % 4 == 0, rows >= 128.  Used by the sweep for the large carries. */
 size_t tnb_project_tc_workspace_bytes(int64_t n, int32_t r);
 int tnb_project_tc_f32(const float* A, int64_t rows, int64_t n, const float* V, int32_t r, float* C, void* workspace,

@@ -343,3 +343,11 @@ def ttmatrix_input(spec):
     rows, cols = math.prod(spec["input_dims"]), math.prod(spec["output_dims"])
     shape = ([spec["batch"]] if spec["batch"] else []) + [rows, cols]
     return _rng(spec["seed"]).standard_normal(shape)
+
+
+def golden_prod(g, key):
+    """L @ R of a truncated_svd.npz case: stored whole, or (to keep the file small) as the case's common column basis
+    times per-key coefficients, exact to ~1e-15 relative."""
+    if key + "/prod" in g.files:
+        return g[key + "/prod"]
+    return g[key.split("/")[0] + "/prod_basis"] @ g[key + "/prod_coef"]

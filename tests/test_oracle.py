@@ -89,7 +89,7 @@ def test_truncated_svd_oracle_matches_reference(name, alg, lo):
     if not (alg == "eig" and name == "lowrank_60x80"):
         assert left.shape[1] == int(g[key + "/rank"])
         tol = 1e-4 if M.dtype == np.float32 else 1e-8
-        np.testing.assert_allclose(left.astype(np.float64) @ right.astype(np.float64), g[key + "/prod"], atol=tol * max(1.0, np.abs(M).max()))
+        np.testing.assert_allclose(left.astype(np.float64) @ right.astype(np.float64), cases.golden_prod(g, key), atol=tol * max(1.0, np.abs(M).max()))
 
 
 def test_truncated_svd_errors():

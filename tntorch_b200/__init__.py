@@ -1,4 +1,4 @@
-"""tntorch_b200 — B200-native (sm_100a) decomposition / rounding hot path of rballester/tntorch.
+"""tntorch_b200 — H100-native (sm_90a) decomposition / rounding hot path of rballester/tntorch.
 
 Drop-in surface for that path: ``Tensor(data, ranks_tt=/eps=)``, ``Tensor.round_tt``, ``round_tt``,
 ``round``, ``truncated_svd``, ``relative_error``, ``Tensor(data, ranks_cp=)`` (CP-ALS), ``cross`` (TT-cross).  Importing does not need a GPU; every compute call does.

@@ -1,4 +1,4 @@
-"""Build libtnb200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libtnb200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python tntorch_b200/csrc/build.py [--force] [--verbose]
 """
@@ -24,7 +24,7 @@ def build(force=False, verbose=False):
         return OUT
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     cmd = [
-        nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+        nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
         "-shared", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
         "-I", os.path.join(HERE, "..", "..", "include"),
         "-o", OUT,

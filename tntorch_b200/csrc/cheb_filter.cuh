@@ -7,16 +7,16 @@
 //
 //   * a cluster of 8 CTAs owns a 128-row slab of the output; CTA q of the cluster holds the G block
 //     (K-slice q: rows [q*n/8, (q+1)*n/8)) x (128 slab columns) — G is symmetric, so this block is the
-//     MN-major A operand of the slab's product — loaded by TMA (128B swizzle, 32B atoms) before step 1;
-//   * each step: TMA-load the matching K-slice of Y_{s-1} (n/8 x b, L2 resident), tcgen05.mma tf32
-//     128 x b x n/8 into TMEM, drain TMEM -> shared memory, cluster barrier, every CTA sums 16 of the
-//     slab's rows over the 8 partial tiles through distributed shared memory, applies the three-term
-//     recurrence and writes its 16 rows of Y_s;
+//     MN-major A operand of the slab's product — loaded by TMA (128B swizzle) before step 1;
+//   * each step: TMA-load the matching K-slice of Y_{s-1} (n/8 x b, L2 resident), 128 x b x n/8 tf32 product
+//     on the tensor cores (mma.sync, four warps of 32 rows, accumulators in registers) into shared memory,
+//     cluster barrier, every CTA sums 16 of the slab's rows over the 8 partial tiles through distributed
+//     shared memory, applies the three-term recurrence and writes its 16 rows of Y_s;
 //   * a grid-wide barrier (all CTAs are co-resident: cooperative launch) separates the steps.
 //
-// A B200 schedules at most 15 clusters of 8 CTAs with this shared-memory footprint (one GPC has room for
-// only one), so n = 2048 (16 slabs) cannot use the cluster form: there the 8 partial tiles of a slab go
-// through L2 instead (row-major partial tiles, coalesced both ways) with a second grid barrier per step.
+// When the GPU cannot hold n/128 clusters of 8 CTAs with this shared-memory footprint at once
+// (cudaOccupancyMaxActiveClusters, asked once per device), the 8 partial tiles of a slab go through L2 instead
+// (row-major partial tiles, coalesced both ways) with a second grid barrier per step.
 //
 // Only the FILTER runs here (TF32 operands: operator accuracy affects the convergence rate only); the
 // Rayleigh-Ritz product stays on the fp32 FFMA path (eig.cuh).
@@ -25,7 +25,6 @@
 
 #include "common.cuh"
 #include "gram_tc.cuh"
-#include "gram_tc2.cuh"
 
 namespace tnb {
 
@@ -58,7 +57,6 @@ struct ChebFilterParams {
   float a[CF_MAX_STEPS], bc[CF_MAX_STEPS], g[CF_MAX_STEPS];
   float* buf[3];   // rotating n x b blocks: step s reads buf[(s-1)%3] (and buf[(s-2)%3]), writes buf[s%3]
   unsigned* counter;  // zeroed grid-barrier counter
-  int tmem_cols;
   int dsmem;          // 1: launched as clusters of 8, partial tiles reduced through distributed shared memory
   float* partial;     // dsmem == 0: [slab][q][128][nbox*32] partial tiles in global memory (L2 resident)
   const ChfsiCtrl* ctrl;  // non-null: steps / coefficients / ring rotation come from the device control block
@@ -89,6 +87,37 @@ __device__ __forceinline__ void cf_grid_barrier(unsigned* ctr, unsigned target) 
   }
 }
 
+// NB = nbox: the warp's 32 x (32 NB) share of the 128 x bn partial tile of this CTA's K-slice
+template <int NB>
+__device__ __forceinline__ void cf_product(const unsigned char* g_sm, const unsigned char* y_sm, int nchunk, int nbox,
+                                           float (&acc)[2][4 * NB][4]) {
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31, g = lane >> 2, t = lane & 3;
+#pragma unroll
+  for (int i = 0; i < 2; ++i)
+#pragma unroll
+    for (int j = 0; j < 4 * NB; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) acc[i][j][e] = 0.f;
+  for (int c = 0; c < nchunk; ++c) {
+    const unsigned char* ga = g_sm + (size_t)c * 4 * TC_BOX_BYTES;
+    const unsigned char* yb = y_sm + (size_t)c * nbox * TC_BOX_BYTES;
+#pragma unroll
+    for (int ks = 0; ks < 32; ks += 8) {
+      uint32_t af[2][4];
+      mma_frag_a_mn(ga, ks, 32 * w, g, t, af[0]);
+      mma_frag_a_mn(ga, ks, 32 * w + 16, g, t, af[1]);
+#pragma unroll
+      for (int j = 0; j < 4 * NB; ++j) {
+        uint32_t bf[2];
+        mma_frag_b_mn(yb, ks, 8 * j, g, t, bf);
+        mma_tf32(acc[0][j], af[0][0], af[0][1], af[0][2], af[0][3], bf[0], bf[1]);
+        mma_tf32(acc[1][j], af[1][0], af[1][1], af[1][2], af[1][3], bf[0], bf[1]);
+      }
+    }
+  }
+}
+
+template <int NB>
 __global__ void __launch_bounds__(CF_THREADS, 1)
 cheb_filter_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_constant__ CUtensorMap tmap_y0,
                    const __grid_constant__ CUtensorMap tmap_y1, const __grid_constant__ CUtensorMap tmap_y2,
@@ -109,10 +138,9 @@ cheb_filter_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_cons
   uint64_t* bars = reinterpret_cast<uint64_t*>(red + (size_t)p.nbox * 32 * CF_RED_LD);
   uint64_t* g_bar = bars;
   uint64_t* y_bar = bars + 1;
-  uint64_t* mma_bar = bars + 2;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(bars + 3);
 
   const int tid = threadIdx.x, warp_idx = tid >> 5, lane = tid & 31;
+  const int g = lane >> 2, t = lane & 3;
   const uint32_t q = blockIdx.x % CF_KS;         // K-slice of this CTA (= its rank in the cluster, if any)
   const int slab = blockIdx.x / CF_KS;           // 128-row slab of the output
   const int m0 = slab * 128, k0 = (int)q * p.ksl;
@@ -122,19 +150,9 @@ cheb_filter_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_cons
   if (tid == 0) {
     mbar_init(g_bar, 1);
     mbar_init(y_bar, 1);
-    mbar_init(mma_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp_idx == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)),
-                 "r"((uint32_t)p.tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   if (tid == 0) {
     // resident block of G: rows k0..k0+ksl, columns m0..m0+128
@@ -143,9 +161,8 @@ cheb_filter_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_cons
       for (int j = 0; j < 4; ++j)
         tma_load_2d(g_sm + ((size_t)c * 4 + j) * TC_BOX_BYTES, &tmap_g, g_bar, m0 + 32 * j, k0 + 32 * c);
   }
-  cluster_sync_all();  // every CTA of the cluster is running before any DSMEM access
+  if (p.dsmem) cluster_sync_all();  // every CTA of the cluster is running before any DSMEM access
 
-  const uint32_t idesc = make_idesc_tf32_mn(128, bn);
   const uint32_t red_addr = smem_u32(red);
   const int row_base = m0 + 16 * (int)q;  // the 16 output rows this CTA reduces and writes
 
@@ -165,22 +182,8 @@ cheb_filter_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_cons
       for (int c = 0; c < nchunk; ++c)
         for (int j = 0; j < p.nbox; ++j)
           tma_load_2d(y_sm + ((size_t)c * p.nbox + j) * TC_BOX_BYTES, tm, y_bar, 32 * j, k0 + 32 * c);
-      if (s == 1) mbar_wait(g_bar, 0);
-      mbar_wait(y_bar, par);
-      tcgen05_fence_after();
-      const uint32_t ga = smem_u32(g_sm), ya = smem_u32(y_sm);
-      for (int c = 0; c < nchunk; ++c) {
-#pragma unroll
-        for (int ks = 0; ks < 4; ++ks) {
-          const uint64_t adesc = make_mn_major_desc(ga + (uint32_t)c * 4u * TC_BOX_BYTES + ks * 1024u, TC_BOX_BYTES, 512, 1);
-          const uint64_t bdesc =
-              make_mn_major_desc(ya + (uint32_t)c * (uint32_t)p.nbox * TC_BOX_BYTES + ks * 1024u, TC_BOX_BYTES, 512, 1);
-          tcgen05_mma_tf32(tmem_base, adesc, bdesc, idesc, (c > 0 || ks > 0) ? 1u : 0u);
-        }
-      }
-      tcgen05_commit(mma_bar);
     }
-    // operands of the recurrence for this thread's share of the 16 x b output rows (independent of the MMA)
+    // operands of the recurrence for this thread's share of the 16 x b output rows (independent of the product)
     float vc[16], vp[16];
 #pragma unroll
     for (int cnt = 0; cnt < 16; ++cnt) {
@@ -194,20 +197,19 @@ cheb_filter_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_cons
         if (cg != 0.f) vp[cnt] = __ldcg(yprev + off);
       }
     }
-    mbar_wait(mma_bar, par);
-    __syncwarp();
-    tcgen05_fence_after();
+    if (s == 1) mbar_wait(g_bar, 0);
+    mbar_wait(y_bar, par);
+    float acc[2][4 * NB][4];
+    cf_product<NB>(g_sm, y_sm, nchunk, NB, acc);
+    // accumulator (row 32w + 16i + g + 8h, column 8j + 2t + e) of the 128 x bn partial tile
     if (p.dsmem) {
-      const int row = warp_idx * 32 + lane;  // accumulator row = slab row
-      for (int c0 = 0; c0 < bn; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(warp_idx * 32) << 16) + (uint32_t)c0, v);
-        tmem_ld_wait();
 #pragma unroll
-        for (int i = 0; i < 32; ++i) red[(size_t)(c0 + i) * CF_RED_LD + row] = __uint_as_float(v[i]);
-      }
-      tcgen05_fence_before();
-      __syncwarp();
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int j = 0; j < 4 * NB; ++j)
+#pragma unroll
+          for (int e = 0; e < 4; ++e)
+            red[(size_t)(8 * j + 2 * t + (e & 1)) * CF_RED_LD + 32 * warp_idx + 16 * i + g + 8 * (e >> 1)] = acc[i][j][e];
       cluster_sync_all();  // all 8 partial tiles of the slab are in shared memory
 #pragma unroll
       for (int cnt = 0; cnt < 16; ++cnt) {
@@ -227,19 +229,16 @@ cheb_filter_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_cons
         if (j < p.b) yout[(size_t)(row_base + r) * p.b + j] = ca * sum + cb * vc[cnt] + cg * vp[cnt];
       }
     } else {
-      const int row = warp_idx * 32 + lane;
-      float* out = p.partial + (((size_t)slab * CF_KS + q) * 128 + row) * (size_t)bn;
-      for (int c0 = 0; c0 < bn; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(warp_idx * 32) << 16) + (uint32_t)c0, v);
-        tmem_ld_wait();
-        float4* o4 = reinterpret_cast<float4*>(out + c0);
+      float* out = p.partial + ((size_t)slab * CF_KS + q) * 128 * (size_t)bn;
 #pragma unroll
-        for (int i = 0; i < 8; ++i)
-          o4[i] = make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]), __uint_as_float(v[4 * i + 2]),
-                              __uint_as_float(v[4 * i + 3]));
-      }
-      tcgen05_fence_before();
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float* orow = out + (size_t)(32 * warp_idx + 16 * i + g + 8 * h) * bn + 2 * t;
+#pragma unroll
+          for (int j = 0; j < 4 * NB; ++j)
+            *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(acc[i][j][2 * h], acc[i][j][2 * h + 1]);
+        }
       __threadfence();
       __syncthreads();
       if (tid == 0) cf_grid_barrier(p.counter, (unsigned)gridDim.x * (unsigned)(2 * s - 1));
@@ -263,12 +262,7 @@ cheb_filter_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_cons
     __syncthreads();
   }
 
-  tcgen05_fence_before();
-  cluster_sync_all();
-  if (warp_idx == 0) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols)
-                 : "memory");
-  }
+  if (p.dsmem) cluster_sync_all();  // the peers may still be reading this CTA's partial tile
 }
 
 inline size_t cheb_filter_workspace_bytes(int n, int b) {
@@ -310,9 +304,6 @@ inline int cheb_filter_f32(const float* G, int n, int b, float* const bufs[3], i
   for (int i = 0; i < 3; ++i) p.buf[i] = bufs[i];
   p.counter = static_cast<unsigned*>(ws);
   p.partial = reinterpret_cast<float*>(static_cast<char*>(ws) + 256);
-  int cols = 32;
-  while (cols < p.nbox * 32) cols <<= 1;
-  p.tmem_cols = cols;
   CUtensorMap tg, ty[3];
   TNB_TRY(encode_rowmajor_f32(&tg, G, n, n));
   for (int i = 0; i < 3; ++i) TNB_TRY(encode_rowmajor_f32(&ty[i], bufs[i], n, b));
@@ -340,14 +331,17 @@ inline int cheb_filter_f32(const float* G, int n, int b, float* const bufs[3], i
   attrs[1].val.clusterDim.y = 1;
   attrs[1].val.clusterDim.z = 1;
   cfg.attrs = attrs;
+  void (*const kernels[4])(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, ChebFilterParams) = {
+      cheb_filter_kernel<1>, cheb_filter_kernel<2>, cheb_filter_kernel<3>, cheb_filter_kernel<4>};
+  const auto kernel = kernels[p.nbox - 1];
   if (max_clusters < 0) {
-    TNB_CUDA(cudaFuncSetAttribute(cheb_filter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    for (auto k : kernels) TNB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     TNB_CUDA(cudaEventCreateWithFlags(&last, cudaEventDisableTiming));
     cudaLaunchConfig_t probe = cfg;
     probe.dynamicSmemBytes = 227 * 1024 - 2048;
     probe.numAttrs = 2;
     int nc = 0;
-    if (cudaOccupancyMaxActiveClusters(&nc, cheb_filter_kernel, &probe) != cudaSuccess) nc = 0;
+    if (cudaOccupancyMaxActiveClusters(&nc, kernels[3], &probe) != cudaSuccess) nc = 0;
     cudaGetLastError();
     max_clusters = nc;
   }
@@ -357,7 +351,7 @@ inline int cheb_filter_f32(const float* G, int n, int b, float* const bufs[3], i
   // two resident filter kernels that each hold part of the SMs would wait on each other for ever:
   // chain them across streams
   TNB_CUDA(cudaStreamWaitEvent(st, last, 0));
-  cudaError_t e = cudaLaunchKernelEx(&cfg, cheb_filter_kernel, tg, ty[0], ty[1], ty[2], p);
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kernel, tg, ty[0], ty[1], ty[2], p);
   if (e != cudaSuccess) {
     cudaGetLastError();
     fail(TNB_ERR_UNSUPPORTED, "resident filter launch refused: %s (n=%d b=%d smem=%zu dsmem=%d, max active clusters %d)",

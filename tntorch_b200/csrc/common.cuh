@@ -1,4 +1,4 @@
-// tnb200 — shared helpers for the CUDA translation unit (sm_100a only).
+// tnb200 — shared helpers for the CUDA translation unit (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -149,7 +149,7 @@ inline std::atomic<int>& reserved_sms_ref() {
   return r;
 }
 inline int usable_sms() {
-  const int sms = device_info().valid ? device_info().sm_count : 148;
+  const int sms = device_info().valid ? device_info().sm_count : 132;
   int r = reserved_sms_ref().load(std::memory_order_relaxed);
   if (r < 0) r = 0;
   if (r > sms - 8) r = sms - 8;

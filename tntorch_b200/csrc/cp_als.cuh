@@ -30,8 +30,8 @@ __global__ void khatri_reduce_kernel(const T* __restrict__ Y, const T* __restric
     double acc = 0.0;
     int i = 0;
     if (sizeof(T) == 4) {
-      // fp32 data: eight products per fp32 partial (eight independent loads in flight), partials summed in fp64 — the
-      // fp64 pipe (16 lanes/clk/SM on B200) would otherwise cap this kernel below HBM speed
+      // fp32 data: eight products per fp32 partial (eight independent loads in flight), partials summed in fp64 — one
+      // fp64 addition per eight products instead of one fp64 FMA per product
       for (; i + 8 <= I; i += 8) {
         float part = 0.f;
 #pragma unroll
@@ -45,7 +45,7 @@ __global__ void khatri_reduce_kernel(const T* __restrict__ Y, const T* __restric
 }
 
 // The same reduction for fp32 data with an even R: two adjacent r per thread (8-byte loads), eight rows in flight.  The
-// scalar kernel keeps 1280 threads x 8 x 4 B = 40 KB in flight per SM and stops at 2.7 TB/s (profiles/r02_khatri_ncu_before.md).
+// scalar kernel keeps only 1280 threads x 8 x 4 B = 40 KB in flight per SM, too little to cover HBM latency.
 __global__ void __launch_bounds__(256) khatri_reduce2_kernel(const float* __restrict__ Y, const float* __restrict__ A,
                                                              float* __restrict__ out, int64_t L, int I, int64_t Q, int R) {
   const int R2 = R >> 1;
@@ -218,7 +218,7 @@ inline int cp_mttkrp(const T* X, const CpDims& d, int n, int R, T* const* A, T* 
   if (n != N - 1) {
     // contract the last mode:  cur[(i_0..i_{N-2}), r] = sum_i X[.., i] A_{N-1}[i, r]
     const int64_t rows = d.numel / d.shape[N - 1];
-    TNB_TRY(project_any<T>(X, rows, d.shape[N - 1], A[N - 1], R, cur, st, tc_ws, tc_ws_bytes));  // 3xTF32 on tcgen05 when it fits
+    TNB_TRY(project_any<T>(X, rows, d.shape[N - 1], A[N - 1], R, cur, st, tc_ws, tc_ws_bytes));  // 3xTF32 on the tensor cores when it fits
     lo = 0;
     hi = N - 2;
   } else {
@@ -293,7 +293,7 @@ struct CpTree {
 template <typename T>
 inline void cp_khatri(const T* Y, const T* A, T* out, int64_t L, int64_t I, int64_t Q, int R, cudaStream_t st) {
   const bool al8 = ((reinterpret_cast<uintptr_t>(Y) | reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(out)) & 7u) == 0;
-  if (std::is_same<T, float>::value && (R & 1) == 0 && al8 && L * Q * (R / 2) < 148 * 256) {
+  if (std::is_same<T, float>::value && (R & 1) == 0 && al8 && L * Q * (R / 2) < (int64_t)usable_sms() * 256) {
     const int64_t threads = L * Q * (R / 2) * 8;
     khatri_reduce2_split_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(
         reinterpret_cast<const float*>(Y), reinterpret_cast<const float*>(A), reinterpret_cast<float*>(out), L, (int)I, Q, R);

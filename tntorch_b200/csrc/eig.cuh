@@ -38,7 +38,7 @@ struct ChfsiWork {
   TB* Tm;                   // b x b
   void* partial;            // split-K scratch, partial_bytes
   size_t partial_bytes;
-  bool use_tc = false;      // filter products on the tcgen05 kernel (fp32 blocks only)
+  bool use_tc = false;      // filter products on the tensor-core kernel (fp32 blocks only)
   bool narrow = false;      // products on one CTA per output tile with a direct epilogue (opt-in, TNB_NARROW; measured slower)
   bool shared_gpu = false;  // TNB_FLAG_CONCURRENT: other decompositions run beside this one: no resident 128-SM filter kernel
   double *S, *lam, *Q, *d;  // b*b, b, b*b, b
@@ -75,7 +75,7 @@ inline void chfsi_carve(ArenaT& ar, int n, int b, ChfsiWork<TB>& w) {
 }
 
 // Y <- a * G*Yin + bc * Yin + g * Xin      (G symmetric, stored n x n in TB)
-// tensorcore = true routes the product through the tcgen05 kernel (TF32 operands): used for the Chebyshev
+// tensorcore = true routes the product through the tensor-core kernel (TF32 operands): used for the Chebyshev
 // FILTER only, where operator accuracy merely affects the convergence rate; the Rayleigh-Ritz product stays
 // fp32 FFMA so that the projected matrix, and with it the captured energy, is exact to fp32.
 template <typename TB>

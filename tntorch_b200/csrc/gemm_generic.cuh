@@ -181,7 +181,7 @@ inline GemmPlan plan_gemm(int64_t M, int64_t N, int64_t K, bool symmetric, int f
   const int64_t tm = ceil_div<int64_t>(M, GEMM_BM), tn = ceil_div<int64_t>(N, GEMM_BN);
   int64_t tiles = symmetric ? tm * (tn + 1) / 2 : tm * tn;
   if (tiles < 1) tiles = 1;
-  int sms = device_info().valid ? device_info().sm_count : 148;
+  int sms = device_info().valid ? device_info().sm_count : 132;
   int64_t want = ceil_div<int64_t>(2 * (int64_t)sms * 2, tiles);  // 2 CTAs/SM resident, 2 waves
   int64_t max_by_k = K / 64 > 0 ? K / 64 : 1;
   int64_t s = want < max_by_k ? want : max_by_k;
@@ -258,7 +258,7 @@ inline GemmPlan plan_batched(int64_t M, int64_t N, int64_t nbatch, bool symmetri
   GemmPlan pl;
   const int64_t tm = ceil_div<int64_t>(M, GEMM_BM), tn = ceil_div<int64_t>(N, GEMM_BN);
   int64_t tiles = symmetric ? tm * (tn + 1) / 2 : tm * tn;
-  int sms = device_info().valid ? device_info().sm_count : 148;
+  int sms = device_info().valid ? device_info().sm_count : 132;
   int64_t s = ceil_div<int64_t>(4 * (int64_t)sms, tiles);
   if (s > nbatch) s = nbatch;
   if (s > 256) s = 256;

@@ -1,17 +1,19 @@
-// Gram matrix G = C^T C of a tall row-major fp32 matrix C (rows x n) on the Blackwell tensor cores.
+// Gram matrix G = C^T C of a tall row-major fp32 matrix C (rows x n) on the Hopper tensor cores.
 //
-//   * row slabs of C are staged HBM -> shared memory by TMA (cp.async.bulk.tensor.2d, 128-byte swizzle with 32-byte atoms,
+//   * row slabs of C are staged HBM -> shared memory by TMA (cp.async.bulk.tensor.2d, 128-byte swizzle,
 //     out-of-bounds rows/columns zero-filled by the TMA unit), 4-stage mbarrier ring;
-//   * the contraction runs over the ROW index of C, so both MMA operands are "MN-major" views of the
-//     very same slab: tcgen05.mma.cta_group::1.kind::tf32, M = 128, N = TN <= 256, K = 8 per instruction,
-//     fp32 accumulation in TMEM;
+//   * the contraction runs over the ROW index of C, so both operands are "MN-major" views of the very same
+//     slab.  tf32 wgmma only takes K-major shared-memory operands, so the products run on the warp-level
+//     tensor-core MMA (mma.sync m16n8k8 .tf32, fp32 accumulation in registers) with the fragments read
+//     straight out of the swizzled slab (mma_frag_* below: conflict-free, no transpose pass);
 //   * G is symmetric: only tiles that touch the upper triangle are computed, and on diagonal tiles the
 //     A operand is a sub-block of the B slab (loaded once);
-//   * split-K over row ranges across CTAs; partial tiles are drained TMEM -> registers (tcgen05.ld)
-//     -> global and summed in fp64 by a deterministic second kernel (no atomics).
+//   * split-K over row ranges across CTAs; partial tiles go registers -> global and are summed in fp64 by a
+//     deterministic second kernel (no atomics).
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer,
-// warps 2..5 = epilogue (TMEM lane group = warp_idx % 4).
+// 256 threads = eight MMA warps, a 2 x 4 grid of 64 x tn/4 warp tiles over the 128 x tn output tile; thread 0 also
+// issues the TMA loads, TC_STAGES - 1 stages ahead.  (A separate producer warp would make it 288 threads, which the
+// register allocator rounds up to 384: 168 registers per thread, too few for the 128 accumulators of a 64 x 64 tile.)
 //
 // Replaces, for large fp32 unfoldings, the QR of tensor.py:1816 / the Gram of round.py:104-110.
 #pragma once
@@ -28,8 +30,13 @@ constexpr int TC_BOX_BYTES = TC_KC * 128;       // one TMA box: 32 fp32 columns 
 constexpr int TC_STAGES = 4;
 constexpr int TC_MAX_BOXES = 12;                // 4 (A) + 8 (B)
 constexpr int TC_STAGE_BYTES = TC_MAX_BOXES * TC_BOX_BYTES;
-constexpr int TC_THREADS = 192;
+constexpr int TC_MMA_WARPS = 8;
+constexpr int TC_THREADS = 32 * TC_MMA_WARPS;
 constexpr int TC_SMEM_BYTES = TC_STAGES * TC_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+// Longest run of rows one CTA accumulates in fp32 registers (512 stages = 16384 rows).  The diagonal of a Gram grows with
+// the row count while the rounding error of an fp32 sum grows faster; 16384-row partial sums keep that error well below
+// the TF32 operand noise the accept rule of the sweep budgets for.
+constexpr int64_t TC_MAX_SPLIT_ITERS = 512;
 
 struct GramTcParams {
   int64_t rows;    // contraction length K (rows of both operands)
@@ -44,15 +51,10 @@ struct GramTcParams {
   int64_t iters_total;      // ceil(rows / KC)
   int64_t iters_per_split;
   float* partial;  // [ksplit][num_tiles][128][tn]
-  int tmem_cols;
-  // shared-memory operand descriptor fields (see make_mn_major_desc)
-  uint32_t desc_layout;  // 1 = SWIZZLE_128B_BASE32B (the only MN-major layout tf32 operands accept)
-  uint32_t desc_lbo;     // bytes between 32-column groups (one TMA box)
-  uint32_t desc_sbo;     // bytes between K atoms (4 rows x 128 B)
   int fold;              // > 1: the matrix was viewed as (rows/fold) x (fold*n_orig); G = sum of the diagonal blocks
   int n_orig;
   // direct epilogue (general A^T B with ksplit == 1): C = alpha * acc + beta * D + gamma * E written by the
-  // epilogue warps, no partial tiles and no finalize kernel.  One CTA per output tile: the narrow form used
+  // MMA warps, no partial tiles and no finalize kernel.  One CTA per output tile: the narrow form used
   // when several decompositions share the GPU (few SMs busy per product instead of all of them).
   int direct;
   float* C;
@@ -73,6 +75,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -84,7 +89,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a wrong descriptor or byte count must surface as an error, never as a hung GPU.
+// Bounded wait: a wrong box or byte count must surface as an error, never as a hung GPU.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;  // fast path: no clock read when the phase has already completed
   const long long t0 = clock64();
@@ -102,79 +107,142 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
       : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tcgen05_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tcgen05_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void tcgen05_mma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                 uint32_t accumulate) {
+// D += A * B, m16n8k8, tf32 operands as raw fp32 bits (the tensor core ignores the low 13 mantissa bits: truncation).
+__device__ __forceinline__ void mma_tf32(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
+                                         uint32_t b1) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// Shared-memory matrix descriptor of an MN-major fp32/tf32 operand (cute::UMMA::SmemDescriptor bit layout):
-//   bits [0,14)  start address >> 4
-//   bits [16,30) leading byte offset >> 4  = stride between 32-column (128-byte) groups along M/N
-//   bits [32,46) stride byte offset >> 4   = stride between K atoms (4 rows of 128 B = 512 B)
-//   bits [46,48) version = 1 (Blackwell)     bits [61,64) layout type
-// tf32 MN-major operands only accept the "128-byte swizzle with 32-byte atoms" layout
-// (UMMA::LayoutType::SWIZZLE_128B_BASE32B = 1; Swizzle<2,5,2>: the 32-byte chunk index is XORed with
-// row % 4), which is what the TMA writes with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B.
-__device__ __forceinline__ uint64_t make_mn_major_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                       uint32_t layout_type) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)(layout_type & 7u) << 61;
-  return d;
+// Fragments from an MN-major region written by TMA with CU_TENSOR_MAP_SWIZZLE_128B: boxes of 32 fp32 columns x
+// TC_KC rows, box j (columns 32j..32j+31) at base + j*TC_BOX_BYTES; element (row k, column c) of a box sits at
+// k*128 + (((c/4) ^ (k%8)) * 16) + (c%4)*4.  The k index of an 8-row step is permuted (fragment k = t -> row 2t,
+// k = t+4 -> row 2t+1) identically for both operands, which leaves the product unchanged and makes every fragment
+// load hit 32 distinct banks.
+__device__ __forceinline__ uint32_t mn_ld(const unsigned char* base, int k, int c) {
+  return *reinterpret_cast<const uint32_t*>(base + (c >> 5) * TC_BOX_BYTES + k * 128 + ((((c & 31) >> 2) ^ (k & 7)) << 4) +
+                                            ((c & 3) << 2));
 }
-// Instruction descriptor (cute::UMMA::InstrDescriptor): fp32 accumulate, tf32 x tf32, both operands MN-major.
-__host__ __device__ inline uint32_t make_idesc_tf32_mn(int M, int N) {
-  uint32_t d = 0;
-  d |= 1u << 4;                    // c_format = F32
-  d |= 2u << 7;                    // a_format = TF32
-  d |= 2u << 10;                   // b_format = TF32
-  d |= 1u << 15;                   // a_major = MN
-  d |= 1u << 16;                   // b_major = MN
-  d |= (uint32_t)(N >> 3) << 17;   // n_dim
-  d |= (uint32_t)(M >> 4) << 24;   // m_dim
-  return d;
+// A fragment of the 16 x 8 block (columns c0..c0+15 as rows of A^T, rows k0..k0+7); g = lane/4, t = lane%4.
+__device__ __forceinline__ void mma_frag_a_mn(const unsigned char* base, int k0, int c0, int g, int t, uint32_t (&a)[4]) {
+  a[0] = mn_ld(base, k0 + 2 * t, c0 + g);
+  a[1] = mn_ld(base, k0 + 2 * t, c0 + g + 8);
+  a[2] = mn_ld(base, k0 + 2 * t + 1, c0 + g);
+  a[3] = mn_ld(base, k0 + 2 * t + 1, c0 + g + 8);
+}
+__device__ __forceinline__ void mma_frag_b_mn(const unsigned char* base, int k0, int c0, int g, int t, uint32_t (&b)[2]) {
+  b[0] = mn_ld(base, k0 + 2 * t, c0 + g);
+  b[1] = mn_ld(base, k0 + 2 * t + 1, c0 + g);
 }
 
 // ---------------------------------------------------------------------------------------------
 // The kernel
 // ---------------------------------------------------------------------------------------------
+// NT = tn / 32: n8 tiles per warp (each warp covers tn / 4 columns)
+// Loads of pipeline iteration `it` (rows it_begin + it) into its ring slot, once the MMA warps have released it.
+__device__ __forceinline__ void gram_tc_produce(const CUtensorMap* tmap, const CUtensorMap* tmap_b, unsigned char* stage_base,
+                                                uint64_t* full_bar, uint64_t* empty_bar, int64_t it, int64_t it_begin,
+                                                int nbox_a, int nbox_b, int a_col0, int b_col0) {
+  const int stage = (int)(it % TC_STAGES);
+  const uint32_t phase = (uint32_t)(it / TC_STAGES) & 1u;
+  mbar_wait(&empty_bar[stage], phase ^ 1u);
+  unsigned char* sb = stage_base + stage * TC_STAGE_BYTES;
+  mbar_expect_tx(&full_bar[stage], (uint32_t)(nbox_a + nbox_b) * TC_BOX_BYTES);
+  const int row0 = (int)((it_begin + it) * TC_KC);
+  // B boxes first (slots 0..nbox_b), then A boxes (slots 8..11)
+  for (int j = 0; j < nbox_b; ++j) tma_load_2d(sb + j * TC_BOX_BYTES, tmap_b, &full_bar[stage], b_col0 + 32 * j, row0);
+  for (int j = 0; j < nbox_a; ++j) tma_load_2d(sb + (8 + j) * TC_BOX_BYTES, tmap, &full_bar[stage], a_col0 + 32 * j, row0);
+}
+
+template <int NT>
+__device__ __forceinline__ void gram_tc_consume(const CUtensorMap* tmap, const CUtensorMap* tmap_b, const GramTcParams& p,
+                                                unsigned char* stage_base, uint64_t* full_bar, uint64_t* empty_bar,
+                                                int64_t it_begin, int64_t iters, int nbox_a, int a_box, int tile_id,
+                                                int split, int a_col0, int b_col0) {
+  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane >> 2, t = lane & 3;
+  const int wm = w >> 2, wn = w & 3;      // 64-row half of the tile, quarter of its columns
+  const int cm = wm * 64, cn = wn * NT * 8;
+  float acc[4][NT][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < NT; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) acc[i][j][e] = 0.f;
+
+  if (threadIdx.x == 0)
+    for (int64_t it = 0; it < TC_STAGES - 1 && it < iters; ++it)
+      gram_tc_produce(tmap, tmap_b, stage_base, full_bar, empty_bar, it, it_begin, nbox_a, NT, a_col0, b_col0);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int64_t it = 0; it < iters; ++it) {
+    if (threadIdx.x == 0 && it + TC_STAGES - 1 < iters)  // refill the slot iteration it - 1 used
+      gram_tc_produce(tmap, tmap_b, stage_base, full_bar, empty_bar, it + TC_STAGES - 1, it_begin, nbox_a, NT, a_col0,
+                      b_col0);
+    __syncwarp();
+    mbar_wait(&full_bar[stage], phase);
+    const unsigned char* sb = stage_base + stage * TC_STAGE_BYTES;
+    const unsigned char* sa = sb + a_box * TC_BOX_BYTES;
+#pragma unroll
+    for (int ks = 0; ks < TC_KC; ks += 8) {
+      uint32_t bf[NT][2];
+#pragma unroll
+      for (int j = 0; j < NT; ++j) mma_frag_b_mn(sb, ks, cn + 8 * j, g, t, bf[j]);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        uint32_t af[4];
+        mma_frag_a_mn(sa, ks, cm + 16 * i, g, t, af);
+#pragma unroll
+        for (int j = 0; j < NT; ++j) mma_tf32(acc[i][j], af[0], af[1], af[2], af[3], bf[j][0], bf[j][1]);
+      }
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);  // this warp is done reading the slot
+    if (++stage == TC_STAGES) { stage = 0; phase ^= 1u; }
+  }
+
+  // epilogue: accumulator element (row r, column c) of the 128 x tn tile; c0/c1 and c2/c3 are column pairs
+  if (p.direct) {
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int gi = a_col0 + cm + 16 * i + g + 8 * h;
+#pragma unroll
+        for (int j = 0; j < NT; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int gj = b_col0 + cn + 8 * j + 2 * t + e;
+            if (gi < p.m && gj < p.n) {
+              float x = p.alpha * acc[i][j][2 * h + e];
+              if (p.D) x += p.beta * p.D[(size_t)gi * p.ldd + gj];
+              if (p.E) x += p.gamma * p.E[(size_t)gi * p.lde + gj];
+              p.C[(size_t)gi * p.ldc + gj] = x;
+            }
+          }
+      }
+    return;
+  }
+  float* out = p.partial + ((size_t)split * p.num_tiles + tile_id) * 128 * (size_t)p.tn;
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float* orow = out + (size_t)(cm + 16 * i + g + 8 * h) * p.tn + cn + 2 * t;
+#pragma unroll
+      for (int j = 0; j < NT; ++j)
+        *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(acc[i][j][2 * h], acc[i][j][2 * h + 1]);
+    }
+}
+
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_b,
                const GramTcParams p) {
@@ -185,12 +253,8 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
   unsigned char* stage_base = tc_smem_raw + pad;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(stage_base + TC_STAGES * TC_STAGE_BYTES);
   uint64_t* empty_bar = full_bar + TC_STAGES;
-  uint64_t* tmem_full_bar = empty_bar + TC_STAGES;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-  int* tile_smem = reinterpret_cast<int*>(tmem_ptr_smem + 1);  // bm, bn
+  int* tile_smem = reinterpret_cast<int*>(empty_bar + TC_STAGES);  // bm, bn
 
-  const int warp_idx = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
   const int tile_id = blockIdx.x, split = blockIdx.y;
 
   if (threadIdx.x == 0) {
@@ -211,130 +275,37 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
     tile_smem[1] = fbn;
     for (int s = 0; s < TC_STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], TC_MMA_WARPS);
     }
-    mbar_init(tmem_full_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp_idx == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)),
-                 "r"((uint32_t)p.tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
 
-  const uint32_t tmem_base = *tmem_ptr_smem;
   const int bm = tile_smem[0], bn = tile_smem[1];
   const int a_col0 = bm * 128, b_col0 = bn * p.tn;
   const int nbox_b = p.tn / 32;
   const bool a_in_b = p.symmetric && (a_col0 >= b_col0) && (a_col0 + 128 <= b_col0 + p.tn);
   const int nbox_a = a_in_b ? 0 : 4;
+  const int a_box = a_in_b ? (a_col0 - b_col0) / 32 : 8;  // first box of the A operand in a stage
   const int64_t it_begin = (int64_t)split * p.iters_per_split;
   int64_t it_end = it_begin + p.iters_per_split;
   if (it_end > p.iters_total) it_end = p.iters_total;
   const int64_t iters = it_end > it_begin ? it_end - it_begin : 0;
 
-  if (warp_idx == 0) {
-    // ================= TMA producer =================
-    if (lane == 0 && iters > 0) {
-      const uint32_t tx_bytes = (uint32_t)(nbox_a + nbox_b) * TC_BOX_BYTES;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int64_t it = 0; it < iters; ++it) {
-        mbar_wait(&empty_bar[stage], phase ^ 1u);
-        unsigned char* sb = stage_base + stage * TC_STAGE_BYTES;
-        mbar_expect_tx(&full_bar[stage], tx_bytes);
-        const int row0 = (int)((it_begin + it) * TC_KC);
-        // B boxes first (slots 0..nbox_b), then A boxes (slots 8..11)
-        for (int j = 0; j < nbox_b; ++j) tma_load_2d(sb + j * TC_BOX_BYTES, &tmap_b, &full_bar[stage], b_col0 + 32 * j, row0);
-        for (int j = 0; j < nbox_a; ++j)
-          tma_load_2d(sb + (8 + j) * TC_BOX_BYTES, &tmap, &full_bar[stage], a_col0 + 32 * j, row0);
-        if (++stage == TC_STAGES) { stage = 0; phase ^= 1u; }
-      }
-    }
-  } else if (warp_idx == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0 && iters > 0) {
-      const uint32_t idesc = make_idesc_tf32_mn(128, p.tn);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int64_t it = 0; it < iters; ++it) {
-        mbar_wait(&full_bar[stage], phase);
-        tcgen05_fence_after();
-        const uint32_t sb = smem_u32(stage_base + stage * TC_STAGE_BYTES);
-        const uint32_t b_addr = sb;
-        const uint32_t a_addr = a_in_b ? sb + (uint32_t)((a_col0 - b_col0) / 32) * TC_BOX_BYTES : sb + 8u * TC_BOX_BYTES;
-#pragma unroll
-        for (int ks = 0; ks < TC_KC / 8; ++ks) {
-          const uint64_t adesc = make_mn_major_desc(a_addr + ks * 1024u, p.desc_lbo, p.desc_sbo, p.desc_layout);
-          const uint64_t bdesc = make_mn_major_desc(b_addr + ks * 1024u, p.desc_lbo, p.desc_sbo, p.desc_layout);
-          tcgen05_mma_tf32(tmem_base, adesc, bdesc, idesc, (it > 0 || ks > 0) ? 1u : 0u);
-        }
-        tcgen05_commit(&empty_bar[stage]);  // smem slot reusable once these MMAs have read it
-        if (++stage == TC_STAGES) { stage = 0; phase ^= 1u; }
-      }
-      tcgen05_commit(tmem_full_bar);  // accumulator complete
-    }
-  } else {
-    // ================= epilogue: TMEM -> registers -> global partial tile =================
-    const int lane_group = warp_idx & 3;          // TMEM lanes [32*lane_group, +32)
-    const int row = lane_group * 32 + lane;       // accumulator row = column (a_col0 + row) of C
-    float* out = p.partial + (((size_t)split * p.num_tiles + tile_id) * 128 + row) * (size_t)p.tn;
-    if (p.direct) {
-      const int gi = a_col0 + row;  // output row
-      if (iters > 0) {
-        mbar_wait(tmem_full_bar, 0);
-        tcgen05_fence_after();
-      }
-      for (int c0 = 0; c0 < p.tn; c0 += 32) {
-        uint32_t v[32];
-        if (iters > 0) {
-          tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(lane_group * 32) << 16) + (uint32_t)c0, v);
-          tmem_ld_wait();
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = 0u;
-        }
-        if (gi < p.m) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const int gj = b_col0 + c0 + i;
-            if (gj < p.n) {
-              float x = p.alpha * __uint_as_float(v[i]);
-              if (p.D) x += p.beta * p.D[(size_t)gi * p.ldd + gj];
-              if (p.E) x += p.gamma * p.E[(size_t)gi * p.lde + gj];
-              p.C[(size_t)gi * p.ldc + gj] = x;
-            }
-          }
-        }
-      }
-    } else if (iters > 0) {
-      mbar_wait(tmem_full_bar, 0);
-      tcgen05_fence_after();
-      for (int c0 = 0; c0 < p.tn; c0 += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(lane_group * 32) << 16) + (uint32_t)c0, v);
-        tmem_ld_wait();
-        float4* o4 = reinterpret_cast<float4*>(out + c0);
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          o4[q] = make_float4(__uint_as_float(v[4 * q]), __uint_as_float(v[4 * q + 1]), __uint_as_float(v[4 * q + 2]),
-                              __uint_as_float(v[4 * q + 3]));
-      }
-    } else {
-      for (int c0 = 0; c0 < p.tn; c0 += 4) *reinterpret_cast<float4*>(out + c0) = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
+#define TNB_GRAM_CONSUME(NT)                                                                                    \
+  gram_tc_consume<NT>(&tmap, &tmap_b, p, stage_base, full_bar, empty_bar, it_begin, iters, nbox_a, a_box, tile_id, split, \
+                      a_col0, b_col0)
+  switch (nbox_b) {
+    case 1: TNB_GRAM_CONSUME(1); break;
+    case 2: TNB_GRAM_CONSUME(2); break;
+    case 3: TNB_GRAM_CONSUME(3); break;
+    case 4: TNB_GRAM_CONSUME(4); break;
+    case 5: TNB_GRAM_CONSUME(5); break;
+    case 6: TNB_GRAM_CONSUME(6); break;
+    case 7: TNB_GRAM_CONSUME(7); break;
+    default: TNB_GRAM_CONSUME(8); break;
   }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)p.tmem_cols)
-                 : "memory");
-  }
+#undef TNB_GRAM_CONSUME
 }
 
 // Sum the split-K partial tiles in fp64 (fixed order), mirror to the lower triangle.
@@ -404,7 +375,7 @@ inline PFN_encodeTiled get_encode_tiled() {
 
 inline bool tc_path_available() {
   const DeviceInfo& di = device_info();
-  return di.valid && di.cc_major == 10 && get_encode_tiled() != nullptr;
+  return di.valid && di.cc_major == 9 && get_encode_tiled() != nullptr;
 }
 
 inline bool gram_tc_shape_ok(int64_t rows, int64_t n) {
@@ -430,20 +401,23 @@ inline void gram_tc_plan(int64_t rows, int64_t n, GramTcParams& p, int64_t m_col
   }
   p.num_tiles = cnt;
   p.iters_total = (rows + TC_KC - 1) / TC_KC;
-  int sms = usable_sms();
-  int64_t ks = sms / cnt;
-  if (ks < 1) ks = 1;
+  // split-K factor: at least sms / cnt and enough splits that no fp32 accumulation chain is longer than
+  // TC_MAX_SPLIT_ITERS stages (the splits are summed in fp64), then up to 8x that if it fills the last wave of CTAs better
+  // while every split keeps >= 64 stages (72 tiles of 262144 rows on 128 SMs: 16 splits, 9 full waves)
+  const int sms = usable_sms();
+  const int64_t base = std::max<int64_t>(cnt < sms ? sms / cnt : 1, (p.iters_total + TC_MAX_SPLIT_ITERS - 1) / TC_MAX_SPLIT_ITERS);
+  int64_t ks = base;
+  double best = 0.0;
+  for (int64_t k = base; k <= 8 * base && k <= p.iters_total && (k == base || 64 * k <= p.iters_total); ++k) {
+    const int64_t ctas = k * cnt, waves = (ctas + sms - 1) / sms;
+    const double eff = (double)ctas / (double)(waves * sms);
+    if (eff > best + 0.02) { best = eff; ks = k; }
+  }
   if (ks > p.iters_total) ks = p.iters_total;
   p.iters_per_split = (p.iters_total + ks - 1) / ks;
   ks = (p.iters_total + p.iters_per_split - 1) / p.iters_per_split;
   p.ksplit = (int)ks;
-  int cols = 32;
-  while (cols < tn) cols <<= 1;
-  p.tmem_cols = cols;
   p.partial = nullptr;
-  p.desc_layout = 1;
-  p.desc_lbo = TC_BOX_BYTES;
-  p.desc_sbo = 512;
   p.fold = 1;
   p.n_orig = (int)n;
   p.direct = 0;
@@ -470,10 +444,22 @@ inline size_t gram_tc_workspace_bytes(int64_t rows, int64_t n) {
   return align_up((size_t)p.ksplit * p.num_tiles * 128 * p.tn * sizeof(float));
 }
 
+inline int encode_rowmajor_f32(CUtensorMap* tmap, const float* ptr, int64_t rows, int64_t cols, int box_rows = TC_KC) {
+  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t gstride[1] = {(cuuint64_t)cols * sizeof(float)};
+  cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult cr = get_encode_tiled()(tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), gdim, gstride, box,
+                                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (cr != CUDA_SUCCESS) return fail(TNB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)cr);
+  return TNB_OK;
+}
+
 // G (n x n fp64) and optionally Gf (fp32 copy) = A^T A, A: rows x n fp32 row-major (device).
 inline int gram_tc_f32(const float* A, int64_t rows, int64_t n, double* G, float* Gf, void* ws, size_t ws_bytes,
                        cudaStream_t st) {
-  if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "gram_tc: tcgen05/TMA path needs an sm_100 device");
+  if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "gram_tc: TMA tensor-core path needs an sm_90 device");
   if (!gram_tc_shape_ok(rows, n)) return fail(TNB_ERR_UNSUPPORTED, "gram_tc: unsupported shape rows=%lld n=%lld", (long long)rows, (long long)n);
   if ((reinterpret_cast<uintptr_t>(A) & 15u) != 0) return fail(TNB_ERR_INVALID, "gram_tc: input must be 16-byte aligned");
   GramTcParams p;
@@ -488,16 +474,8 @@ inline int gram_tc_f32(const float* A, int64_t rows, int64_t n, double* G, float
   if (ws_bytes < need) return fail(TNB_ERR_WORKSPACE, "gram_tc: workspace %zu < %zu", ws_bytes, need);
   p.partial = static_cast<float*>(ws);
 
-  const CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B;  // matches UMMA SWIZZLE_128B_BASE32B
   CUtensorMap tmap;
-  cuuint64_t gdim[2] = {(cuuint64_t)n, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)n * sizeof(float)};
-  cuuint32_t box[2] = {32, (cuuint32_t)TC_KC};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult cr = get_encode_tiled()(&tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(A), gdim, gstride, box,
-                                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
-                                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) return fail(TNB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)cr);
+  TNB_TRY(encode_rowmajor_f32(&tmap, A, rows, n));
 
   static PerDeviceFlag attr_done;
   TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel, TC_SMEM_BYTES));
@@ -544,22 +522,10 @@ inline size_t atb_tc_workspace_bytes(int64_t K, int64_t m, int64_t n) {
   return align_up((size_t)p.ksplit * p.num_tiles * 128 * p.tn * sizeof(float));
 }
 
-inline int encode_rowmajor_f32(CUtensorMap* tmap, const float* ptr, int64_t rows, int64_t cols, int box_rows = TC_KC) {
-  cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)cols * sizeof(float)};
-  cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult cr = get_encode_tiled()(tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), gdim, gstride, box,
-                                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B,
-                                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) return fail(TNB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)cr);
-  return TNB_OK;
-}
-
 inline int atb_tc_f32(const float* A, int64_t K, int64_t m, const float* B, int64_t n, float* C, int ldc, float alpha,
                       const float* D, int ldd, float beta, const float* E, int lde, float gamma, void* ws,
                       size_t ws_bytes, cudaStream_t st, bool narrow = false) {
-  if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "atb_tc: tcgen05/TMA path needs an sm_100 device");
+  if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "atb_tc: TMA tensor-core path needs an sm_90 device");
   if (!atb_tc_shape_ok(K, m, n)) return fail(TNB_ERR_UNSUPPORTED, "atb_tc: unsupported shape K=%lld m=%lld n=%lld", (long long)K, (long long)m, (long long)n);
   if (((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B)) & 15u) != 0)
     return fail(TNB_ERR_INVALID, "atb_tc: operands must be 16-byte aligned");

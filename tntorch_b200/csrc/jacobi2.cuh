@@ -108,6 +108,9 @@ __device__ inline int jac2_solve(const Jac2<R>& Jin, int max_sweeps, int* sweeps
       { R* t = cr; cr = cw; cw = t; }
     }
     conv = (*fl == 0);
+    // the flags alternate: thread 0 clears this one again at the top of the next sweep, so every thread must have read
+    // it first (a late warp would otherwise see the cleared flag and leave the loop alone)
+    __syncthreads();
   }
   __syncthreads();
   if (sweeps_out) *sweeps_out = conv ? sweep : -sweep;
@@ -206,8 +209,8 @@ __global__ void __launch_bounds__(1024) jacobi2_eigh_kernel(const double* __rest
   if (tid == 0 && info) info[0] = s_sweeps;
 }
 
-// fp64 results at mostly fp32 cost.  The B200 issues ~16 fp64 FMAs per clock and SM against 128 fp32 ones, and a 64 x 64
-// fp64 Jacobi solve is bound by exactly that (measured 0.88 ms, nine sweeps).  Here the sweeps that do the real work run
+// fp64 results at mostly fp32 cost: fp64 FMAs issue at half the fp32 rate, and a 64 x 64 fp64 Jacobi solve is bound
+// by that rate.  Here the sweeps that do the real work run
 // in fp32; their basis V is promoted, re-orthonormalised in fp64 (one Newton-Schulz step: 1e-7 -> 1e-14), the matrix is
 // taken into that basis in fp64, S2 = V^T G V — now diagonal up to ~1e-6 — and fp64 sweeps finish from there: two of them
 // by quadratic convergence (1e-6 -> 1e-12 -> below the threshold).  Same contract and accuracy as the all-fp64 kernel.

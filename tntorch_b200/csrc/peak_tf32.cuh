@@ -1,72 +1,35 @@
-// Measured dense TF32 tcgen05 peak (SURVEY.md §8d: "the builder must measure a TF32 tcgen05 peak ... before quoting
-// tensor-pipe fractions").  One CTA per SM issues tcgen05.mma.cta_group::1.kind::tf32 M=128, N=256, K=8 back to back on
-// operand tiles that sit in shared memory for the whole run (no TMA, no global traffic: the tensor pipe is the only thing
-// exercised), accumulating into TMEM; `reps` commits of `per_commit` MMAs each.  FLOP = 2*128*256*8 per MMA.
+// Measured dense TF32 peak of the tensor-core instruction the kernels use (SURVEY.md §8d: "the builder must measure a
+// TF32 peak ... before quoting tensor-pipe fractions").  Every warp of two 256-thread CTAs per SM issues
+// mma.sync.m16n8k8 .tf32 back to back on register operands into eight independent accumulators (no shared or global
+// traffic: the tensor pipe is the only thing exercised); `reps` x `per_commit` MMAs per accumulator.
+// FLOP = 2*16*8*8 per MMA.
 #pragma once
 #include "common.cuh"
 #include "gram_tc.cuh"
 
 namespace tnb {
 
-constexpr int PK_THREADS = 128;
-constexpr int PK_SMEM = 4 * TC_BOX_BYTES + 8 * TC_BOX_BYTES + 1024 + 64;  // A: 128 x 32 rows, B: 256 x 32 rows (MN-major boxes)
+constexpr int PK_THREADS = 256;
+constexpr int PK_ACC = 8;
 
 __global__ void __launch_bounds__(PK_THREADS) peak_tf32_kernel(int reps, int per_commit, float* sink) {
-  extern __shared__ unsigned char pk_smem_raw[];
-  const uint32_t raw = smem_u32(pk_smem_raw);
-  const uint32_t pad = (1024u - (raw & 1023u)) & 1023u;
-  unsigned char* a_sm = pk_smem_raw + pad;
-  unsigned char* b_sm = a_sm + 4 * TC_BOX_BYTES;
-  uint64_t* bar = reinterpret_cast<uint64_t*>(b_sm + 8 * TC_BOX_BYTES);
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bar + 1);
-  const int tid = threadIdx.x, warp = tid >> 5;
-  for (int i = tid; i < 12 * TC_BOX_BYTES / 4; i += PK_THREADS) reinterpret_cast<float*>(a_sm)[i] = 1.0f + (float)(i & 7) * 0.125f;
-  if (tid == 0) {
-    mbar_init(bar, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 0) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr)), "r"(256u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("fence.proxy.async;" ::: "memory");
-  tcgen05_fence_before();
-  __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  if (tid == 0) {
-    const uint32_t idesc = make_idesc_tf32_mn(128, 256);
-    const uint32_t aa = smem_u32(a_sm), ba = smem_u32(b_sm);
-    for (int r = 0; r < reps; ++r) {
-      for (int m = 0; m < per_commit; ++m) {
-        const uint32_t ks = (uint32_t)(m & 3);
-        const uint64_t adesc = make_mn_major_desc(aa + ks * 1024u, TC_BOX_BYTES, 512, 1);
-        const uint64_t bdesc = make_mn_major_desc(ba + ks * 1024u, TC_BOX_BYTES, 512, 1);
-        tcgen05_mma_tf32(tmem_base, adesc, bdesc, idesc, (r > 0 || m > 0) ? 1u : 0u);
-      }
-      tcgen05_commit(bar);
-      mbar_wait(bar, (uint32_t)r & 1u);
-    }
-  }
-  __syncthreads();
-  tcgen05_fence_after();
-  if (warp == 0) {
-    uint32_t v[32];
-    tmem_ld_32x32b_x32(tmem_base, v);
-    tmem_ld_wait();
-    if (sink && tid == 0 && blockIdx.x == 0) sink[0] = __uint_as_float(v[0]);
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(256u) : "memory");
+  const uint32_t x = __float_as_uint(1.0f + (float)(threadIdx.x & 7) * 0.125f);
+  const uint32_t y = __float_as_uint(0.5f + (float)(threadIdx.x >> 5) * 0.0625f);
+  float acc[PK_ACC][4] = {};
+  for (int r = 0; r < reps; ++r)
+    for (int m = 0; m < per_commit; ++m)
+#pragma unroll
+      for (int a = 0; a < PK_ACC; ++a) mma_tf32(acc[a], x, y, x, y, x, y);
+  float s = 0.f;
+#pragma unroll
+  for (int a = 0; a < PK_ACC; ++a) s += acc[a][0] + acc[a][1] + acc[a][2] + acc[a][3];
+  if (sink && s == 12345.f) sink[0] = s;  // keeps the products live; never true for these operands
 }
 
-// Returns TFLOP/s of the best of `trials` timed launches (CUDA events on `st`), one CTA per SM.
+// Returns TFLOP/s of the best of `trials` timed launches (CUDA events on `st`).
 inline int measure_tf32_peak(int reps, int per_commit, int trials, double* tflops_out, double* ms_out, cudaStream_t st) {
-  if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "tcgen05 path not available on this device");
-  static PerDeviceFlag attr_done;
-  TNB_CUDA(ensure_dyn_smem(attr_done, peak_tf32_kernel, PK_SMEM));
-  const int sms = device_info().sm_count;
+  if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "tensor-core path not available on this device");
+  const int blocks = 2 * device_info().sm_count;
   float* sink = nullptr;
   TNB_CUDA(cudaMalloc(&sink, 256));
   cudaEvent_t e0, e1;
@@ -75,7 +38,7 @@ inline int measure_tf32_peak(int reps, int per_commit, int trials, double* tflop
   double best = 1e30;
   for (int t = 0; t < trials + 2; ++t) {
     TNB_CUDA(cudaEventRecord(e0, st));
-    peak_tf32_kernel<<<sms, PK_THREADS, PK_SMEM, st>>>(reps, per_commit, sink);
+    peak_tf32_kernel<<<blocks, PK_THREADS, 0, st>>>(reps, per_commit, sink);
     TNB_CUDA(cudaEventRecord(e1, st));
     TNB_CUDA(cudaEventSynchronize(e1));
     TNB_COUNT_LAUNCH();
@@ -88,7 +51,7 @@ inline int measure_tf32_peak(int reps, int per_commit, int trials, double* tflop
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
   cudaFree(sink);
-  const double flop = 2.0 * 128 * 256 * 8 * (double)reps * per_commit * sms;
+  const double flop = 2.0 * 16 * 8 * 8 * PK_ACC * (double)reps * per_commit * (PK_THREADS / 32) * blocks;
   *tflops_out = flop / (best * 1e-3) / 1e12;
   if (ms_out) *ms_out = best;
   return TNB_OK;

@@ -1,44 +1,27 @@
-// Tall-skinny projection C (rows x r) = A (rows x K) * V (K x r) on the tcgen05 tensor cores at fp32 accuracy
+// Tall-skinny projection C (rows x r) = A (rows x K) * V (K x r) on the Hopper tensor cores at fp32 accuracy
 // ("3xTF32": A = A_hi + A_lo, V = V_hi + V_lo, C = A_hi V_hi + A_hi V_lo + A_lo V_hi, error ~2^-21 relative,
 // i.e. the accuracy class of an fp32 FFMA product — a plain TF32 projection would put a 2^-11 relative error
 // straight into the reconstruction).  This is the "C <- C V_r" step of the sweep (round.py:181, tensor.py:2081-2083).
 //
 //   * A row blocks (128 rows x 32 k) are staged by TMA (K-major, SWIZZLE_128B) into a deep mbarrier ring (11 x 16 KB
-//     when V fits in shared memory, else 8 x 24 KB with the V chunk riding in the stage); V_hi^T / V_lo^T are stacked
-//     as ONE B operand of 2*r_pad rows;
-//   * four "split" warps (thread = row, conflict-free reads of the swizzled tile) put BOTH the raw tile and
-//     A_lo = A - trunc(A) into TENSOR MEMORY (tcgen05.st); every MMA then takes its A operand from TMEM (TS form):
-//     A_raw x [V_hi; V_lo] (N = 2*r_pad; the tensor core truncates the raw bits to TF32 itself, so this is
-//     A_hi V_hi | A_hi V_lo side by side) and A_lo x V_hi (N = r_pad) onto the first r_pad accumulator columns.
-//     The tile crosses the shared-memory port twice (TMA fill, split read) instead of six times;
-//   * four epilogue warps drain finished tiles (tcgen05.ld), add the two halves and store, while the next row
-//     block is already being multiplied (persistent CTAs, static round-robin over row blocks).
-//
-// What bounds it (measured, profiles/r01_ncu_summaries.md): a tcgen05.mma of M=128, K=8 occupies the tensor pipe for
-// ~100 (TS) to ~140 (SS) cycles however small N is, and one thread issues all of them, so the MMA-issuing thread
-// paces the CTA: 8 instructions per 16 KB chunk.  With all-TS operands and no integer divisions in that thread's
-// loop a chunk takes ~1050 cycles: A is ingested at ~4.4 TB/s whatever K is (K = 64 .. 2048, V resident or streamed,
-// scripts/gpu_proj_k.py); with the output of the K = 64 step (half the input again) that is 5.8 TB/s = 88 % of the
-// measured copy peak.  Halving the instruction count needs the operands swapped (V stack on the M side, 256 rows of A
-// per instruction on the N side).
+//     when V fits in shared memory, else 8 x 24 KB with the V chunk riding in the stage); V_hi^T / V_lo^T are
+//     prepared once (split_v_kernel) and staged as K-major tiles of npad rows each;
+//   * eight MMA warps, 16 rows of the block each, read their A fragments from the swizzled tile (conflict-free),
+//     split them in registers (A_lo = A - trunc_tf32(A); the tensor core truncates the raw bits of A_hi itself) and
+//     issue the three products per 8-wide k-step with mma.sync m16n8k8 .tf32; every 32-wide chunk is folded into an
+//     fp32 running sum so that the accumulation error does not grow with K;
+//   * persistent CTAs, static round-robin over row blocks; each warp stores its 16 x r piece of C from registers.
 #pragma once
 #include "gram_tc.cuh"
 
 namespace tnb {
 
-constexpr int PT_BM = 128, PT_KC = 32, PT_MAX_STAGES = 12, PT_THREADS = 320;
+constexpr int PT_BM = 128, PT_KC = 32, PT_MAX_STAGES = 12, PT_MMA_WARPS = 8, PT_THREADS = 32 * (1 + PT_MMA_WARPS);
 constexpr int PT_A_BYTES = PT_BM * PT_KC * 4;      // 16 KB
 constexpr int PT_MAX_N = 64;                        // r padded to a multiple of 16, <= 64
 constexpr int PT_RING_BYTES = 192 * 1024;           // stage ring (+ resident V when it fits)
-constexpr int PT_EPI_BYTES = 4 * 32 * 64 * 4;        // per epilogue warp: 32 rows x <= 64 columns, staged for coalesced stores
-constexpr int PT_SMEM_BYTES = PT_RING_BYTES + 1024 + 512 + PT_EPI_BYTES;
+constexpr int PT_SMEM_BYTES = PT_RING_BYTES + 1024 + 256;
 constexpr int PT_VRES_MAX_BYTES = 32 * 1024;        // V_hi|V_lo kept in shared memory for the whole kernel up to this size
-constexpr int PT_ACC_COLS = 256;                    // accumulator slots: 256 / (2*npad) of width 2*npad
-constexpr int PT_ALO_COL = PT_ACC_COLS;             // A_lo ring: PT_ALO_SLOTS x 32 columns behind the accumulators
-constexpr int PT_ALO_SLOTS = 4;  // 4 x (32 raw + 32 lo) columns: with the 256 accumulator columns exactly the 512 of an SM
-constexpr int PT_ALO_W = 2 * PT_KC;
-constexpr int PT_TMEM_COLS = 512;
-constexpr int PT_MAX_SLOTS = 8;
 
 struct ProjTcParams {
   int64_t rows;
@@ -47,64 +30,99 @@ struct ProjTcParams {
   int npad;    // r rounded up to a multiple of 16
   int64_t num_row_blocks;
   int nk;      // K chunks
-  int slab;    // chunks per accumulator slab: the TMEM accumulator truncates on every add, so long K ranges are cut
-               // into slabs of PT_SLAB_CHUNKS*32 columns whose partial tiles are summed in fp32 (RN) by the epilogue
-  int nslabs;
   int vres;         // 1: all V chunks resident in shared memory (small K), stages hold A only
   int stage_bytes;  // 16 KB (+ 2*npad*128 B of V chunk when streaming V)
   int nstages;      // ring depth that fits PT_RING_BYTES: the HBM latency needs >= ~140 KB in flight per SM
-  int alo_slots;    // A_lo ring depth in use (<= PT_ALO_SLOTS)
   float* C;
 };
-constexpr int PT_SLAB_CHUNKS = 8;
 
-// K-major operand, SWIZZLE_128B: 8-row groups 1024 B apart (SBO); LBO unused for swizzled K-major layouts.
-__device__ __forceinline__ uint64_t make_k_major_desc(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;                       // LBO (ignored)
-  d |= (uint64_t)((1024u >> 4) & 0x3FFF) << 32; // SBO
-  d |= (uint64_t)1 << 46;                       // version
-  d |= (uint64_t)2 << 61;                       // SWIZZLE_128B
-  return d;
+// element (row m, column k) of a K-major tile of 32 fp32 columns written by TMA with SWIZZLE_128B
+__device__ __forceinline__ uint32_t km_ld(const unsigned char* base, int m, int k) {
+  return *reinterpret_cast<const uint32_t*>(base + m * 128 + ((((k >> 2) ^ (m & 7))) << 4) + ((k & 3) << 2));
 }
-__host__ __device__ inline uint32_t make_idesc_tf32_kk(int M, int N) {
-  uint32_t d = 0;
-  d |= 1u << 4;                    // c_format = F32
-  d |= 2u << 7;                    // a_format = TF32
-  d |= 2u << 10;                   // b_format = TF32
-  d |= (uint32_t)(N >> 3) << 17;   // n_dim   (a_major = b_major = K-major = 0)
-  d |= (uint32_t)(M >> 4) << 24;   // m_dim
-  return d;
+
+// NT = npad / 8 n8 tiles
+template <int NT>
+__device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const unsigned char* stage_base,
+                                                   const unsigned char* v_res, uint64_t* full_bar, uint64_t* empty_bar,
+                                                   uint64_t* v_bar, int64_t total_items) {
+  const int w = (threadIdx.x >> 5) - 1, lane = threadIdx.x & 31;
+  const int g = lane >> 2, t = lane & 3;
+  const int m0 = 16 * w;
+  const int vchunk_bytes = 2 * p.npad * PT_KC * 4;
+  const int vlo_off = p.npad * PT_KC * 4;
+  if (p.vres && total_items > 0) mbar_wait(v_bar, 0);
+  float out[NT][4];
+#pragma unroll
+  for (int j = 0; j < NT; ++j)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) out[j][e] = 0.f;
+  int stage = 0, kc = 0;
+  uint32_t phase = 0;
+  int64_t row0 = (int64_t)blockIdx.x * PT_BM;
+  for (int64_t item = 0; item < total_items; ++item) {
+    mbar_wait(&full_bar[stage], phase);
+    const unsigned char* sa = stage_base + (size_t)stage * p.stage_bytes;
+    const unsigned char* vh = p.vres ? v_res + (size_t)kc * vchunk_bytes : sa + PT_A_BYTES;
+    const unsigned char* vl = vh + vlo_off;
+    float acc[NT][4];
+#pragma unroll
+    for (int j = 0; j < NT; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) acc[j][e] = 0.f;
+#pragma unroll
+    for (int ks = 0; ks < PT_KC; ks += 8) {
+      uint32_t a[4], lo[4];
+      a[0] = km_ld(sa, m0 + g, ks + t);
+      a[1] = km_ld(sa, m0 + g + 8, ks + t);
+      a[2] = km_ld(sa, m0 + g, ks + t + 4);
+      a[3] = km_ld(sa, m0 + g + 8, ks + t + 4);
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+        lo[i] = __float_as_uint(__uint_as_float(a[i]) - __uint_as_float(a[i] & 0xFFFFE000u));
+#pragma unroll
+      for (int j = 0; j < NT; ++j) {
+        const uint32_t bh0 = km_ld(vh, 8 * j + g, ks + t), bh1 = km_ld(vh, 8 * j + g, ks + t + 4);
+        const uint32_t bl0 = km_ld(vl, 8 * j + g, ks + t), bl1 = km_ld(vl, 8 * j + g, ks + t + 4);
+        mma_tf32(acc[j], a[0], a[1], a[2], a[3], bl0, bl1);      // A_hi V_lo
+        mma_tf32(acc[j], lo[0], lo[1], lo[2], lo[3], bh0, bh1);  // A_lo V_hi
+        mma_tf32(acc[j], a[0], a[1], a[2], a[3], bh0, bh1);      // A_hi V_hi
+      }
+    }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);
+    if (++stage == p.nstages) { stage = 0; phase ^= 1u; }
+#pragma unroll
+    for (int j = 0; j < NT; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) out[j][e] += acc[j][e];
+    if (++kc < p.nk) continue;
+    // row block complete: rows m0+g (c0, c1) and m0+g+8 (c2, c3), columns 8j+2t, 8j+2t+1
+    kc = 0;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t grow = row0 + m0 + g + 8 * h;
+      if (grow < p.rows) {
+        float* crow = p.C + grow * p.r;
+#pragma unroll
+        for (int j = 0; j < NT; ++j) {
+          const int c = 8 * j + 2 * t;
+          if ((p.r & 1) == 0) {
+            if (c < p.r) *reinterpret_cast<float2*>(crow + c) = make_float2(out[j][2 * h], out[j][2 * h + 1]);
+          } else {
+            if (c < p.r) crow[c] = out[j][2 * h];
+            if (c + 1 < p.r) crow[c + 1] = out[j][2 * h + 1];
+          }
+        }
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < NT; ++j)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) out[j][e] = 0.f;
+    row0 += (int64_t)gridDim.x * PT_BM;
+  }
 }
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-// D[tmem] += A[tmem] * B[smem]  (A operand read from tensor memory: lane = row, column = k)
-__device__ __forceinline__ void tcgen05_mma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                                    uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-      :
-      : "r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      :
-      : "r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-        "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]),
-        "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]),
-        "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 __global__ void __launch_bounds__(PT_THREADS, 1)
 project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_vhi,
@@ -116,43 +134,19 @@ project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   unsigned char* v_res = stage_base + (size_t)p.nstages * p.stage_bytes;   // resident V (vres): nk x [V_hi; V_lo] chunks
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(stage_base + PT_RING_BYTES);
   uint64_t* empty_bar = full_bar + PT_MAX_STAGES;
-  uint64_t* alo_full = empty_bar + PT_MAX_STAGES;
-  uint64_t* alo_empty = alo_full + PT_ALO_SLOTS;
-  uint64_t* acc_full = alo_empty + PT_ALO_SLOTS;
-  uint64_t* acc_empty = acc_full + PT_MAX_SLOTS;
-  uint64_t* v_bar = acc_empty + PT_MAX_SLOTS;
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(v_bar + 1);
-  const int slot_w = 2 * p.npad;                 // A_hi V_hi (+ A_lo V_hi) | A_hi V_lo
-  const int nslots = PT_ACC_COLS / slot_w;       // 8 (npad 16) .. 2 (npad 64)
+  uint64_t* v_bar = empty_bar + PT_MAX_STAGES;
   const int vchunk_bytes = 2 * p.npad * PT_KC * 4;
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     for (int s = 0; s < PT_MAX_STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < PT_ALO_SLOTS; ++s) {
-      mbar_init(&alo_full[s], 4);    // one arrival per split warp
-      mbar_init(&alo_empty[s], 1);
-    }
-    for (int s = 0; s < PT_MAX_SLOTS; ++s) {
-      mbar_init(&acc_full[s], 1);
-      mbar_init(&acc_empty[s], 4);   // one arrival per epilogue warp
+      mbar_init(&empty_bar[s], PT_MMA_WARPS);
     }
     mbar_init(v_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp_idx == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_ptr_smem)),
-                 "r"((uint32_t)PT_TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
   const int64_t my_blocks = (p.num_row_blocks - blockIdx.x + gridDim.x - 1) / gridDim.x;  // may be 0
   const int64_t total_items = my_blocks * p.nk;
@@ -186,175 +180,13 @@ project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         if (++stage == p.nstages) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp_idx == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      const uint32_t idesc2 = make_idesc_tf32_kk(PT_BM, 2 * p.npad);  // A x [V_hi; V_lo]
-      const uint32_t idesc1 = make_idesc_tf32_kk(PT_BM, p.npad);      // A_lo x V_hi
-      int stage = 0, aslot = 0, slot = 0, sl = 0;
-      uint32_t phase = 0, aphase = 0, acc_phase = 0;
-      const int64_t tiles = my_blocks * p.nslabs;
-      if (p.vres && tiles > 0) mbar_wait(v_bar, 0);
-      // descriptors differ only in the 14-bit start-address field: build the constant part once
-      const uint64_t desc_hi = make_k_major_desc(0);
-      const uint32_t stage0 = smem_u32(stage_base), vres0 = smem_u32(v_res);
-      for (int64_t tile = 0; tile < tiles; ++tile) {  // no 64-bit divisions in here: this one thread paces the CTA
-        const int kc_begin = sl * p.slab, kc_end = (kc_begin + p.slab < p.nk) ? kc_begin + p.slab : p.nk;
-        mbar_wait(&acc_empty[slot], acc_phase ^ 1u);  // epilogue has drained this accumulator
-        tcgen05_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(slot * slot_w);
-        for (int kc = kc_begin; kc < kc_end; ++kc) {
-          const uint32_t sb = stage0 + (uint32_t)(stage * p.stage_bytes);
-          const uint32_t vb = p.vres ? vres0 + (uint32_t)(kc * vchunk_bytes) : sb + PT_A_BYTES;
-          const uint64_t bd = desc_hi | (uint64_t)((vb >> 4) & 0x3FFF);
-          const uint32_t araw = tmem_base + (uint32_t)(PT_ALO_COL + aslot * PT_ALO_W), alo = araw + PT_KC;
-          mbar_wait(&full_bar[stage], phase);   // V chunk of this stage (streaming mode) landed
-          mbar_wait(&alo_full[aslot], aphase);  // the split warps have put A (raw) and A_lo of this chunk in tensor memory
-          tcgen05_fence_after();
-          // A_hi (raw bits, truncated by the tensor core) x [V_hi; V_lo]; one k-step = 8 TMEM columns / 32 B of V
-          tcgen05_mma_tf32_ts(tmem_d, araw, bd, idesc2, kc > kc_begin ? 1u : 0u);
-          tcgen05_mma_tf32_ts(tmem_d, araw + 8, bd + 2, idesc2, 1u);
-          tcgen05_mma_tf32_ts(tmem_d, araw + 16, bd + 4, idesc2, 1u);
-          tcgen05_mma_tf32_ts(tmem_d, araw + 24, bd + 6, idesc2, 1u);
-          tcgen05_mma_tf32_ts(tmem_d, alo, bd, idesc1, 1u);
-          tcgen05_mma_tf32_ts(tmem_d, alo + 8, bd + 2, idesc1, 1u);
-          tcgen05_mma_tf32_ts(tmem_d, alo + 16, bd + 4, idesc1, 1u);
-          tcgen05_mma_tf32_ts(tmem_d, alo + 24, bd + 6, idesc1, 1u);
-          tcgen05_commit(&empty_bar[stage]);   // shared-memory stage reusable
-          tcgen05_commit(&alo_empty[aslot]);   // tensor-memory A_lo slot reusable
-          if (++stage == p.nstages) { stage = 0; phase ^= 1u; }
-          if (++aslot == p.alo_slots) { aslot = 0; aphase ^= 1u; }
-        }
-        tcgen05_commit(&acc_full[slot]);
-        if (++slot == nslots) { slot = 0; acc_phase ^= 1u; }
-        if (++sl == p.nslabs) sl = 0;
-      }
-    }
-  } else if (warp_idx < 6) {
-    // ================= split warps: A_lo = A - trunc_tf32(A), one row per thread, into tensor memory =================
-    const int lg = warp_idx & 3;          // TMEM lane group this warp may access
-    const int m = lg * 32 + lane;         // tile row
-    const uint32_t row_off = (uint32_t)((m >> 3) * 1024 + (m & 7) * 128);
-    int stage = 0, aslot = 0;
-    uint32_t phase = 0, aphase = 0;
-    for (int64_t item = 0; item < total_items; ++item) {
-      mbar_wait(&full_bar[stage], phase);
-      const unsigned char* a = stage_base + (size_t)stage * p.stage_bytes + row_off;
-      uint32_t raw[32], lo[32];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {  // 16-byte unit u of the row sits at (u ^ (row % 8)) under SWIZZLE_128B
-        const float4 v = *reinterpret_cast<const float4*>(a + ((u ^ (m & 7)) << 4));
-        raw[4 * u + 0] = __float_as_uint(v.x);
-        raw[4 * u + 1] = __float_as_uint(v.y);
-        raw[4 * u + 2] = __float_as_uint(v.z);
-        raw[4 * u + 3] = __float_as_uint(v.w);
-        lo[4 * u + 0] = __float_as_uint(v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u));
-        lo[4 * u + 1] = __float_as_uint(v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u));
-        lo[4 * u + 2] = __float_as_uint(v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u));
-        lo[4 * u + 3] = __float_as_uint(v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u));
-      }
-      mbar_wait(&alo_empty[aslot], aphase ^ 1u);  // the MMAs that read this slot last have completed
-      tcgen05_fence_after();
-      const uint32_t tdst = tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(PT_ALO_COL + aslot * PT_ALO_W);
-      tmem_st_32x32b_x32(tdst, raw);
-      tmem_st_32x32b_x32(tdst + PT_KC, lo);
-      tmem_st_wait();
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&alo_full[aslot]);
-      if (++stage == p.nstages) { stage = 0; phase ^= 1u; }
-      if (++aslot == p.alo_slots) { aslot = 0; aphase ^= 1u; }
-    }
-  } else {
-    // ================= epilogue warps =================
-    const int lane_group = warp_idx & 3;
-    const int row_in_tile = lane_group * 32 + lane;
-    float* epi = reinterpret_cast<float*>(stage_base + PT_RING_BYTES + 512) + (size_t)lane_group * 32 * 64;
-    const int64_t tiles = my_blocks * p.nslabs;
-    int slot = 0, sl = 0;
-    uint32_t acc_phase = 0;
-    int64_t grow = (int64_t)blockIdx.x * PT_BM + row_in_tile;
-    for (int64_t tile = 0; tile < tiles; ++tile) {
-      const bool add = sl != 0;  // later slabs of a row block add to what this warp stored before
-      mbar_wait(&acc_full[slot], acc_phase);
-      tcgen05_fence_after();
-      if ((p.r & 3) == 0) {
-        // r a multiple of 4 (the TT sweep): every lane stores its own row in 16-byte pieces
-        for (int c0 = 0; c0 < p.npad; c0 += 16) {
-          uint32_t v[16], w[16];
-          const uint32_t t0 = tmem_base + ((uint32_t)(lane_group * 32) << 16) + (uint32_t)(slot * slot_w + c0);
-          tmem_ld_32x32b_x16(t0, v);                       // A_hi V_hi + A_lo V_hi
-          tmem_ld_32x32b_x16(t0 + (uint32_t)p.npad, w);    // A_hi V_lo
-          tmem_ld_wait();
-          if (grow < p.rows) {
-            float* out = p.C + grow * p.r + c0;
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-              if (c0 + 4 * q + 3 < p.r) {
-                float4 o = make_float4(__uint_as_float(v[4 * q]) + __uint_as_float(w[4 * q]),
-                                       __uint_as_float(v[4 * q + 1]) + __uint_as_float(w[4 * q + 1]),
-                                       __uint_as_float(v[4 * q + 2]) + __uint_as_float(w[4 * q + 2]),
-                                       __uint_as_float(v[4 * q + 3]) + __uint_as_float(w[4 * q + 3]));
-                float4* dst = reinterpret_cast<float4*>(out + 4 * q);
-                if (add) {
-                  const float4 old = *dst;
-                  o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w;
-                }
-                *dst = o;
-              }
-          }
-        }
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&acc_empty[slot]);
-      } else {
-        // Any other r (the CP-ALS projections, r = 50): a lane storing its own row would write 4-byte pieces into 32
-        // different sectors per instruction.  The 32 rows of this warp are ONE contiguous block of 32*r floats of C, so
-        // the tile goes through shared memory (row-major, stride r) and leaves as full 128-byte lines.
-        for (int c0 = 0; c0 < p.npad; c0 += 16) {
-          uint32_t v[16], w[16];
-          const uint32_t t0 = tmem_base + ((uint32_t)(lane_group * 32) << 16) + (uint32_t)(slot * slot_w + c0);
-          tmem_ld_32x32b_x16(t0, v);
-          tmem_ld_32x32b_x16(t0 + (uint32_t)p.npad, w);
-          tmem_ld_wait();
-          float* srow = epi + lane * p.r + c0;
-#pragma unroll
-          for (int q = 0; q < 16; ++q)
-            if (c0 + q < p.r) srow[q] = __uint_as_float(v[q]) + __uint_as_float(w[q]);
-        }
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&acc_empty[slot]);  // the accumulator is free while the tile drains from shared memory
-        const int64_t wrow0 = grow - lane;  // first row of this warp's block
-        int64_t nvalid = p.rows - wrow0;
-        if (nvalid > 32) nvalid = 32;
-        if (nvalid > 0) {
-          float* gout = p.C + wrow0 * p.r;  // 32*r*4 bytes per warp block, 128*r*4 per tile: 16-byte aligned
-          const int nfl = (int)nvalid * p.r, n4 = nfl >> 2;
-          const float4* s4 = reinterpret_cast<const float4*>(epi);
-          float4* g4 = reinterpret_cast<float4*>(gout);
-          for (int i = lane; i < n4; i += 32) {
-            float4 o = s4[i];
-            if (add) {
-              const float4 old = g4[i];
-              o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w;
-            }
-            g4[i] = o;
-          }
-          for (int i = 4 * n4 + lane; i < nfl; i += 32) gout[i] = add ? gout[i] + epi[i] : epi[i];
-        }
-        __syncwarp();  // the staging block is rewritten by the next tile
-      }
-      if (++slot == nslots) { slot = 0; acc_phase ^= 1u; }
-      if (++sl == p.nslabs) { sl = 0; grow += (int64_t)gridDim.x * PT_BM; }
-    }
+    return;
   }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp_idx == 1) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)PT_TMEM_COLS)
-                 : "memory");
+  switch (p.npad) {
+    case 16: project_tc_consume<2>(p, stage_base, v_res, full_bar, empty_bar, v_bar, total_items); break;
+    case 32: project_tc_consume<4>(p, stage_base, v_res, full_bar, empty_bar, v_bar, total_items); break;
+    case 48: project_tc_consume<6>(p, stage_base, v_res, full_bar, empty_bar, v_bar, total_items); break;
+    default: project_tc_consume<8>(p, stage_base, v_res, full_bar, empty_bar, v_bar, total_items); break;
   }
 }
 
@@ -397,22 +229,19 @@ inline int encode_kmajor_f32(CUtensorMap* tmap, const float* ptr, int64_t rows, 
 // C (rows x r) = A (rows x K) V (K x r); ws: project_tc_workspace_bytes(K, r).
 inline int project_tc_f32(const float* A, int64_t rows, int64_t K, const float* V, int r, float* C, void* ws, size_t ws_bytes,
                           cudaStream_t st) {
-  if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "project_tc: needs an sm_100 device");
+  if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "project_tc: needs an sm_90 device");
   if (!project_tc_shape_ok(rows, K, r, A, C)) return fail(TNB_ERR_UNSUPPORTED, "project_tc: unsupported shape");
   if (ws_bytes < project_tc_workspace_bytes(K, r)) return fail(TNB_ERR_WORKSPACE, "project_tc: workspace too small");
   ProjTcParams p;
   p.rows = rows; p.K = (int)K; p.r = r; p.npad = (r + 15) / 16 * 16;
   p.num_row_blocks = (rows + PT_BM - 1) / PT_BM;
   p.nk = (int)((K + PT_KC - 1) / PT_KC);
-  p.slab = PT_SLAB_CHUNKS;
-  p.nslabs = (p.nk + p.slab - 1) / p.slab;
   p.C = C;
   const int vchunk = 2 * p.npad * PT_KC * 4;
   p.vres = ((int64_t)p.nk * vchunk <= PT_VRES_MAX_BYTES) ? 1 : 0;
   p.stage_bytes = PT_A_BYTES + (p.vres ? 0 : vchunk);
   p.nstages = (PT_RING_BYTES - (p.vres ? p.nk * vchunk : 0)) / p.stage_bytes;
   if (p.nstages > PT_MAX_STAGES) p.nstages = PT_MAX_STAGES;
-  p.alo_slots = PT_ALO_SLOTS;
   float* Vhi = static_cast<float*>(ws);
   float* Vlo = reinterpret_cast<float*>(static_cast<char*>(ws) + align_up((size_t)p.npad * K * sizeof(float)));
   split_v_kernel<<<grid_for((int64_t)p.npad * K), 256, 0, st>>>(V, (int)K, r, p.npad, Vhi, Vlo);
@@ -425,8 +254,7 @@ inline int project_tc_f32(const float* A, int64_t rows, int64_t K, const float* 
   TNB_CUDA(ensure_dyn_smem(attr_done, project_tc_kernel, PT_SMEM_BYTES));
   const int sms = usable_sms();
   const int64_t grid = p.num_row_blocks < sms ? p.num_row_blocks : sms;
-  const int smem = PT_SMEM_BYTES - ((r & 3) == 0 ? PT_EPI_BYTES : 0);  // the staging block only where it is used
-  project_tc_kernel<<<(unsigned)grid, PT_THREADS, smem, st>>>(ta, th, tl, p);
+  project_tc_kernel<<<(unsigned)grid, PT_THREADS, PT_SMEM_BYTES, st>>>(ta, th, tl, p);
   TNB_LAUNCH_CHECK();
   return TNB_OK;
 }

@@ -19,7 +19,6 @@
 #include "jacobi2.cuh"
 #include "small_kernels.cuh"
 #include "gram_tc.cuh"
-#include "gram_tc2.cuh"
 #include "project.cuh"
 #include "project_tc.cuh"
 #include "chfsi_dev.cuh"
@@ -42,11 +41,6 @@ inline int project_any(const T* A, int64_t rows, int64_t n, const T* V, int64_t 
     return project_f32_fast(reinterpret_cast<const float*>(A), rows, n, reinterpret_cast<const float*>(V), (int)r,
                             reinterpret_cast<float*>(C), st);
   return gemm_direct<T, T, T, T>(rows, r, n, A, n, true, V, r, false, C, r, (T)1, nullptr, 0, (T)0, nullptr, 0, (T)0, st);
-}
-
-inline bool gram_use_pairs(int64_t rows, int64_t n) {
-  static const bool disabled = getenv("TNB_GRAM_TC2") && atoi(getenv("TNB_GRAM_TC2")) == 0;  // A/B switch for profiling
-  return !disabled && gram_tc2_shape_ok(rows, n);
 }
 
 constexpr int64_t TC_MIN_ROWS = 2048;  // below this the generic fp64-accumulating Gram is used
@@ -111,7 +105,7 @@ inline void gram_carve(ArenaT& ar, int64_t rows, int64_t n, bool allow_tc, GramW
   w.tc_bytes = 0;
   w.tc_ws = nullptr;
   if (allow_tc && std::is_same<T, float>::value && tall && rows >= TC_MIN_ROWS && gram_tc_shape_ok(rows, n)) {
-    w.tc_bytes = std::max(gram_tc_workspace_bytes(rows, n), gram_tc2_shape_ok(rows, n) ? gram_tc2_workspace_bytes(rows, n) : 0);
+    w.tc_bytes = gram_tc_workspace_bytes(rows, n);
     w.tc_ws = ar.template take<char>(w.tc_bytes);
   }
 }
@@ -124,8 +118,6 @@ inline int gram_small_side(const T* C, int64_t rows, int64_t n, double* G, float
   if (tall) {
     if (use_tc && w.tc_ws && std::is_same<T, float>::value) {
       if (used_tc) *used_tc = 1;
-      if (gram_use_pairs(rows, n))  // wide Gram: 256 x 256 tiles on CTA pairs
-        return gram_tc2_f32(reinterpret_cast<const float*>(C), rows, n, G, Gf, w.tc_ws, w.tc_bytes, st);
       return gram_tc_f32(reinterpret_cast<const float*>(C), rows, n, G, Gf, w.tc_ws, w.tc_bytes, st);
     }
     GemmPlan pl = plan_gemm(n, n, rows, true);
@@ -493,14 +485,16 @@ inline int spec_step_eig_begin(const StepCtx& cx, SpecStep<T>& s) {
   cudaStream_t st = cx.st;
   if (!s.chfsi) {
     // a TF32 Gram is accurate to ~2e-6 ||G||: rotating it in fp32 (backward error ~1e-6 ||G||, covered by the accept rule's
-    // noise allowance) is consistent with it and 3-4x cheaper than fp64 on this machine (~16 fp64 FMAs / clk / SM);
+    // noise allowance) is consistent with it and cheaper than fp64 rotations.  The stop is at 2e-7, near the fp32
+    // resolution, not at the noise level: the eigenvectors at the rank cutoff decide what the next steps see (a 2e-6 stop
+    // moved a flat-spectrum randn 64^4 decomposition by 3e-6 in relative error against the fp64 rotations);
     // eigenvalues still come out as fp64 Rayleigh quotients and the vectors are re-orthonormalised (jacobi2.cuh).
     // The same holds for fp32 DATA whatever Gram kernel produced G, as long as the accept rule — which then guards the
     // fp32 solve instead of the TF32 Gram, same noise allowance — finds the spectrum benign; a rejected step is repeated
     // on the host-driven path with fp64 rotations.
     const bool single = std::is_same<T, float>::value && (cx.allow_tc && !cx.exact_gram) && jacobi2_ok((int)L, true);
     s.used_tc = (s.used_tc || single) ? 1 : 0;
-    return jacobi2_eigh(s.G, (int)L, (int)L, s.w, s.V, s.jscratch, s.jinfo, st, single, single ? 2e-6 : 0.0);
+    return jacobi2_eigh(s.G, (int)L, (int)L, s.w, s.V, s.jscratch, s.jinfo, st, single, single ? 2e-7 : 0.0);
   }
   if (cx.info) cx.info->eig_solves += 1;
   return cd_begin(s.cd, s.Gf, (int)L, (int)s.kcap, s.b, &cx.sc->trace, 1e-6, s.cw, s.w, s.V, cx.d_flags, st);
@@ -929,7 +923,7 @@ inline int ttsvd_batch_impl(void* workspace, size_t per_tensor_bytes, int inflig
     for (int s = 0; s < g && rc == TNB_OK; ++s)
       rc = spec_begin<T, Arena>(runs[s], arenas[s], false, data[g0 + s], d, eps, bflags, cores[g0 + s], &infos[g0 + s],
                                 pool.st[s], hbs + g0 + s);
-    // Enqueue order (TNB_BATCH_ORDER, measured on B200 with 6 x 64^5 in flight — profiles/r02_batch_schedule.md):
+    // Enqueue order (TNB_BATCH_ORDER):
     //   "stage" (default): step by step; all Gram kernels of a step, then the eigen stages of all tensors INTERLEAVED
     //            stage by stage (the resident filter kernels of all streams run one after the other, cheb_filter.cuh:
     //            this way tensor A's Rayleigh-Ritz step is in flight while tensor B's filter runs), then every

@@ -1,12 +1,11 @@
 // tnb200 — single translation unit: C-ABI entry points declared in include/tnb200.h.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -shared -Xcompiler -fPIC (see build.py)
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -shared -Xcompiler -fPIC (see build.py)
 #include "common.cuh"
 #include "gemm_generic.cuh"
 #include "jacobi.cuh"
 #include "small_kernels.cuh"
 #include "eig.cuh"
 #include "gram_tc.cuh"
-#include "gram_tc2.cuh"
 #include "sweep.cuh"
 #include "round_impl.cuh"
 #include "cp_als.cuh"
@@ -117,7 +116,7 @@ size_t tnb_ttsvd_batch_workspace_bytes(int dtype, int batch, int ndim, const int
   const size_t one = tnb_ttsvd_workspace_bytes(dtype, ndim, shape, rmax, flags);
   if (per_tensor_bytes) *per_tensor_bytes = one;
   if (one == 0 || batch < 1) return 0;
-  const int inflight = batch < TNB_BATCH_MAX_INFLIGHT ? batch : TNB_BATCH_MAX_INFLIGHT;  // measured on B200: 4 -> 171, 6 -> 172, 8 -> 175 GElements/s
+  const int inflight = batch < TNB_BATCH_MAX_INFLIGHT ? batch : TNB_BATCH_MAX_INFLIGHT;
   return one * (size_t)inflight;
 }
 
@@ -586,16 +585,13 @@ int tnb_gram(int dtype, const void* A, int64_t rows, int64_t n, double* G, void*
 
 size_t tnb_gram_tc_workspace_bytes(int64_t rows, int64_t n) {
   if (!gram_tc_shape_ok(rows, n)) return 0;
-  size_t b = gram_tc_workspace_bytes(rows, n);
-  if (gram_tc2_shape_ok(rows, n)) b = std::max(b, gram_tc2_workspace_bytes(rows, n));
-  return b + 256;
+  return gram_tc_workspace_bytes(rows, n) + 256;
 }
 
 int tnb_gram_tc_f32(const float* A, int64_t rows, int64_t n, double* G, void* workspace, size_t workspace_bytes,
                     void* stream) {
   TNB_TRY(require_device());
   if (!A || !G || !workspace) return fail(TNB_ERR_INVALID, "tnb_gram_tc_f32: null argument");
-  if (gram_use_pairs(rows, n)) return gram_tc2_f32(A, rows, n, G, nullptr, workspace, workspace_bytes, as_stream(stream));
   return gram_tc_f32(A, rows, n, G, nullptr, workspace, workspace_bytes, as_stream(stream));
 }
 

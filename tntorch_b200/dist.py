@@ -110,7 +110,7 @@ def round_tt_batch_sharded(tts: Sequence[Sequence[torch.Tensor]], rmax=None, eps
 
 
 def cp_als_batch_sharded(tensors: Sequence[torch.Tensor], R: int, max_iter: int = 25, tol: float = 1e-4, gather: bool = True):
-    """config 4 ("1 vs 8 B200 batch-sharded"): independent CP-ALS problems, one per owned tensor."""
+    """config 4 ("1 vs 8 GPUs batch-sharded"): independent CP-ALS problems, one per owned tensor."""
     from . import ops
 
     return batch_sharded(tensors, lambda X: ops.cp_als(X, R, max_iter=max_iter, tol=tol), gather)

@@ -65,7 +65,7 @@ def set_reserved_sms(n: int) -> None:
 
 
 def measure_tf32_peak(reps: int = 200, per_commit: int = 64, trials: int = 5):
-    """Dense TF32 tcgen05 peak of the current GPU in TFLOP/s (csrc/peak_tf32.cuh)."""
+    """Dense TF32 mma.sync peak of the current GPU in TFLOP/s (csrc/peak_tf32.cuh)."""
     tf, ms = (C.c_double * 1)(), (C.c_double * 1)()
     check(lib().tnb_measure_tf32_peak(int(reps), int(per_commit), int(trials), tf, ms, _stream()))
     return float(tf[0]), float(ms[0])
@@ -658,7 +658,7 @@ def qr(A: torch.Tensor, return_r: bool = False):
 
 
 def gram(A: torch.Tensor, tensorcore: bool = False) -> torch.Tensor:
-    """fp64 Gram matrix A^T A of a (rows x n) matrix; tensorcore=True uses the tcgen05/TMA kernel (fp32 only)."""
+    """fp64 Gram matrix A^T A of a (rows x n) matrix; tensorcore=True uses the TMA tensor-core kernel (fp32 only)."""
     _require_cuda(A, "gram")
     A = A.contiguous()
     rows, n = A.shape
@@ -682,7 +682,7 @@ def gram(A: torch.Tensor, tensorcore: bool = False) -> torch.Tensor:
 
 def atb_tensorcore(A: torch.Tensor, B: torch.Tensor, alpha: float = 1.0, D: Optional[torch.Tensor] = None,
                    beta: float = 0.0) -> torch.Tensor:
-    """alpha * A^T B + beta * D on the tcgen05 kernel (A: K x m, B: K x n, fp32)."""
+    """alpha * A^T B + beta * D on the tensor-core kernel (A: K x m, B: K x n, fp32)."""
     _require_cuda(A, "atb_tensorcore")
     A, B = A.contiguous(), B.contiguous()
     K, m = A.shape

@@ -18,7 +18,7 @@ from . import ops
 def _default_device(device):
     if device is None:
         if not torch.cuda.is_available():
-            raise RuntimeError("tntorch_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+            raise RuntimeError("tntorch_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
         return torch.device("cuda", torch.cuda.current_device())
     device = torch.device(device)
     if device.type != "cuda":
@@ -27,7 +27,7 @@ def _default_device(device):
 
 
 class Tensor(object):
-    """TT tensor whose decomposition / rounding runs on B200 kernels (mirror of tntorch.Tensor)."""
+    """TT tensor whose decomposition / rounding runs on H100 kernels (mirror of tntorch.Tensor)."""
 
     def __init__(
         self,
@@ -185,7 +185,7 @@ class Tensor(object):
                       batch=self.batch)
 
     def __repr__(self):
-        return f"{self.dim()}D TT tensor (B200): shape {list(self.shape)}, TT ranks {self.ranks_tt.tolist()}"
+        return f"{self.dim()}D TT tensor (H100): shape {list(self.shape)}, TT ranks {self.ranks_tt.tolist()}"
 
     # ------------------------------------------------------------------ arithmetic that feeds the rounding path
     def _tt_cores(self):
