@@ -184,6 +184,11 @@ int tnb_tt_hadamard(int dtype, const void* const* cores_a, const void* const* co
  * `reps` x `per_commit` MMAs per accumulator; best of `trials` launches timed with CUDA events.  The denominator of the
  * tensor-bound roofline fractions. */
 int tnb_measure_tf32_peak(int32_t reps, int32_t per_commit, int32_t trials, double* tflops_host, double* ms_host, void* stream);
+/* The same for wgmma.mma_async m64n256k8 .tf32, the instruction of the Gram / A^T B kernel: one CTA per SM, two
+ * warpgroups each issuing it with A from registers and B from a fixed shared-memory buffer into their own 128
+ * accumulators; `reps` commit groups of 4 x `per_commit` wgmma per warpgroup. */
+int tnb_measure_wgmma_tf32_peak(int32_t reps, int32_t per_commit, int32_t trials, double* tflops_host, double* ms_host,
+                                void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Two-factor rank-revealing split  M (m x n)  ->  left (m x r), right (r x n).

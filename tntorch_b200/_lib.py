@@ -84,6 +84,7 @@ SIGNATURES = {
                                          _vp]),
     "tnb_cross_tt_eval": (C.c_int, [C.POINTER(_vp), C.c_int32, _i32p, _i32p, _vp, C.c_int32, C.c_int32, C.c_int32, _vp, _vp]),
     "tnb_measure_tf32_peak": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, _f64p, _f64p, _vp]),
+    "tnb_measure_wgmma_tf32_peak": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, _f64p, _f64p, _vp]),
     "tnb_matmul": (C.c_int, [C.c_int, _vp, _vp, _vp, C.c_int64, C.c_int64, C.c_int64, _vp]),
     "tnb_qr_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
     "tnb_qr_householder": (C.c_int, [_vp, C.c_int32, C.c_int32, C.c_int32, _vp, C.c_size_t, _vp, _vp, _vp]),

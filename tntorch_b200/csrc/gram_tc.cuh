@@ -3,17 +3,19 @@
 //   * row slabs of C are staged HBM -> shared memory by TMA (cp.async.bulk.tensor.2d, 128-byte swizzle,
 //     out-of-bounds rows/columns zero-filled by the TMA unit), 4-stage mbarrier ring;
 //   * the contraction runs over the ROW index of C, so both operands are "MN-major" views of the very same
-//     slab.  tf32 wgmma only takes K-major shared-memory operands, so the products run on the warp-level
-//     tensor-core MMA (mma.sync m16n8k8 .tf32, fp32 accumulation in registers) with the fragments read
-//     straight out of the swizzled slab (mma_frag_* below: conflict-free, no transpose pass);
+//     slab.  tf32 wgmma takes its shared-memory B operand K-major only, but takes A from registers: the A
+//     fragments are read straight out of the swizzled slab (mma_frag_a_mn: conflict-free), and only the B
+//     columns of each stage are transposed into a K-major, 128-byte-swizzled buffer that a wgmma descriptor reads;
 //   * G is symmetric: only tiles that touch the upper triangle are computed, and on diagonal tiles the
 //     A operand is a sub-block of the B slab (loaded once);
 //   * split-K over row ranges across CTAs; partial tiles go registers -> global and are summed in fp64 by a
 //     deterministic second kernel (no atomics).
 //
-// 256 threads = eight MMA warps, a 2 x 4 grid of 64 x tn/4 warp tiles over the 128 x tn output tile; thread 0 also
-// issues the TMA loads, TC_STAGES - 1 stages ahead.  (A separate producer warp would make it 288 threads, which the
-// register allocator rounds up to 384: 168 registers per thread, too few for the 128 accumulators of a 64 x 64 tile.)
+// 384 threads = three warpgroups, warp-specialized.  Warpgroup 0 is the producer: its warp 0 issues the TMA loads of a
+// TC_STAGES-deep slab ring, its warps 1-3 transpose the B boxes of each stage into one of TC_TB_STAGES K-major buffers.
+// Warpgroups 1 and 2 are the consumers: each owns 64 rows of the 128 x tn output tile and runs
+// wgmma.mma_async m64n{tn}k8 .f32.tf32.tf32 with A from registers, accumulating in registers.  setmaxnreg moves the
+// register file to the consumers (TC_CONSUMER_REGS: 128 accumulators plus two stages of A fragments).
 //
 // Replaces, for large fp32 unfoldings, the QR of tensor.py:1816 / the Gram of round.py:104-110.
 #pragma once
@@ -27,12 +29,17 @@ namespace tnb {
 
 constexpr int TC_KC = 32;                       // rows of C per pipeline stage
 constexpr int TC_BOX_BYTES = TC_KC * 128;       // one TMA box: 32 fp32 columns x KC rows
-constexpr int TC_STAGES = 4;
+constexpr int TC_STAGES = 3;                    // slab ring depth
 constexpr int TC_MAX_BOXES = 12;                // 4 (A) + 8 (B)
 constexpr int TC_STAGE_BYTES = TC_MAX_BOXES * TC_BOX_BYTES;
-constexpr int TC_MMA_WARPS = 8;
-constexpr int TC_THREADS = 32 * TC_MMA_WARPS;
-constexpr int TC_SMEM_BYTES = TC_STAGES * TC_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+constexpr int TC_TB_STAGES = 2;                 // transposed-B ring depth (the consumer loop is unrolled by it)
+constexpr int TC_TB_BYTES = 256 * TC_KC * 4;    // up to 256 columns x KC rows, K-major
+constexpr int TC_TRANSPOSE_THREADS = 96;        // producer warps 1-3
+constexpr int TC_THREADS = 384;
+constexpr int TC_PRODUCER_REGS = 40;
+constexpr int TC_CONSUMER_REGS = 232;
+constexpr int TC_SMEM_BYTES =
+    TC_STAGES * TC_STAGE_BYTES + TC_TB_STAGES * TC_TB_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 // Longest run of rows one CTA accumulates in fp32 registers (512 stages = 16384 rows).  The diagonal of a Gram grows with
 // the row count while the rounding error of an fp32 sum grows faster; 16384-row partial sums keep that error well below
 // the TF32 operand noise the accept rule of the sweep budgets for.
@@ -100,6 +107,21 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
   }
 }
+// The same bound without the printf, for kernels that issue wgmma: a function call anywhere in such a kernel makes ptxas
+// serialize the wgmma pipeline.
+__device__ __forceinline__ void mbar_wait_quiet(uint64_t* bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity))
+    if (clock64() - t0 > 4000000000LL) __trap();
+}
+// Unbounded wait, for warps that raised their register budget with setmaxnreg: a trap in that region makes ptxas fall
+// back to the launch budget (spills, serialized wgmma).  Only use it on barriers whose producer waits with a bound, so
+// that a stuck pipeline still ends in that producer's trap.
+__device__ __forceinline__ void mbar_wait_spin(uint64_t* bar, uint32_t parity) {
+  while (!mbar_try_wait(bar, parity)) {
+  }
+}
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int c0, int c1) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
@@ -143,16 +165,219 @@ __device__ __forceinline__ void mma_frag_b_mn(const unsigned char* base, int k0,
 }
 
 // ---------------------------------------------------------------------------------------------
+// wgmma: tf32, A from registers, B from a K-major SWIZZLE_128B shared-memory buffer
+// ---------------------------------------------------------------------------------------------
+// Shared-memory descriptor of a K-major SWIZZLE_128B operand: rows of 128 bytes (32 tf32 along K), 8-row atoms of
+// 1024 bytes stacked along N (stride byte offset 1024; the leading byte offset is unused by this layout).  The buffer is
+// 1024-byte aligned, so the base offset is 0.  Adding 2 (32 bytes) to the descriptor selects the next k8 slice.
+__device__ __forceinline__ uint64_t wgmma_desc_kmajor_sw128(const void* p) {
+  return (uint64_t)((smem_u32(p) & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
+         ((uint64_t)1 << 62);
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// Keeps the compiler from moving accesses of an accumulator across the asynchronous wgmma window.
+template <int R>
+__device__ __forceinline__ void wgmma_fence_operand(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// Orders this thread's generic-proxy shared-memory writes before later async-proxy (wgmma, TMA) accesses.
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+
+// D (64 x 32*NT fp32) += A (64 x 8) * B (8 x 32*NT), wgmma.mma_async m64n{32*NT}k8 .f32.tf32.tf32.  A is the m16n8k8 row
+// fragment of each warp's 16 rows (a0: row g, k t; a1: row g+8, k t; a2: row g, k t+4; a3: row g+8, k t+4); d[4j+2h+e]
+// is row 16*warp + g + 8h, column 8j + 2t + e.  B is read through `desc`.  The tensor core truncates the operands to tf32.
+template <int NT>
+__device__ void wgmma_tf32(float (&d)[NT * 16], const uint32_t (&a)[4], uint64_t desc);
+template <>
+__device__ __forceinline__ void wgmma_tf32<1>(float (&d)[16], const uint32_t (&a)[4], uint64_t desc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15"
+      "}, {%16, %17, %18, %19}, %20, 1, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<2>(float (&d)[32], const uint32_t (&a)[4], uint64_t desc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, {%32, %33, %34, %35}, %36, 1, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<3>(float (&d)[48], const uint32_t (&a)[4], uint64_t desc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n96k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47"
+      "}, {%48, %49, %50, %51}, %52, 1, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<4>(float (&d)[64], const uint32_t (&a)[4], uint64_t desc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, {%64, %65, %66, %67}, %68, 1, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<5>(float (&d)[80], const uint32_t (&a)[4], uint64_t desc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n160k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79"
+      "}, {%80, %81, %82, %83}, %84, 1, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<6>(float (&d)[96], const uint32_t (&a)[4], uint64_t desc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n192k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79,"
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+      "}, {%96, %97, %98, %99}, %100, 1, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<7>(float (&d)[112], const uint32_t (&a)[4], uint64_t desc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n224k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79,"
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95,"
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111"
+      "}, {%112, %113, %114, %115}, %116, 1, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+}
+template <>
+__device__ __forceinline__ void wgmma_tf32<8>(float (&d)[128], const uint32_t (&a)[4], uint64_t desc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79,"
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95,"
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111,"
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, {%128, %129, %130, %131}, %132, 1, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
+}
+
+// ---------------------------------------------------------------------------------------------
 // The kernel
 // ---------------------------------------------------------------------------------------------
-// NT = tn / 32: n8 tiles per warp (each warp covers tn / 4 columns)
-// Loads of pipeline iteration `it` (rows it_begin + it) into its ring slot, once the MMA warps have released it.
+// Loads of pipeline iteration `it` (rows it_begin + it) into its ring slot, once the transposers and the consumers have
+// released it.
 __device__ __forceinline__ void gram_tc_produce(const CUtensorMap* tmap, const CUtensorMap* tmap_b, unsigned char* stage_base,
                                                 uint64_t* full_bar, uint64_t* empty_bar, int64_t it, int64_t it_begin,
                                                 int nbox_a, int nbox_b, int a_col0, int b_col0) {
   const int stage = (int)(it % TC_STAGES);
   const uint32_t phase = (uint32_t)(it / TC_STAGES) & 1u;
-  mbar_wait(&empty_bar[stage], phase ^ 1u);
+  mbar_wait_quiet(&empty_bar[stage], phase ^ 1u);
   unsigned char* sb = stage_base + stage * TC_STAGE_BYTES;
   mbar_expect_tx(&full_bar[stage], (uint32_t)(nbox_a + nbox_b) * TC_BOX_BYTES);
   const int row0 = (int)((it_begin + it) * TC_KC);
@@ -161,86 +386,132 @@ __device__ __forceinline__ void gram_tc_produce(const CUtensorMap* tmap, const C
   for (int j = 0; j < nbox_a; ++j) tma_load_2d(sb + (8 + j) * TC_BOX_BYTES, tmap, &full_bar[stage], a_col0 + 32 * j, row0);
 }
 
-template <int NT>
-__device__ __forceinline__ void gram_tc_consume(const CUtensorMap* tmap, const CUtensorMap* tmap_b, const GramTcParams& p,
-                                                unsigned char* stage_base, uint64_t* full_bar, uint64_t* empty_bar,
-                                                int64_t it_begin, int64_t iters, int nbox_a, int a_box, int tile_id,
-                                                int split, int a_col0, int b_col0) {
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = lane >> 2, t = lane & 3;
-  const int wm = w >> 2, wn = w & 3;      // 64-row half of the tile, quarter of its columns
-  const int cm = wm * 64, cn = wn * NT * 8;
-  float acc[4][NT][4];
+// Transposes the nbox B boxes of a slab stage into the K-major buffer tb: element (row k, column c) of box j, at
+// j*TC_BOX_BYTES + k*128 + ((((c%32)/4) ^ (k%8)) * 16) + (c%4)*4, goes to (column c, fragment index kl) at
+// c*128 + (((kl/4) ^ (c%8)) * 16) + (kl%4)*4.  kl is the k index of mma_frag_a_mn: inside each 8-row step kl = t is row
+// 2t and kl = t+4 is row 2t+1, so B carries the permutation of the A fragments and the product is unchanged.
+// A work unit is a 4 x 4 block, 4 columns (16-byte chunk cq of a box row) by 4 fragment indices (16-byte chunk q of a
+// tb row): four 16-byte loads, a register transpose, four 16-byte stores.  The 8 lanes of a quarter-warp take cq = l
+// and q = (l/2) ^ s for one s in 0..7; then both the loads (chunk cq ^ (k%8)) and the stores (chunk q ^ (c%8)) reach 8
+// distinct 16-byte bank groups: no bank conflicts on either side.
+__device__ __forceinline__ void gram_tc_transpose_b(const unsigned char* sb, unsigned char* tb, int nbox, int tid) {
+  for (int u = tid; u < nbox * 64; u += TC_TRANSPOSE_THREADS) {
+    const int l = u & 7, s = (u >> 3) & 7, j = u >> 6;
+    const int q = (l >> 1) ^ s;
+    const int k0 = 8 * (q >> 1) + (q & 1);  // rows k0, k0+2, k0+4, k0+6 hold kl = 4q .. 4q+3
+    float4 v[4];
 #pragma unroll
-  for (int i = 0; i < 4; ++i)
-#pragma unroll
-    for (int j = 0; j < NT; ++j)
-#pragma unroll
-      for (int e = 0; e < 4; ++e) acc[i][j][e] = 0.f;
-
-  if (threadIdx.x == 0)
-    for (int64_t it = 0; it < TC_STAGES - 1 && it < iters; ++it)
-      gram_tc_produce(tmap, tmap_b, stage_base, full_bar, empty_bar, it, it_begin, nbox_a, NT, a_col0, b_col0);
-  int stage = 0;
-  uint32_t phase = 0;
-  for (int64_t it = 0; it < iters; ++it) {
-    if (threadIdx.x == 0 && it + TC_STAGES - 1 < iters)  // refill the slot iteration it - 1 used
-      gram_tc_produce(tmap, tmap_b, stage_base, full_bar, empty_bar, it + TC_STAGES - 1, it_begin, nbox_a, NT, a_col0,
-                      b_col0);
-    __syncwarp();
-    mbar_wait(&full_bar[stage], phase);
-    const unsigned char* sb = stage_base + stage * TC_STAGE_BYTES;
-    const unsigned char* sa = sb + a_box * TC_BOX_BYTES;
-#pragma unroll
-    for (int ks = 0; ks < TC_KC; ks += 8) {
-      uint32_t bf[NT][2];
-#pragma unroll
-      for (int j = 0; j < NT; ++j) mma_frag_b_mn(sb, ks, cn + 8 * j, g, t, bf[j]);
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        uint32_t af[4];
-        mma_frag_a_mn(sa, ks, cm + 16 * i, g, t, af);
-#pragma unroll
-        for (int j = 0; j < NT; ++j) mma_tf32(acc[i][j], af[0], af[1], af[2], af[3], bf[j][0], bf[j][1]);
-      }
+    for (int r = 0; r < 4; ++r) {
+      const int k = k0 + 2 * r;
+      v[r] = *reinterpret_cast<const float4*>(sb + j * TC_BOX_BYTES + k * 128 + ((l ^ (k & 7)) << 4));
     }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty_bar[stage]);  // this warp is done reading the slot
-    if (++stage == TC_STAGES) { stage = 0; phase ^= 1u; }
+    const int c0 = 32 * j + 4 * l;
+    *reinterpret_cast<float4*>(tb + (c0 + 0) * 128 + ((q ^ ((c0 + 0) & 7)) << 4)) = make_float4(v[0].x, v[1].x, v[2].x, v[3].x);
+    *reinterpret_cast<float4*>(tb + (c0 + 1) * 128 + ((q ^ ((c0 + 1) & 7)) << 4)) = make_float4(v[0].y, v[1].y, v[2].y, v[3].y);
+    *reinterpret_cast<float4*>(tb + (c0 + 2) * 128 + ((q ^ ((c0 + 2) & 7)) << 4)) = make_float4(v[0].z, v[1].z, v[2].z, v[3].z);
+    *reinterpret_cast<float4*>(tb + (c0 + 3) * 128 + ((q ^ ((c0 + 3) & 7)) << 4)) = make_float4(v[0].w, v[1].w, v[2].w, v[3].w);
   }
+}
 
-  // epilogue: accumulator element (row r, column c) of the 128 x tn tile; c0/c1 and c2/c3 are column pairs
+// Producer warps 1-3: for every stage, transpose its B boxes into the transposed-B ring and release the slab slot.
+__device__ __forceinline__ void gram_tc_transposer(unsigned char* stage_base, unsigned char* tb_base, uint64_t* full_bar,
+                                                   uint64_t* empty_bar, uint64_t* tb_full, uint64_t* tb_empty,
+                                                   int64_t iters, int nbox_b) {
+  const int tid = threadIdx.x - 32;
+  for (int64_t it = 0; it < iters; ++it) {
+    const int s = (int)(it % TC_STAGES), b = (int)(it % TC_TB_STAGES);
+    mbar_wait_quiet(&full_bar[s], (uint32_t)(it / TC_STAGES) & 1u);
+    mbar_wait_quiet(&tb_empty[b], ((uint32_t)(it / TC_TB_STAGES) & 1u) ^ 1u);
+    gram_tc_transpose_b(stage_base + s * TC_STAGE_BYTES, tb_base + b * TC_TB_BYTES, nbox_b, tid);
+    fence_proxy_async_smem();  // the stores are read by wgmma (async proxy)
+    mbar_arrive(&tb_full[b]);
+    __syncwarp();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(&empty_bar[s]);
+  }
+}
+
+// One pipeline stage of a consumer warp: A fragments of stage `it` into `af`, four k8 wgmma into `acc`, then release
+// the slab slot and, once the previous stage's group has completed, its transposed-B buffer.
+template <int NT>
+__device__ __forceinline__ void gram_tc_consume_stage(float (&acc)[NT * 16], uint32_t (&af)[4][4], int64_t it,
+                                                      const unsigned char* stage_base, uint64_t* full_bar, uint64_t* empty_bar, uint64_t* tb_full,
+                                                      uint64_t* tb_empty, uint64_t desc, int a_box, int cm, int lane) {
+  const int g = lane >> 2, t = lane & 3;
+  const int s = (int)(it % TC_STAGES), b = (int)(it % TC_TB_STAGES);
+  mbar_wait_spin(&full_bar[s], (uint32_t)(it / TC_STAGES) & 1u);
+  const unsigned char* sa = stage_base + s * TC_STAGE_BYTES + a_box * TC_BOX_BYTES;
+#pragma unroll
+  for (int kk = 0; kk < TC_KC / 8; ++kk) mma_frag_a_mn(sa, 8 * kk, cm, g, t, af[kk]);
+  mbar_wait_spin(&tb_full[b], (uint32_t)(it / TC_TB_STAGES) & 1u);
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < TC_KC / 8; ++kk) wgmma_tf32<NT>(acc, af[kk], desc + 2 * kk);
+  wgmma_commit();
+  __syncwarp();
+  if (lane == 0) mbar_arrive(&empty_bar[s]);  // A of this stage is in registers: the slab slot may be refilled
+  wgmma_wait<1>();                            // the previous stage's wgmma group has finished reading its buffer
+  if (it > 0 && lane == 0) mbar_arrive(&tb_empty[(it - 1) % TC_TB_STAGES]);
+}
+
+// Consumer warpgroup cw (0 or 1): rows 64*cw .. 64*cw+63 of the 128 x tn tile, tn = 32*NT, as one m64n{tn} wgmma
+// accumulator.  A fragments of a stage are read from the slab into registers (two register sets: the loads of a stage
+// overlap the wgmma of the previous one), B through the descriptor of the stage's transposed buffer.
+template <int NT>
+__device__ __forceinline__ void gram_tc_consumer(const GramTcParams& p, const unsigned char* stage_base,
+                                                 const unsigned char* tb_base, uint64_t* full_bar, uint64_t* empty_bar,
+                                                 uint64_t* tb_full, uint64_t* tb_empty, int64_t iters, int a_box,
+                                                 int tile_id, int split, int a_col0, int b_col0) {
+  const int ct = threadIdx.x - 128;
+  const int lane = ct & 31, w = (ct >> 5) & 3;
+  const int g = lane >> 2, t = lane & 3;
+  const int cm = 64 * (ct >> 7) + 16 * w;  // first of this warp's 16 rows of the tile
+  float acc[NT * 16];
+#pragma unroll
+  for (int i = 0; i < NT * 16; ++i) acc[i] = 0.f;
+  wgmma_fence_operand(acc);
+
+  // TC_TB_STAGES == 2: even stages read transposed buffer 0 (A fragments af0), odd stages buffer 1 (af1)
+  const uint64_t desc0 = wgmma_desc_kmajor_sw128(tb_base), desc1 = wgmma_desc_kmajor_sw128(tb_base + TC_TB_BYTES);
+  uint32_t af0[4][4], af1[4][4];
+  // The loop leaves right after an odd number of stages: on the back edge only the af1 group can be in flight, so
+  // ptxas can prove that loading af0 does not overwrite registers a pending wgmma reads (else it serializes them).
+  for (int64_t it = 0; it < iters; it += 2) {
+    gram_tc_consume_stage<NT>(acc, af0, it, stage_base, full_bar, empty_bar, tb_full, tb_empty, desc0, a_box, cm, lane);
+    if (it + 1 == iters) break;
+    gram_tc_consume_stage<NT>(acc, af1, it + 1, stage_base, full_bar, empty_bar, tb_full, tb_empty, desc1, a_box, cm,
+                              lane);
+  }
+  wgmma_wait<0>();
+  wgmma_fence_operand(acc);
+
+  // epilogue: acc[4j + 2h + e] is (row cm + g + 8h, column 8j + 2t + e) of the 128 x tn tile
   if (p.direct) {
 #pragma unroll
-    for (int i = 0; i < 4; ++i)
+    for (int h = 0; h < 2; ++h) {
+      const int gi = a_col0 + cm + g + 8 * h;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int gi = a_col0 + cm + 16 * i + g + 8 * h;
+      for (int j = 0; j < 4 * NT; ++j)
 #pragma unroll
-        for (int j = 0; j < NT; ++j)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int gj = b_col0 + cn + 8 * j + 2 * t + e;
-            if (gi < p.m && gj < p.n) {
-              float x = p.alpha * acc[i][j][2 * h + e];
-              if (p.D) x += p.beta * p.D[(size_t)gi * p.ldd + gj];
-              if (p.E) x += p.gamma * p.E[(size_t)gi * p.lde + gj];
-              p.C[(size_t)gi * p.ldc + gj] = x;
-            }
+        for (int e = 0; e < 2; ++e) {
+          const int gj = b_col0 + 8 * j + 2 * t + e;
+          if (gi < p.m && gj < p.n) {
+            float x = p.alpha * acc[4 * j + 2 * h + e];
+            if (p.D) x += p.beta * p.D[(size_t)gi * p.ldd + gj];
+            if (p.E) x += p.gamma * p.E[(size_t)gi * p.lde + gj];
+            p.C[(size_t)gi * p.ldc + gj] = x;
           }
-      }
+        }
+    }
     return;
   }
   float* out = p.partial + ((size_t)split * p.num_tiles + tile_id) * 128 * (size_t)p.tn;
 #pragma unroll
-  for (int i = 0; i < 4; ++i)
+  for (int h = 0; h < 2; ++h) {
+    float* orow = out + (size_t)(cm + g + 8 * h) * p.tn + 2 * t;
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      float* orow = out + (size_t)(cm + 16 * i + g + 8 * h) * p.tn + cn + 2 * t;
-#pragma unroll
-      for (int j = 0; j < NT; ++j)
-        *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(acc[i][j][2 * h], acc[i][j][2 * h + 1]);
-    }
+    for (int j = 0; j < 4 * NT; ++j)
+      *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+  }
 }
 
 __global__ void __launch_bounds__(TC_THREADS, 1)
@@ -251,9 +522,12 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
   const uint32_t raw_addr = smem_u32(tc_smem_raw);
   const uint32_t pad = (1024u - (raw_addr & 1023u)) & 1023u;
   unsigned char* stage_base = tc_smem_raw + pad;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stage_base + TC_STAGES * TC_STAGE_BYTES);
+  unsigned char* tb_base = stage_base + TC_STAGES * TC_STAGE_BYTES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(tb_base + TC_TB_STAGES * TC_TB_BYTES);
   uint64_t* empty_bar = full_bar + TC_STAGES;
-  int* tile_smem = reinterpret_cast<int*>(empty_bar + TC_STAGES);  // bm, bn
+  uint64_t* tb_full = empty_bar + TC_STAGES;
+  uint64_t* tb_empty = tb_full + TC_TB_STAGES;
+  int* tile_smem = reinterpret_cast<int*>(tb_empty + TC_TB_STAGES);  // bm, bn
 
   const int tile_id = blockIdx.x, split = blockIdx.y;
 
@@ -275,7 +549,11 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
     tile_smem[1] = fbn;
     for (int s = 0; s < TC_STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], TC_MMA_WARPS);
+      mbar_init(&empty_bar[s], TC_TRANSPOSE_THREADS / 32 + 8);  // per warp: transposers and consumers
+    }
+    for (int b = 0; b < TC_TB_STAGES; ++b) {
+      mbar_init(&tb_full[b], TC_TRANSPOSE_THREADS);  // per thread: each orders its own stores for the async proxy
+      mbar_init(&tb_empty[b], 8);                    // per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -292,9 +570,20 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
   if (it_end > p.iters_total) it_end = p.iters_total;
   const int64_t iters = it_end > it_begin ? it_end - it_begin : 0;
 
-#define TNB_GRAM_CONSUME(NT)                                                                                    \
-  gram_tc_consume<NT>(&tmap, &tmap_b, p, stage_base, full_bar, empty_bar, it_begin, iters, nbox_a, a_box, tile_id, split, \
-                      a_col0, b_col0)
+  if (threadIdx.x < 128) {  // producer warpgroup
+    setmaxnreg_dec<TC_PRODUCER_REGS>();
+    if (threadIdx.x == 0) {
+      for (int64_t it = 0; it < iters; ++it)
+        gram_tc_produce(&tmap, &tmap_b, stage_base, full_bar, empty_bar, it, it_begin, nbox_a, nbox_b, a_col0, b_col0);
+    } else if (threadIdx.x >= 32) {
+      gram_tc_transposer(stage_base, tb_base, full_bar, empty_bar, tb_full, tb_empty, iters, nbox_b);
+    }
+    return;
+  }
+  setmaxnreg_inc<TC_CONSUMER_REGS>();
+#define TNB_GRAM_CONSUME(NT)                                                                                          \
+  gram_tc_consumer<NT>(p, stage_base, tb_base, full_bar, empty_bar, tb_full, tb_empty, iters, a_box, tile_id, split, \
+                       a_col0, b_col0)
   switch (nbox_b) {
     case 1: TNB_GRAM_CONSUME(1); break;
     case 2: TNB_GRAM_CONSUME(2); break;

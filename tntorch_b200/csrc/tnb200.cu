@@ -533,6 +533,14 @@ int tnb_measure_tf32_peak(int32_t reps, int32_t per_commit, int32_t trials, doub
   return measure_tf32_peak(reps, per_commit, trials, tflops_host, ms_host, as_stream(stream));
 }
 
+int tnb_measure_wgmma_tf32_peak(int32_t reps, int32_t per_commit, int32_t trials, double* tflops_host, double* ms_host,
+                                void* stream) {
+  TNB_TRY(require_device());
+  if (!tflops_host || reps < 1 || per_commit < 1 || trials < 1)
+    return fail(TNB_ERR_INVALID, "tnb_measure_wgmma_tf32_peak: bad argument");
+  return measure_tf32_peak(reps, per_commit, trials, tflops_host, ms_host, as_stream(stream), /*wgmma=*/true);
+}
+
 int tnb_matmul(int dtype, const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, void* stream) {
   TNB_TRY(check_dtype(dtype));
   TNB_TRY(require_device());

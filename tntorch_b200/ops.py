@@ -71,6 +71,13 @@ def measure_tf32_peak(reps: int = 200, per_commit: int = 64, trials: int = 5):
     return float(tf[0]), float(ms[0])
 
 
+def measure_wgmma_tf32_peak(reps: int = 64, per_commit: int = 64, trials: int = 5):
+    """Dense TF32 wgmma (m64n256k8, A from registers) peak of the current GPU in TFLOP/s (csrc/peak_tf32.cuh)."""
+    tf, ms = (C.c_double * 1)(), (C.c_double * 1)()
+    check(lib().tnb_measure_wgmma_tf32_peak(int(reps), int(per_commit), int(trials), tf, ms, _stream()))
+    return float(tf[0]), float(ms[0])
+
+
 def has_tensorcore_path() -> bool:
     return bool(lib().tnb_has_tensorcore_path())
 
