@@ -303,6 +303,12 @@ int tnb_gram(int dtype, const void* A, int64_t rows, int64_t n, double* G, void*
 size_t tnb_gram_tc_workspace_bytes(int64_t rows, int64_t n);
 int tnb_gram_tc_f32(const float* A, int64_t rows, int64_t n, double* G, void* workspace, size_t workspace_bytes,
                     void* stream);
+/* The same Gram of A stored K-blocked: element (k, c) of the rows x n matrix at
+ * (((k / 8 * n / 8 + c / 8) * 2 + k % 8 / 4) * 8 + c % 8) * 4 + k % 4, the layout the speculative sweep uses for a carry
+ * whose Gram has n >= 256 (both wgmma operands then load K-major, no shared-memory transpose).  n >= 256, n % 8 == 0,
+ * rows % 8 == 0; workspace from tnb_gram_tc_workspace_bytes. */
+int tnb_gram_tc_kblocked_f32(const float* A, int64_t rows, int64_t n, double* G, void* workspace, size_t workspace_bytes,
+                             void* stream);
 /* C (m x n) = alpha * A^T B + beta * D on the same tensor-core kernel (A: K x m, B: K x n, row-major fp32, TF32
  * operands, fp32 accumulation; m, n multiples of 4, >= 32).  The Chebyshev-filter products G*Y of
  * tnb_eig_topk's subspace iteration run through this entry (G symmetric => A = G).  D may be NULL. */
@@ -328,6 +334,14 @@ int tnb_project(int dtype, const void* A, int64_t rows, int64_t n, const void* V
 size_t tnb_project_tc_workspace_bytes(int64_t n, int32_t r);
 int tnb_project_tc_f32(const float* A, int64_t rows, int64_t n, const float* V, int32_t r, float* C, void* workspace,
                        size_t workspace_bytes, void* stream);
+/* The same products with C written K-blocked as the (rows / inner) x (inner * r) matrix whose row a is rows
+ * a * inner .. a * inner + inner - 1 of C (inner % 16 == 0, rows % (8 * inner) == 0, r % 16 == 0, r <= 48), and with A read
+ * K-blocked (rows % 8 == 0, n % 8 == 0; C row-major).  The K-blocked layout is that of tnb_gram_tc_kblocked_f32.  Each element of C
+ * is the same sum as tnb_project_tc_f32's. */
+int tnb_project_tc_kblocked_out_f32(const float* A, int64_t rows, int64_t n, const float* V, int32_t r, int64_t inner,
+                                    float* C, void* workspace, size_t workspace_bytes, void* stream);
+int tnb_project_tc_kblocked_in_f32(const float* A, int64_t rows, int64_t n, const float* V, int32_t r, float* C,
+                                   void* workspace, size_t workspace_bytes, void* stream);
 /* Symmetric eigendecomposition of a PSD matrix G (n x n fp64): all eigenpairs by one-CTA parallel
  * Jacobi (n <= 256), eigenvalues descending in w, eigenvectors in the columns of V (row-major n x n).
  * Replaces: torch.linalg.eigh round.py:114 / the U,S of torch.linalg.svd round.py:96. */

@@ -6,7 +6,8 @@ input, and the TF32 noise floor of their Gram kernels.
 OTHER_TREE is a second checkout with its library already built (e.g. the parent commit).  Every bench.py run is a fresh
 process; the JSON written to DIR/ab_gram.json holds, per run, value, ms_per_step, phases_ms.gram_ms, the roofline,
 sweep_roofline.single_call_ms and run.speculative_sweeps_accepted, plus the card's name and power limit.  Gram noise:
-||G_tf32 - (1 - c) G_fp64||_2 / ||G_fp64||_2 on randn(262144, 2048), c the least-squares truncation bias.
+||G_tf32 - (1 - c) G_fp64||_2 / ||G_fp64||_2 on randn(262144, 2048), c the least-squares truncation bias, for the
+row-major Gram and, where the build has it, the Gram of the same matrix stored K-blocked.
 """
 import argparse
 import json
@@ -26,14 +27,20 @@ def gram_noise(tree):
 
     g = torch.Generator(device="cuda").manual_seed(5)
     A = torch.randn(262144, 2048, generator=g, device="cuda", dtype=torch.float32)
-    G = ops.gram(A, tensorcore=True)
+    grams = {"rowmajor": ops.gram(A, tensorcore=True)}
+    if hasattr(ops, "gram_kblocked"):
+        grams["kblocked"] = ops.gram_kblocked(ops.to_kblocked(A), *A.shape)
     A64 = A.double()
     ref = A64.T @ A64
     del A64
-    c = 1.0 - float((G * ref).sum() / (ref * ref).sum())
-    E = G - (1.0 - c) * ref
-    noise = float(torch.linalg.matrix_norm(E, ord=2) / torch.linalg.matrix_norm(ref, ord=2))
-    return {"tree": tree, "bias_c": c, "noise_rel_2norm": noise}
+    out = {"tree": tree}
+    for k, G in grams.items():
+        c = 1.0 - float((G * ref).sum() / (ref * ref).sum())
+        E = G - (1.0 - c) * ref
+        noise = float(torch.linalg.matrix_norm(E, ord=2) / torch.linalg.matrix_norm(ref, ord=2))
+        out.update({"bias_c" if k == "rowmajor" else f"bias_c_{k}": c,
+                    "noise_rel_2norm" if k == "rowmajor" else f"noise_rel_2norm_{k}": noise})
+    return out
 
 
 def bench(tree, args, dump):
@@ -45,6 +52,7 @@ def bench(tree, args, dump):
     res = json.loads([line for line in out.stdout.splitlines() if line.startswith("{")][-1])
     ph = res.get("phases_ms", {})
     return {"value": res["value"], "ms_per_step": res.get("ms_per_step"), "gram_ms": ph.get("gram_ms"),
+            "factor_ms": ph.get("factor_ms"),
             "roofline": res.get("roofline"), "single_call_ms": res.get("sweep_roofline", {}).get("single_call_ms"),
             "speculative_sweeps_accepted": res.get("run", {}).get("speculative_sweeps_accepted"),
             "ranks": res.get("run", {}).get("ranks"), "rel_error": res.get("rel_error"),
@@ -82,6 +90,7 @@ def main():
     ap.add_argument("--out", required=True, help="directory for ab_gram.json and the dumped cores of both builds")
     args = ap.parse_args()
     other = os.path.abspath(args.other)
+    args.out = os.path.abspath(args.out)  # bench.py runs in each tree's directory
     os.makedirs(args.out, exist_ok=True)
     smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv"],
                          capture_output=True, text=True).stdout.strip()
@@ -91,7 +100,8 @@ def main():
         for k, tree in trees.items():
             r = bench(tree, args, os.path.join(args.out, f"dump_{k}"))
             runs[k].append(r)
-            print(k, i, json.dumps({x: r[x] for x in ("value", "ms_per_step", "gram_ms", "single_call_ms")}), flush=True)
+            print(k, i, json.dumps({x: r[x] for x in ("value", "ms_per_step", "gram_ms", "factor_ms", "single_call_ms")}),
+                  flush=True)
     noise = {}
     for k, tree in trees.items():
         out = subprocess.run([sys.executable, os.path.abspath(__file__), "--noise", tree], capture_output=True, text=True)
@@ -101,7 +111,9 @@ def main():
         v = [r["value"] for r in runs[k]]
         summary[k] = {"median_value": statistics.median(v), "spread": max(v) - min(v),
                       "median_gram_ms": [statistics.median(r["gram_ms"][j] for r in runs[k]) for j in range(2)]
-                      if runs[k][0]["gram_ms"] else None}
+                      if runs[k][0]["gram_ms"] else None,
+                      "median_factor_ms": [statistics.median(r["factor_ms"][j] for r in runs[k]) for j in range(2)]
+                      if runs[k][0]["factor_ms"] else None}
     result = {"nvidia_smi": smi, "runs": runs, "summary": summary, "noise": noise,
               "dumps": compare_dumps(os.path.join(args.out, "dump_other"), os.path.join(args.out, "dump_this"))}
     json.dump(result, open(os.path.join(args.out, "ab_gram.json"), "w"), indent=1)

@@ -92,6 +92,7 @@ SIGNATURES = {
     "tnb_gram": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, _vp, C.c_size_t, _vp]),
     "tnb_gram_tc_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
     "tnb_gram_tc_f32": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, _vp, C.c_size_t, _vp]),
+    "tnb_gram_tc_kblocked_f32": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, _vp, C.c_size_t, _vp]),
     "tnb_atb_tc_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int64]),
     "tnb_atb_tc_f32": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, C.c_int64, _vp, C.c_float, _vp, C.c_float, _vp,
                                  C.c_size_t, _vp]),
@@ -101,6 +102,9 @@ SIGNATURES = {
     "tnb_project": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int32, _vp, _vp]),
     "tnb_project_tc_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int32]),
     "tnb_project_tc_f32": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, C.c_int32, _vp, _vp, C.c_size_t, _vp]),
+    "tnb_project_tc_kblocked_out_f32": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, C.c_int32, C.c_int64, _vp, _vp,
+                                                  C.c_size_t, _vp]),
+    "tnb_project_tc_kblocked_in_f32": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, C.c_int32, _vp, _vp, C.c_size_t, _vp]),
     "tnb_eigh_workspace_bytes": (C.c_size_t, [C.c_int32]),
     "tnb_eigh_jacobi": (C.c_int, [_vp, C.c_int32, _vp, _vp, _vp, C.c_size_t, _vp]),
     "tnb_eig_topk_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),

@@ -17,6 +17,13 @@
 // wgmma.mma_async m64n{tn}k8 .f32.tf32.tf32 with A from registers, accumulating in registers.  setmaxnreg moves the
 // register file to the consumers (TC_CONSUMER_REGS: 128 accumulators plus two stages of A fragments).
 //
+// K-blocked mode (gram_tc_f32(..., kblocked)): C is stored as wgmma's K-major core matrices, [rows/8][n/8][2][8][4]:
+// element (k, c) at (((k/8 * n/8 + c/8) * 2 + k%8/4) * 8 + c%8) * 4 + k%4, the layout the sweep's projection writes for
+// the next step.  Each 8 x 4 core matrix is 128 contiguous bytes and the 8 rows of a k8 step over 256 columns are one
+// contiguous 8 KB run, so TMA loads both operands (256-byte lines, no swizzle) straight into the layout tf32 wgmma reads
+// from shared memory: no transposers, A and B through descriptors, and the freed shared memory holds a
+// TC_BLK_STAGES-deep slab ring.  The 8 rows each k8 step sums are the same 8 rows as in the row-major mode.
+//
 // Replaces, for large fp32 unfoldings, the QR of tensor.py:1816 / the Gram of round.py:104-110.
 #pragma once
 #include <cuda.h>
@@ -38,8 +45,10 @@ constexpr int TC_TRANSPOSE_THREADS = 96;        // producer warps 1-3
 constexpr int TC_THREADS = 384;
 constexpr int TC_PRODUCER_REGS = 40;
 constexpr int TC_CONSUMER_REGS = 232;
-constexpr int TC_SMEM_BYTES =
-    TC_STAGES * TC_STAGE_BYTES + TC_TB_STAGES * TC_TB_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+constexpr int TC_RING_BYTES = TC_STAGES * TC_STAGE_BYTES + TC_TB_STAGES * TC_TB_BYTES;
+constexpr int TC_SMEM_BYTES = TC_RING_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+constexpr int TC_BLK_STAGES = 4;                // slab ring depth of the K-blocked mode (no transposed-B buffers)
+static_assert(TC_BLK_STAGES * TC_STAGE_BYTES <= TC_RING_BYTES, "K-blocked ring must fit the row-major mode's buffers");
 // Longest run of rows one CTA accumulates in fp32 registers (512 stages = 16384 rows).  The diagonal of a Gram grows with
 // the row count while the rounding error of an fp32 sum grows faster; 16384-row partial sums keep that error well below
 // the TF32 operand noise the accept rule of the sweep budgets for.
@@ -129,6 +138,13 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
       : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int c0, int c1, int c2) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
+      :
+      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
+      : "memory");
+}
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
   asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -173,6 +189,11 @@ __device__ __forceinline__ void mma_frag_b_mn(const unsigned char* base, int k0,
 __device__ __forceinline__ uint64_t wgmma_desc_kmajor_sw128(const void* p) {
   return (uint64_t)((smem_u32(p) & 0x3FFFFu) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) |
          ((uint64_t)1 << 62);
+}
+// K-major operand without swizzle: 8 x 16-byte core matrices of 128 contiguous bytes, the two of a k8 step 128 bytes
+// apart (leading byte offset), 8-row groups 256 bytes apart along M/N (stride byte offset).
+__device__ __forceinline__ uint64_t wgmma_desc_kmajor_core(const void* p) {
+  return (uint64_t)((smem_u32(p) & 0x3FFFFu) >> 4) | ((uint64_t)(128 >> 4) << 16) | ((uint64_t)(256 >> 4) << 32);
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -366,24 +387,63 @@ __device__ __forceinline__ void wgmma_tf32<8>(float (&d)[128], const uint32_t (&
         "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
 }
+// The same m64n256k8 with A read from shared memory through `desc_a` as well (K-blocked mode).
+__device__ __forceinline__ void wgmma_tf32_ss(float (&d)[128], uint64_t desc_a, uint64_t desc_b) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63,"
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79,"
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95,"
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111,"
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, 1, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(desc_a), "l"(desc_b));
+}
 
 // ---------------------------------------------------------------------------------------------
 // The kernel
 // ---------------------------------------------------------------------------------------------
 // Loads of pipeline iteration `it` (rows it_begin + it) into its ring slot, once the transposers and the consumers have
-// released it.
+// released it.  B first (slots 0..nbox_b), then A (slots 8..11).  Row-major: boxes of 32 columns.  K-blocked: one box
+// of (64, tn / 8 column groups, 4 row groups) for B and one of (64, 16, 4) for A, i.e. four k8 slices of tn (128)
+// columns x 32 bytes.
+template <bool BLOCKED>
 __device__ __forceinline__ void gram_tc_produce(const CUtensorMap* tmap, const CUtensorMap* tmap_b, unsigned char* stage_base,
                                                 uint64_t* full_bar, uint64_t* empty_bar, int64_t it, int64_t it_begin,
                                                 int nbox_a, int nbox_b, int a_col0, int b_col0) {
-  const int stage = (int)(it % TC_STAGES);
-  const uint32_t phase = (uint32_t)(it / TC_STAGES) & 1u;
+  constexpr int STAGES = BLOCKED ? TC_BLK_STAGES : TC_STAGES;
+  const int stage = (int)(it % STAGES);
+  const uint32_t phase = (uint32_t)(it / STAGES) & 1u;
   mbar_wait_quiet(&empty_bar[stage], phase ^ 1u);
   unsigned char* sb = stage_base + stage * TC_STAGE_BYTES;
   mbar_expect_tx(&full_bar[stage], (uint32_t)(nbox_a + nbox_b) * TC_BOX_BYTES);
   const int row0 = (int)((it_begin + it) * TC_KC);
-  // B boxes first (slots 0..nbox_b), then A boxes (slots 8..11)
-  for (int j = 0; j < nbox_b; ++j) tma_load_2d(sb + j * TC_BOX_BYTES, tmap_b, &full_bar[stage], b_col0 + 32 * j, row0);
-  for (int j = 0; j < nbox_a; ++j) tma_load_2d(sb + (8 + j) * TC_BOX_BYTES, tmap, &full_bar[stage], a_col0 + 32 * j, row0);
+  if constexpr (BLOCKED) {
+    tma_load_3d(sb, tmap_b, &full_bar[stage], 0, b_col0 / 8, row0 / 8);
+    if (nbox_a) tma_load_3d(sb + 8 * TC_BOX_BYTES, tmap, &full_bar[stage], 0, a_col0 / 8, row0 / 8);
+  } else {
+    for (int j = 0; j < nbox_b; ++j) tma_load_2d(sb + j * TC_BOX_BYTES, tmap_b, &full_bar[stage], b_col0 + 32 * j, row0);
+    for (int j = 0; j < nbox_a; ++j) tma_load_2d(sb + (8 + j) * TC_BOX_BYTES, tmap, &full_bar[stage], a_col0 + 32 * j, row0);
+  }
 }
 
 // Transposes the nbox B boxes of a slab stage into the K-major buffer tb: element (row k, column c) of box j, at
@@ -430,6 +490,10 @@ __device__ __forceinline__ void gram_tc_transposer(unsigned char* stage_base, un
   }
 }
 
+template <int NT>
+__device__ __forceinline__ void gram_tc_epilogue(const GramTcParams& p, const float (&acc)[NT * 16], int cm, int lane,
+                                                 int tile_id, int split, int a_col0, int b_col0);
+
 // One pipeline stage of a consumer warp: A fragments of stage `it` into `af`, four k8 wgmma into `acc`, then release
 // the slab slot and, once the previous stage's group has completed, its transposed-B buffer.
 template <int NT>
@@ -463,7 +527,6 @@ __device__ __forceinline__ void gram_tc_consumer(const GramTcParams& p, const un
                                                  int tile_id, int split, int a_col0, int b_col0) {
   const int ct = threadIdx.x - 128;
   const int lane = ct & 31, w = (ct >> 5) & 3;
-  const int g = lane >> 2, t = lane & 3;
   const int cm = 64 * (ct >> 7) + 16 * w;  // first of this warp's 16 rows of the tile
   float acc[NT * 16];
 #pragma unroll
@@ -483,8 +546,46 @@ __device__ __forceinline__ void gram_tc_consumer(const GramTcParams& p, const un
   }
   wgmma_wait<0>();
   wgmma_fence_operand(acc);
+  gram_tc_epilogue<NT>(p, acc, cm, lane, tile_id, split, a_col0, b_col0);
+}
 
-  // epilogue: acc[4j + 2h + e] is (row cm + g + 8h, column 8j + 2t + e) of the 128 x tn tile
+// Consumer warpgroup cw of the K-blocked mode (tn = 256): both operands through descriptors of the stage's k8 slices.  B slice kk is at kk * 8 KB; A (this warpgroup's 64 rows) at a_off + kk * a_slice + 64 * cw rows.  A slot is
+// released once the wgmma group that read it has completed, i.e. one stage later.
+__device__ __forceinline__ void gram_tc_consumer_blocked(const GramTcParams& p, const unsigned char* stage_base,
+                                                         uint64_t* full_bar, uint64_t* empty_bar, int64_t iters,
+                                                         int a_off, int a_slice, int tile_id, int split, int a_col0,
+                                                         int b_col0) {
+  const int ct = threadIdx.x - 128;
+  const int lane = ct & 31, w = (ct >> 5) & 3, cw = ct >> 7;
+  const int cm = 64 * cw + 16 * w;
+  float acc[128];
+#pragma unroll
+  for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+  wgmma_fence_operand(acc);
+  for (int64_t it = 0; it < iters; ++it) {
+    const int s = (int)(it % TC_BLK_STAGES);
+    mbar_wait_spin(&full_bar[s], (uint32_t)(it / TC_BLK_STAGES) & 1u);
+    const unsigned char* sb = stage_base + s * TC_STAGE_BYTES;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < TC_KC / 8; ++kk)
+      wgmma_tf32_ss(acc, wgmma_desc_kmajor_core(sb + a_off + kk * a_slice + 64 * cw * 32),
+                    wgmma_desc_kmajor_core(sb + kk * 256 * 32));
+    wgmma_commit();
+    wgmma_wait<1>();
+    __syncwarp();
+    if (it > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % TC_BLK_STAGES]);
+  }
+  wgmma_wait<0>();
+  wgmma_fence_operand(acc);
+  gram_tc_epilogue<8>(p, acc, cm, lane, tile_id, split, a_col0, b_col0);
+}
+
+// Output of one consumer warp: acc[4j + 2h + e] is (row cm + g + 8h, column 8j + 2t + e) of the 128 x tn tile.
+template <int NT>
+__device__ __forceinline__ void gram_tc_epilogue(const GramTcParams& p, const float (&acc)[NT * 16], int cm, int lane,
+                                                 int tile_id, int split, int a_col0, int b_col0) {
+  const int g = lane >> 2, t = lane & 3;
   if (p.direct) {
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
@@ -514,6 +615,9 @@ __device__ __forceinline__ void gram_tc_consumer(const GramTcParams& p, const un
   }
 }
 
+// BLOCKED: the operands are K-blocked (see the top of the file); tmap / tmap_b are 3-D maps with boxes (64, 16, 4) and
+// (64, 32, 4).  Otherwise row-major, 2-D maps with boxes of 32 columns x TC_KC rows.
+template <bool BLOCKED>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_b,
                const GramTcParams p) {
@@ -522,10 +626,10 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
   const uint32_t raw_addr = smem_u32(tc_smem_raw);
   const uint32_t pad = (1024u - (raw_addr & 1023u)) & 1023u;
   unsigned char* stage_base = tc_smem_raw + pad;
-  unsigned char* tb_base = stage_base + TC_STAGES * TC_STAGE_BYTES;
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(tb_base + TC_TB_STAGES * TC_TB_BYTES);
-  uint64_t* empty_bar = full_bar + TC_STAGES;
-  uint64_t* tb_full = empty_bar + TC_STAGES;
+  unsigned char* tb_base = stage_base + TC_STAGES * TC_STAGE_BYTES;  // row-major mode only
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stage_base + TC_RING_BYTES);
+  uint64_t* empty_bar = full_bar + TC_BLK_STAGES;
+  uint64_t* tb_full = empty_bar + TC_BLK_STAGES;
   uint64_t* tb_empty = tb_full + TC_TB_STAGES;
   int* tile_smem = reinterpret_cast<int*>(tb_empty + TC_TB_STAGES);  // bm, bn
 
@@ -547,9 +651,10 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
     }
     tile_smem[0] = fbm;
     tile_smem[1] = fbn;
-    for (int s = 0; s < TC_STAGES; ++s) {
+    for (int s = 0; s < (BLOCKED ? TC_BLK_STAGES : TC_STAGES); ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], TC_TRANSPOSE_THREADS / 32 + 8);  // per warp: transposers and consumers
+      // per warp: transposers and consumers (K-blocked: consumers only)
+      mbar_init(&empty_bar[s], (BLOCKED ? 0 : TC_TRANSPOSE_THREADS / 32) + 8);
     }
     for (int b = 0; b < TC_TB_STAGES; ++b) {
       mbar_init(&tb_full[b], TC_TRANSPOSE_THREADS);  // per thread: each orders its own stores for the async proxy
@@ -574,13 +679,20 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
     setmaxnreg_dec<TC_PRODUCER_REGS>();
     if (threadIdx.x == 0) {
       for (int64_t it = 0; it < iters; ++it)
-        gram_tc_produce(&tmap, &tmap_b, stage_base, full_bar, empty_bar, it, it_begin, nbox_a, nbox_b, a_col0, b_col0);
-    } else if (threadIdx.x >= 32) {
+        gram_tc_produce<BLOCKED>(&tmap, &tmap_b, stage_base, full_bar, empty_bar, it, it_begin, nbox_a, nbox_b, a_col0,
+                                 b_col0);
+    } else if (!BLOCKED && threadIdx.x >= 32) {
       gram_tc_transposer(stage_base, tb_base, full_bar, empty_bar, tb_full, tb_empty, iters, nbox_b);
     }
     return;
   }
   setmaxnreg_inc<TC_CONSUMER_REGS>();
+  if constexpr (BLOCKED) {  // tn == 256; A inside B: its k8 slices are rows of B's (8 KB apart), else 128-row slices in slot 8
+    gram_tc_consumer_blocked(p, stage_base, full_bar, empty_bar, iters,
+                             a_in_b ? (a_col0 - b_col0) * 32 : 8 * TC_BOX_BYTES, a_in_b ? 256 * 32 : 128 * 32, tile_id,
+                             split, a_col0, b_col0);
+    return;
+  } else {
 #define TNB_GRAM_CONSUME(NT)                                                                                          \
   gram_tc_consumer<NT>(p, stage_base, tb_base, full_bar, empty_bar, tb_full, tb_empty, iters, a_box, tile_id, split, \
                        a_col0, b_col0)
@@ -595,6 +707,7 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
     default: TNB_GRAM_CONSUME(8); break;
   }
 #undef TNB_GRAM_CONSUME
+  }
 }
 
 // Sum the split-K partial tiles in fp64 (fixed order), mirror to the lower triangle.
@@ -745,14 +858,34 @@ inline int encode_rowmajor_f32(CUtensorMap* tmap, const float* ptr, int64_t rows
   return TNB_OK;
 }
 
-// G (n x n fp64) and optionally Gf (fp32 copy) = A^T A, A: rows x n fp32 row-major (device).
+// 3-D map over a K-blocked matrix (64 floats per 8 rows x 8 columns, cols / 8 column groups, rows / 8 row groups):
+// box (64, box_cols / 8, TC_KC / 8) lands in shared memory as TC_KC / 8 k8 slices of box_cols columns x 32 bytes.
+inline int encode_kblocked_f32(CUtensorMap* tmap, const float* ptr, int64_t rows, int64_t cols, int box_cols) {
+  cuuint64_t gdim[3] = {64, (cuuint64_t)(cols / 8), (cuuint64_t)(rows / 8)};
+  cuuint64_t gstride[2] = {64 * sizeof(float), (cuuint64_t)cols * 8 * sizeof(float)};
+  cuuint32_t box[3] = {64, (cuuint32_t)box_cols / 8, TC_KC / 8};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult cr = get_encode_tiled()(tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(ptr), gdim, gstride, box,
+                                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (cr != CUDA_SUCCESS) return fail(TNB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)cr);
+  return TNB_OK;
+}
+
+inline bool gram_tc_kblocked_shape_ok(int64_t rows, int64_t n) {
+  return gram_tc_shape_ok(rows, n) && n >= 256 && n % 8 == 0 && rows % 8 == 0;
+}
+
+// G (n x n fp64) and optionally Gf (fp32 copy) = A^T A, A: rows x n fp32 (device), row-major or, with kblocked, stored
+// K-blocked (then n >= 256, n % 8 == 0 and rows % 8 == 0).
 inline int gram_tc_f32(const float* A, int64_t rows, int64_t n, double* G, float* Gf, void* ws, size_t ws_bytes,
-                       cudaStream_t st) {
+                       cudaStream_t st, bool kblocked = false) {
   if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "gram_tc: TMA tensor-core path needs an sm_90 device");
-  if (!gram_tc_shape_ok(rows, n)) return fail(TNB_ERR_UNSUPPORTED, "gram_tc: unsupported shape rows=%lld n=%lld", (long long)rows, (long long)n);
+  if (!(kblocked ? gram_tc_kblocked_shape_ok(rows, n) : gram_tc_shape_ok(rows, n)))
+    return fail(TNB_ERR_UNSUPPORTED, "gram_tc: unsupported shape rows=%lld n=%lld", (long long)rows, (long long)n);
   if ((reinterpret_cast<uintptr_t>(A) & 15u) != 0) return fail(TNB_ERR_INVALID, "gram_tc: input must be 16-byte aligned");
   GramTcParams p;
-  const int fold = gram_tc_fold(rows, n);
+  const int fold = gram_tc_fold(rows, n);  // 1 for n >= 128
   const int64_t n_in = n;
   rows /= fold;
   n *= fold;
@@ -763,13 +896,21 @@ inline int gram_tc_f32(const float* A, int64_t rows, int64_t n, double* G, float
   if (ws_bytes < need) return fail(TNB_ERR_WORKSPACE, "gram_tc: workspace %zu < %zu", ws_bytes, need);
   p.partial = static_cast<float*>(ws);
 
-  CUtensorMap tmap;
-  TNB_TRY(encode_rowmajor_f32(&tmap, A, rows, n));
-
-  static PerDeviceFlag attr_done;
-  TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel, TC_SMEM_BYTES));
   dim3 grid((unsigned)p.num_tiles, (unsigned)p.ksplit);
-  gram_tc_kernel<<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(tmap, tmap, p);
+  if (kblocked) {
+    CUtensorMap ta, tb;
+    TNB_TRY(encode_kblocked_f32(&ta, A, rows, n, 128));
+    TNB_TRY(encode_kblocked_f32(&tb, A, rows, n, 256));
+    static PerDeviceFlag attr_done;
+    TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel<true>, TC_SMEM_BYTES));
+    gram_tc_kernel<true><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(ta, tb, p);
+  } else {
+    CUtensorMap tmap;
+    TNB_TRY(encode_rowmajor_f32(&tmap, A, rows, n));
+    static PerDeviceFlag attr_done;
+    TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel<false>, TC_SMEM_BYTES));
+    gram_tc_kernel<false><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(tmap, tmap, p);
+  }
   TNB_LAUNCH_CHECK();
   const int64_t total = n_in * n_in * (p.fold > 1 ? 32 : 1);  // folded form: one warp per element
   gram_tc_finalize_kernel<<<(unsigned)std::min<int64_t>((total + 255) / 256, 4096), 256, 0, st>>>(p, G, Gf);
@@ -835,9 +976,9 @@ inline int atb_tc_f32(const float* A, int64_t K, int64_t m, const float* B, int6
   TNB_TRY(encode_rowmajor_f32(&ta, A, K, m));
   TNB_TRY(encode_rowmajor_f32(&tb, B, K, n));
   static PerDeviceFlag attr_done;
-  TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel, TC_SMEM_BYTES));
+  TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel<false>, TC_SMEM_BYTES));
   dim3 grid((unsigned)p.num_tiles, (unsigned)p.ksplit);
-  gram_tc_kernel<<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(ta, tb, p);
+  gram_tc_kernel<false><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(ta, tb, p);
   TNB_LAUNCH_CHECK();
   if (narrow) return TNB_OK;
   const int64_t total = m * n;

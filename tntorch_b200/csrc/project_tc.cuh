@@ -11,6 +11,14 @@
 //     issue the three products per 8-wide k-step with mma.sync m16n8k8 .tf32; every 32-wide chunk is folded into an
 //     fp32 running sum so that the accumulation error does not grow with K;
 //   * persistent CTAs, static round-robin over row blocks; each warp stores its 16 x r piece of C from registers.
+//
+// Two more layouts serve the K-blocked carry of the sweep (the next step's matrix M, rows' x n', stored as wgmma's K-major
+// core matrices [rows'/8][n'/8][2][8][4] so that its Gram loads K-major operands, gram_tc.cuh):
+//   * PT_OUT_KBLOCKED writes C in that layout.  C's row a * inner + i is row a of M, columns i * r .. i * r + r - 1.  A
+//     row block is 8 a's x 16 i's (warp w: a0 + w) loaded by a 3-D map as the same 128 x 32 swizzled tile, so the
+//     products are unchanged; its output is one contiguous 16 x r x 8 run of the carry, staged through shared memory past
+//     the ring (the ring keeps its depth) and stored with 16-byte writes.
+//   * PT_IN_KBLOCKED reads A in that layout (a 1 KB run per 8 rows and 32 columns, no swizzle) and writes C row-major.
 #pragma once
 #include "gram_tc.cuh"
 
@@ -20,8 +28,10 @@ constexpr int PT_BM = 128, PT_KC = 32, PT_MAX_STAGES = 12, PT_MMA_WARPS = 8, PT_
 constexpr int PT_A_BYTES = PT_BM * PT_KC * 4;      // 16 KB
 constexpr int PT_MAX_N = 64;                        // r padded to a multiple of 16, <= 64
 constexpr int PT_RING_BYTES = 192 * 1024;           // stage ring (+ resident V when it fits)
-constexpr int PT_SMEM_BYTES = PT_RING_BYTES + 1024 + 256;
+constexpr int PT_STG_MAX_BYTES = 29 * 1024;         // PT_OUT_KBLOCKED output staging (r <= 48), past the ring
+constexpr int PT_SMEM_BYTES = PT_RING_BYTES + PT_STG_MAX_BYTES + 1024 + 256;
 constexpr int PT_VRES_MAX_BYTES = 32 * 1024;        // V_hi|V_lo kept in shared memory for the whole kernel up to this size
+constexpr int PT_ROWMAJOR = 0, PT_OUT_KBLOCKED = 1, PT_IN_KBLOCKED = 2;
 
 struct ProjTcParams {
   int64_t rows;
@@ -34,7 +44,24 @@ struct ProjTcParams {
   int stage_bytes;  // 16 KB (+ 2*npad*128 B of V chunk when streaming V)
   int nstages;      // ring depth that fits PT_RING_BYTES: the HBM latency needs >= ~140 KB in flight per SM
   float* C;
+  int inner16;      // PT_OUT_KBLOCKED: inner / 16 row blocks per 8 rows of M
+  int64_t out_ld;   // PT_OUT_KBLOCKED: n' = inner * r
 };
+
+// element (row m, column k) of a 128 x 32 tile of a K-blocked matrix: 16 runs of 32 columns x 8 rows, each four 8 x 8
+// blocks of two 4-row core matrices (column-minor)
+__device__ __forceinline__ uint32_t kb_ld(const unsigned char* base, int m, int k) {
+  return *reinterpret_cast<const uint32_t*>(
+      base + (((m >> 3) << 8) + (((((k >> 3) << 1) + ((m & 7) >> 2)) << 5) + ((k & 7) << 2) + (m & 3)) << 2));
+}
+// Staging of a PT_OUT_KBLOCKED tile: warp w's 16 x R piece at w * SW + row * RS + column.  RS = R + 8 makes the float2
+// stores of each half-warp conflict-free, SW = 16 RS + 4 (4 SW = 16 mod 32 banks) the gathers of the copy-out.
+template <int R>
+struct PtStage {
+  static constexpr int RS = R + 8, SW = 16 * RS + 4;
+  static_assert(8 * SW * 4 <= PT_STG_MAX_BYTES, "staging must fit past the ring");
+};
+
 
 // element (row m, column k) of a K-major tile of 32 fp32 columns written by TMA with SWIZZLE_128B
 __device__ __forceinline__ uint32_t km_ld(const unsigned char* base, int m, int k) {
@@ -42,10 +69,10 @@ __device__ __forceinline__ uint32_t km_ld(const unsigned char* base, int m, int 
 }
 
 // NT = npad / 8 n8 tiles
-template <int NT>
+template <int NT, int MODE>
 __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const unsigned char* stage_base,
-                                                   const unsigned char* v_res, uint64_t* full_bar, uint64_t* empty_bar,
-                                                   uint64_t* v_bar, int64_t total_items) {
+                                                   const unsigned char* v_res, float* stg, uint64_t* full_bar,
+                                                   uint64_t* empty_bar, uint64_t* v_bar, int64_t total_items) {
   const int w = (threadIdx.x >> 5) - 1, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
   const int m0 = 16 * w;
@@ -59,7 +86,7 @@ __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const 
     for (int e = 0; e < 4; ++e) out[j][e] = 0.f;
   int stage = 0, kc = 0;
   uint32_t phase = 0;
-  int64_t row0 = (int64_t)blockIdx.x * PT_BM;
+  int64_t rb = blockIdx.x;
   for (int64_t item = 0; item < total_items; ++item) {
     mbar_wait(&full_bar[stage], phase);
     const unsigned char* sa = stage_base + (size_t)stage * p.stage_bytes;
@@ -73,10 +100,17 @@ __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const 
 #pragma unroll
     for (int ks = 0; ks < PT_KC; ks += 8) {
       uint32_t a[4], lo[4];
-      a[0] = km_ld(sa, m0 + g, ks + t);
-      a[1] = km_ld(sa, m0 + g + 8, ks + t);
-      a[2] = km_ld(sa, m0 + g, ks + t + 4);
-      a[3] = km_ld(sa, m0 + g + 8, ks + t + 4);
+      if constexpr (MODE == PT_IN_KBLOCKED) {
+        a[0] = kb_ld(sa, m0 + g, ks + t);
+        a[1] = kb_ld(sa, m0 + g + 8, ks + t);
+        a[2] = kb_ld(sa, m0 + g, ks + t + 4);
+        a[3] = kb_ld(sa, m0 + g + 8, ks + t + 4);
+      } else {
+        a[0] = km_ld(sa, m0 + g, ks + t);
+        a[1] = km_ld(sa, m0 + g + 8, ks + t);
+        a[2] = km_ld(sa, m0 + g, ks + t + 4);
+        a[3] = km_ld(sa, m0 + g + 8, ks + t + 4);
+      }
 #pragma unroll
       for (int i = 0; i < 4; ++i)
         lo[i] = __float_as_uint(__uint_as_float(a[i]) - __uint_as_float(a[i] & 0xFFFFE000u));
@@ -99,6 +133,26 @@ __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const 
     if (++kc < p.nk) continue;
     // row block complete: rows m0+g (c0, c1) and m0+g+8 (c2, c3), columns 8j+2t, 8j+2t+1
     kc = 0;
+    if constexpr (MODE == PT_OUT_KBLOCKED) {  // r == npad
+      constexpr int R = 8 * NT, RS = PtStage<R>::RS, SW = PtStage<R>::SW;
+      asm volatile("bar.sync 1, %0;" ::"n"(PT_MMA_WARPS * 32) : "memory");  // the last copy-out has read the staging
+      float* sw = stg + w * SW;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < NT; ++j)
+          *reinterpret_cast<float2*>(sw + (g + 8 * h) * RS + 8 * j + 2 * t) = make_float2(out[j][2 * h], out[j][2 * h + 1]);
+      asm volatile("bar.sync 1, %0;" ::"n"(PT_MMA_WARPS * 32) : "memory");
+      // element (row ii of warp w, column col) is row a0 + w of M, column (i0 + ii) * R + col = (i0 * R) + pi: word
+      // ((pi / 8) * 2 + w / 4) * 32 + (pi % 8) * 4 + w % 4 of the run that starts at M row group a0 / 8, column i0 * R
+      float* dst = p.C + ((rb / p.inner16) * p.out_ld + (rb % p.inner16) * 16 * R) * 8;
+      for (int q = threadIdx.x - 32; q < 32 * R; q += PT_MMA_WARPS * 32) {
+        const int pi = ((q >> 4) << 3) + (q & 7);
+        const float* src = stg + ((q >> 3) & 1) * 4 * SW + (pi / R) * RS + pi % R;
+        *reinterpret_cast<float4*>(dst + 4 * (int64_t)q) = make_float4(src[0], src[SW], src[2 * SW], src[3 * SW]);
+      }
+    } else {
+    const int64_t row0 = rb * PT_BM;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int64_t grow = row0 + m0 + g + 8 * h;
@@ -116,14 +170,16 @@ __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const 
         }
       }
     }
+    }
 #pragma unroll
     for (int j = 0; j < NT; ++j)
 #pragma unroll
       for (int e = 0; e < 4; ++e) out[j][e] = 0.f;
-    row0 += (int64_t)gridDim.x * PT_BM;
+    rb += gridDim.x;
   }
 }
 
+template <int MODE>
 __global__ void __launch_bounds__(PT_THREADS, 1)
 project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_vhi,
                   const __grid_constant__ CUtensorMap tmap_vlo, const ProjTcParams p) {
@@ -132,7 +188,8 @@ project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   const uint32_t pad = (1024u - (raw_addr & 1023u)) & 1023u;
   unsigned char* stage_base = pt_smem_raw + pad;
   unsigned char* v_res = stage_base + (size_t)p.nstages * p.stage_bytes;   // resident V (vres): nk x [V_hi; V_lo] chunks
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stage_base + PT_RING_BYTES);
+  float* stg = reinterpret_cast<float*>(stage_base + PT_RING_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(stage_base + PT_RING_BYTES + PT_STG_MAX_BYTES);
   uint64_t* empty_bar = full_bar + PT_MAX_STAGES;
   uint64_t* v_bar = empty_bar + PT_MAX_STAGES;
   const int vchunk_bytes = 2 * p.npad * PT_KC * 4;
@@ -165,28 +222,35 @@ project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       int stage = 0;
       uint32_t phase = 0;
       int kc = 0;
-      int row0 = (int)blockIdx.x * PT_BM;           // rows < 2^31 (checked on the host)
-      const int row_step = (int)gridDim.x * PT_BM;
+      int rb = (int)blockIdx.x;           // rows < 2^31 (checked on the host)
       for (int64_t item = 0; item < total_items; ++item) {
         mbar_wait(&empty_bar[stage], phase ^ 1u);
         unsigned char* sb = stage_base + (size_t)stage * p.stage_bytes;
         mbar_expect_tx(&full_bar[stage], tx_bytes);
-        tma_load_2d(sb, &tmap_a, &full_bar[stage], kc * PT_KC, row0);
+        if (MODE == PT_OUT_KBLOCKED)
+          tma_load_3d(sb, &tmap_a, &full_bar[stage], kc * PT_KC, (rb % p.inner16) * 16, (rb / p.inner16) * 8);
+        else if (MODE == PT_IN_KBLOCKED)
+          tma_load_2d(sb, &tmap_a, &full_bar[stage], kc * PT_KC * 8, rb * (PT_BM / 8));
+        else
+          tma_load_2d(sb, &tmap_a, &full_bar[stage], kc * PT_KC, rb * PT_BM);
         if (!p.vres) {
           tma_load_2d(sb + PT_A_BYTES, &tmap_vhi, &full_bar[stage], kc * PT_KC, 0);
           tma_load_2d(sb + PT_A_BYTES + p.npad * PT_KC * 4, &tmap_vlo, &full_bar[stage], kc * PT_KC, 0);  // rows npad..2npad-1
         }
-        if (++kc == p.nk) { kc = 0; row0 += row_step; }
+        if (++kc == p.nk) { kc = 0; rb += (int)gridDim.x; }
         if (++stage == p.nstages) { stage = 0; phase ^= 1u; }
       }
     }
     return;
   }
   switch (p.npad) {
-    case 16: project_tc_consume<2>(p, stage_base, v_res, full_bar, empty_bar, v_bar, total_items); break;
-    case 32: project_tc_consume<4>(p, stage_base, v_res, full_bar, empty_bar, v_bar, total_items); break;
-    case 48: project_tc_consume<6>(p, stage_base, v_res, full_bar, empty_bar, v_bar, total_items); break;
-    default: project_tc_consume<8>(p, stage_base, v_res, full_bar, empty_bar, v_bar, total_items); break;
+    case 16: project_tc_consume<2, MODE>(p, stage_base, v_res, stg, full_bar, empty_bar, v_bar, total_items); break;
+    case 32: project_tc_consume<4, MODE>(p, stage_base, v_res, stg, full_bar, empty_bar, v_bar, total_items); break;
+    case 48: project_tc_consume<6, MODE>(p, stage_base, v_res, stg, full_bar, empty_bar, v_bar, total_items); break;
+    default:  // r <= 48 with a K-blocked output (project_tc_f32)
+      if constexpr (MODE != PT_OUT_KBLOCKED)
+        project_tc_consume<8, MODE>(p, stage_base, v_res, stg, full_bar, empty_bar, v_bar, total_items);
+      break;
   }
 }
 
@@ -227,16 +291,27 @@ inline int encode_kmajor_f32(CUtensorMap* tmap, const float* ptr, int64_t rows, 
 }
 
 // C (rows x r) = A (rows x K) V (K x r); ws: project_tc_workspace_bytes(K, r).
+//   layout PT_ROWMAJOR:     A and C row-major;
+//   layout PT_OUT_KBLOCKED: A row-major, C stored as the K-blocked (gram_tc.cuh) (rows / inner) x (inner * r) matrix;
+//                           needs inner % 16 == 0, rows % (8 * inner) == 0, r % 16 == 0, r <= 48;
+//   layout PT_IN_KBLOCKED:  A stored K-blocked (rows % 8 == 0, K % 8 == 0), C row-major.
 inline int project_tc_f32(const float* A, int64_t rows, int64_t K, const float* V, int r, float* C, void* ws, size_t ws_bytes,
-                          cudaStream_t st) {
+                          cudaStream_t st, int layout = PT_ROWMAJOR, int64_t inner = 0) {
   if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "project_tc: needs an sm_90 device");
   if (!project_tc_shape_ok(rows, K, r, A, C)) return fail(TNB_ERR_UNSUPPORTED, "project_tc: unsupported shape");
+  if (layout == PT_OUT_KBLOCKED && !(inner >= 16 && inner % 16 == 0 && rows % (8 * inner) == 0 && r % 16 == 0 && r <= 48))
+    return fail(TNB_ERR_UNSUPPORTED,
+                "project_tc: K-blocked output needs inner %% 16 == 0, rows %% (8 inner) == 0, r %% 16 == 0, r <= 48");
+  if (layout == PT_IN_KBLOCKED && (rows % 8 != 0 || K % 8 != 0))
+    return fail(TNB_ERR_UNSUPPORTED, "project_tc: K-blocked input needs rows %% 8 == 0 and K %% 8 == 0");
   if (ws_bytes < project_tc_workspace_bytes(K, r)) return fail(TNB_ERR_WORKSPACE, "project_tc: workspace too small");
   ProjTcParams p;
   p.rows = rows; p.K = (int)K; p.r = r; p.npad = (r + 15) / 16 * 16;
   p.num_row_blocks = (rows + PT_BM - 1) / PT_BM;
   p.nk = (int)((K + PT_KC - 1) / PT_KC);
   p.C = C;
+  p.inner16 = layout == PT_OUT_KBLOCKED ? (int)(inner / 16) : 1;
+  p.out_ld = layout == PT_OUT_KBLOCKED ? inner * r : 0;
   const int vchunk = 2 * p.npad * PT_KC * 4;
   p.vres = ((int64_t)p.nk * vchunk <= PT_VRES_MAX_BYTES) ? 1 : 0;
   p.stage_bytes = PT_A_BYTES + (p.vres ? 0 : vchunk);
@@ -247,14 +322,42 @@ inline int project_tc_f32(const float* A, int64_t rows, int64_t K, const float* 
   split_v_kernel<<<grid_for((int64_t)p.npad * K), 256, 0, st>>>(V, (int)K, r, p.npad, Vhi, Vlo);
   TNB_LAUNCH_CHECK();
   CUtensorMap ta, th, tl;
-  TNB_TRY(encode_kmajor_f32(&ta, A, rows, K, PT_BM));
+  CUresult cr = CUDA_SUCCESS;
+  if (layout == PT_OUT_KBLOCKED) {  // (K, inner, rows / inner), box (32, 16, 8): the 128 x 32 tile of 8 rows of M
+    cuuint64_t gdim[3] = {(cuuint64_t)K, (cuuint64_t)inner, (cuuint64_t)(rows / inner)};
+    cuuint64_t gstride[2] = {(cuuint64_t)K * sizeof(float), (cuuint64_t)(inner * K) * sizeof(float)};
+    cuuint32_t box[3] = {(cuuint32_t)PT_KC, 16, 8}, estr[3] = {1, 1, 1};
+    cr = get_encode_tiled()(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(A), gdim, gstride, box, estr,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  } else if (layout == PT_IN_KBLOCKED) {  // (8 K, rows / 8), box (8 x 32 columns, 16 row groups), no swizzle
+    cuuint64_t gdim[2] = {(cuuint64_t)(8 * K), (cuuint64_t)(rows / 8)};
+    cuuint64_t gstride[1] = {(cuuint64_t)(8 * K) * sizeof(float)};
+    cuuint32_t box[2] = {8 * PT_KC, PT_BM / 8}, estr[2] = {1, 1};
+    cr = get_encode_tiled()(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(A), gdim, gstride, box, estr,
+                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  } else {
+    TNB_TRY(encode_kmajor_f32(&ta, A, rows, K, PT_BM));
+  }
+  if (cr != CUDA_SUCCESS) return fail(TNB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)cr);
   TNB_TRY(encode_kmajor_f32(&th, Vhi, p.npad, K, p.npad));
   TNB_TRY(encode_kmajor_f32(&tl, Vlo, p.npad, K, p.npad));
-  static PerDeviceFlag attr_done;
-  TNB_CUDA(ensure_dyn_smem(attr_done, project_tc_kernel, PT_SMEM_BYTES));
   const int sms = usable_sms();
   const int64_t grid = p.num_row_blocks < sms ? p.num_row_blocks : sms;
-  project_tc_kernel<<<(unsigned)grid, PT_THREADS, PT_SMEM_BYTES, st>>>(ta, th, tl, p);
+  if (layout == PT_OUT_KBLOCKED) {
+    static PerDeviceFlag attr_done;
+    TNB_CUDA(ensure_dyn_smem(attr_done, project_tc_kernel<PT_OUT_KBLOCKED>, PT_SMEM_BYTES));
+    project_tc_kernel<PT_OUT_KBLOCKED><<<(unsigned)grid, PT_THREADS, PT_SMEM_BYTES, st>>>(ta, th, tl, p);
+  } else if (layout == PT_IN_KBLOCKED) {
+    static PerDeviceFlag attr_done;
+    TNB_CUDA(ensure_dyn_smem(attr_done, project_tc_kernel<PT_IN_KBLOCKED>, PT_SMEM_BYTES));
+    project_tc_kernel<PT_IN_KBLOCKED><<<(unsigned)grid, PT_THREADS, PT_SMEM_BYTES, st>>>(ta, th, tl, p);
+  } else {
+    static PerDeviceFlag attr_done;
+    TNB_CUDA(ensure_dyn_smem(attr_done, project_tc_kernel<PT_ROWMAJOR>, PT_SMEM_BYTES));
+    project_tc_kernel<PT_ROWMAJOR><<<(unsigned)grid, PT_THREADS, PT_SMEM_BYTES, st>>>(ta, th, tl, p);
+  }
   TNB_LAUNCH_CHECK();
   return TNB_OK;
 }

@@ -83,6 +83,24 @@ inline int make_dims(int ndim, const int64_t* shape, const int32_t* rmax, SweepD
   return TNB_OK;
 }
 
+// The carry that step mu + 1 writes and step mu reads, M (rows' x n' = d.rows[mu] x shape[mu] * rcap[mu+1]), is stored
+// K-blocked, as wgmma's K-major core matrices (gram_tc.cuh), when the speculative sweep runs both ends on kernels that have that form:
+// step mu takes the tensor-core Gram unfolded (n' >= 256) and the tensor-core projection, and step mu + 1 projects on the
+// tensor cores with an epilogue that can write it (rcap[mu+1] % 16 == 0 and <= 48, shape[mu] % 16 == 0).  Its Gram then loads
+// K-major operands directly instead of transposing every slab in shared memory.  The writer's own input must be
+// row-major, and the last carry (step mu = 0's core) stays row-major.
+template <typename T>
+inline bool carry_kblocked(const SweepDims& d, int mu, bool allow_tc) {
+  if (!std::is_same<T, float>::value || !allow_tc || mu < 1 || mu + 1 > d.N - 1) return false;
+  const int64_t rows = d.rows[mu], n = d.shape[mu] * d.rcap[mu + 1], k = std::min<int64_t>(d.rcap[mu], n);
+  const bool reader = rows >= n && rows >= std::max(TC_MIN_ROWS, PROJ_TC_MIN_ROWS) && gram_tc_kblocked_shape_ok(rows, n) &&
+                      k <= PT_MAX_N && project_tc_shape_ok(rows, n, k, nullptr, nullptr);
+  const int64_t wrows = d.rows[mu + 1], wn = d.shape[mu + 1] * d.rcap[mu + 2], r = d.rcap[mu + 1];
+  const bool writer = wrows >= wn && wrows >= PROJ_TC_MIN_ROWS && wn >= 32 && project_tc_shape_ok(wrows, wn, r, nullptr, nullptr) &&
+                      r % 16 == 0 && r <= 48 && d.shape[mu] % 16 == 0;
+  return reader && writer && !carry_kblocked<T>(d, mu + 1, allow_tc);
+}
+
 // ---------------------------------------------------------------------------------------------
 // Gram of a (rows x n) row-major matrix on whichever side is smaller, into fp64 G (L x L).
 // ---------------------------------------------------------------------------------------------
@@ -247,6 +265,7 @@ struct SweepInfo {
   int fused_filters = 0;  // Chebyshev filters run as one resident kernel (cheb_filter.cuh)
   int rr_sweeps = 0, rr_solves = 0;  // Jacobi sweeps / solves of the Rayleigh-Ritz steps (diagnostic)
   int tc_grams = 0;
+  int kblocked_steps = 0;  // steps whose Gram and projection read a K-blocked carry (carry_kblocked)
   int speculative = 0;  // 1: the sync-free sweep was accepted (one host synchronisation in total)
   int spec_flags = 0;   // why a speculative sweep was repeated on the host-driven path (spec_check_kernel bits)
   // TNB_FLAG_PROFILE: CUDA-event timings (ms) on the launching stream, per step (t = 0 is the first Gram)
@@ -419,6 +438,8 @@ struct SpecStep {
   size_t ptc_bytes = 0;
   int ldv = 0, b = 0, used_tc = 0;
   bool chfsi = false, tc_gram = false;
+  bool in_kblocked = false;   // C is K-blocked (carry_kblocked of this step)
+  int64_t out_inner = 0;      // > 0: write Cn K-blocked for the next step, whose rows hold out_inner rows of Cn each
   int64_t L = 0, kcap = 0;
   CdRun cd;  // the subspace solve of this step, enqueued stage by stage
 };
@@ -468,9 +489,14 @@ inline int spec_step_gram(const StepCtx& cx, const T* C, int64_t rows, int64_t n
   const bool concurrent = (cx.flags & TNB_FLAG_CONCURRENT) != 0;
   {
     BigKernelGate gate(st, concurrent && s.gw.tc_ws != nullptr);
-    TNB_TRY(gram_small_side<T>(C, rows, n, s.G, s.Gf, s.gw, s.tc_gram, &s.used_tc, st));
+    if (s.in_kblocked) {
+      s.used_tc = 1;
+      TNB_TRY(gram_tc_f32(reinterpret_cast<const float*>(C), rows, n, s.G, s.Gf, s.gw.tc_ws, s.gw.tc_bytes, st, true));
+    } else {
+      TNB_TRY(gram_small_side<T>(C, rows, n, s.G, s.Gf, s.gw, s.tc_gram, &s.used_tc, st));
+    }
   }
-  if (cx.info) cx.info->tc_grams += s.used_tc;
+  if (cx.info) cx.info->tc_grams += s.used_tc, cx.info->kblocked_steps += s.in_kblocked ? 1 : 0;
   trace_kernel<<<1, 256, 0, st>>>(s.G, (int)s.L, (int)s.L, cx.sc, first_step ? 1 : 0, cx.eps_scaled2);
   TNB_LAUNCH_CHECK();
   if (prof_on) prof.mark(st);
@@ -532,7 +558,12 @@ inline int spec_step_rest(const StepCtx& cx, const T* C, int64_t rows, int64_t n
     TNB_LAUNCH_CHECK();
     {
       BigKernelGate gate(st, concurrent && rows >= PROJ_TC_MIN_ROWS);
-      TNB_TRY(project_any<T>(C, rows, n, s.fac, rank, Cn, st, s.ptc_ws, s.ptc_bytes));
+      if (s.in_kblocked || s.out_inner > 0)
+        TNB_TRY(project_tc_f32(reinterpret_cast<const float*>(C), rows, n, reinterpret_cast<const float*>(s.fac), (int)rank,
+                               reinterpret_cast<float*>(Cn), s.ptc_ws, s.ptc_bytes, st,
+                               s.in_kblocked ? PT_IN_KBLOCKED : PT_OUT_KBLOCKED, s.out_inner));
+      else
+        TNB_TRY(project_any<T>(C, rows, n, s.fac, rank, Cn, st, s.ptc_ws, s.ptc_bytes));
     }
   } else {
     scale_extract_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(s.V, s.ldv, (int)rows, (int)rank, s.w, s.fac, 1, 0);
@@ -707,6 +738,8 @@ inline int spec_phase1(SpecRun<T, ArenaT>& r, bool dry, const SweepDims& d, int 
   ArenaT& ar = *r.ar;
   r.mark = ar.off;
   spec_step_carve<T>(ar, r.cx, d.rows[mu], d.shape[mu] * d.rcap[mu + 1], d.rcap[mu], r.step);
+  r.step.in_kblocked = carry_kblocked<T>(d, mu, r.cx.allow_tc);
+  r.step.out_inner = carry_kblocked<T>(d, mu - 1, r.cx.allow_tc) ? d.shape[mu - 1] : 0;
   if (ar.off > r.peak) r.peak = ar.off;
   if (dry) return TNB_OK;
   if (!ar.ok) return fail(TNB_ERR_WORKSPACE, "workspace too small (need > %zu bytes)", ar.off);

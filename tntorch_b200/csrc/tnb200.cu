@@ -99,6 +99,7 @@ int tnb_ttsvd(int dtype, const void* data, int ndim, const int64_t* shape, const
     info_host[30] = info.rr_solves;
     info_host[26] = info.speculative;
     info_host[27] = info.spec_flags;
+    info_host[28] = info.kblocked_steps;
     for (int t = 0; t < info.nsteps && t < 6; ++t) {
       info_host[4] += info.gram_ms[t];
       info_host[5] += info.eig_ms[t];
@@ -603,6 +604,13 @@ int tnb_gram_tc_f32(const float* A, int64_t rows, int64_t n, double* G, void* wo
   return gram_tc_f32(A, rows, n, G, nullptr, workspace, workspace_bytes, as_stream(stream));
 }
 
+int tnb_gram_tc_kblocked_f32(const float* A, int64_t rows, int64_t n, double* G, void* workspace, size_t workspace_bytes,
+                             void* stream) {
+  TNB_TRY(require_device());
+  if (!A || !G || !workspace) return fail(TNB_ERR_INVALID, "tnb_gram_tc_kblocked_f32: null argument");
+  return gram_tc_f32(A, rows, n, G, nullptr, workspace, workspace_bytes, as_stream(stream), true);
+}
+
 size_t tnb_atb_tc_workspace_bytes(int64_t K, int64_t m, int64_t n) {
   if (!atb_tc_shape_ok(K, m, n)) return 0;
   return atb_tc_workspace_bytes(K, m, n) + 256;
@@ -655,6 +663,20 @@ int tnb_project_tc_f32(const float* A, int64_t rows, int64_t n, const float* V, 
   TNB_TRY(require_device());
   if (!A || !V || !C || !workspace) return fail(TNB_ERR_INVALID, "tnb_project_tc_f32: null argument");
   return project_tc_f32(A, rows, n, V, r, C, workspace, workspace_bytes, as_stream(stream));
+}
+
+int tnb_project_tc_kblocked_out_f32(const float* A, int64_t rows, int64_t n, const float* V, int32_t r, int64_t inner,
+                                    float* C, void* workspace, size_t workspace_bytes, void* stream) {
+  TNB_TRY(require_device());
+  if (!A || !V || !C || !workspace) return fail(TNB_ERR_INVALID, "tnb_project_tc_kblocked_out_f32: null argument");
+  return project_tc_f32(A, rows, n, V, r, C, workspace, workspace_bytes, as_stream(stream), PT_OUT_KBLOCKED, inner);
+}
+
+int tnb_project_tc_kblocked_in_f32(const float* A, int64_t rows, int64_t n, const float* V, int32_t r, float* C,
+                                   void* workspace, size_t workspace_bytes, void* stream) {
+  TNB_TRY(require_device());
+  if (!A || !V || !C || !workspace) return fail(TNB_ERR_INVALID, "tnb_project_tc_kblocked_in_f32: null argument");
+  return project_tc_f32(A, rows, n, V, r, C, workspace, workspace_bytes, as_stream(stream), PT_IN_KBLOCKED);
 }
 
 size_t tnb_eigh_workspace_bytes(int32_t n) {

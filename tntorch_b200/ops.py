@@ -118,7 +118,7 @@ def ttsvd(data: torch.Tensor, rmax=None, eps: float = 1e-14, batch_mode: bool = 
     if return_info:
         return cores, dict(norm=info[0], eig_solves=int(info[1]), chfsi_products=int(info[2]), tc_grams=int(info[3]),
                            fused_filters=int(info[31]), rr_sweeps=int(info[29]), outer_iterations=int(info[30]),
-                           speculative=int(info[26]), spec_flags=int(info[27]))
+                           speculative=int(info[26]), spec_flags=int(info[27]), kblocked_steps=int(info[28]))
     return cores
 
 
@@ -687,6 +687,34 @@ def gram(A: torch.Tensor, tensorcore: bool = False) -> torch.Tensor:
     return G
 
 
+def to_kblocked(M: torch.Tensor) -> torch.Tensor:
+    """The K-blocked storage of a (rows x n) matrix (rows, n multiples of 8): wgmma's K-major 8 x 4 core matrices,
+    [rows/8][n/8][2][8][4], element (k, c) at (((k/8 * n/8 + c/8) * 2 + k%8/4) * 8 + c%8) * 4 + k%4."""
+    rows, n = M.shape
+    return M.reshape(rows // 8, 2, 4, n // 8, 8).permute(0, 3, 1, 4, 2).contiguous()
+
+
+def from_kblocked(B: torch.Tensor, rows: int, n: int) -> torch.Tensor:
+    """The (rows x n) matrix stored K-blocked in B (inverse of to_kblocked)."""
+    return B.reshape(rows // 8, n // 8, 2, 8, 4).permute(0, 2, 4, 1, 3).reshape(rows, n)
+
+
+def gram_kblocked(B: torch.Tensor, rows: int, n: int) -> torch.Tensor:
+    """fp64 A^T A of the (rows x n) fp32 matrix A stored K-blocked in B (to_kblocked), on the tensor-core Gram kernel
+    that reads both operands K-major (n >= 256, rows % 8 == 0)."""
+    _require_cuda(B, "gram_kblocked")
+    assert B.dtype == torch.float32 and B.is_contiguous() and B.numel() == rows * n
+    G = torch.empty(n, n, dtype=torch.float64, device=B.device)
+    L = lib()
+    wsb = L.tnb_gram_tc_workspace_bytes(rows, n)
+    if wsb == 0:
+        check(_lib.ERR_UNSUPPORTED)
+    ws = _ws(wsb, B.device)
+    with torch.cuda.device(B.device):
+        check(L.tnb_gram_tc_kblocked_f32(_ptr(B), rows, n, _ptr(G), _ptr(ws), ws.numel(), _stream()))
+    return G
+
+
 def atb_tensorcore(A: torch.Tensor, B: torch.Tensor, alpha: float = 1.0, D: Optional[torch.Tensor] = None,
                    beta: float = 0.0) -> torch.Tensor:
     """alpha * A^T B + beta * D on the tensor-core kernel (A: K x m, B: K x n, fp32)."""
@@ -742,6 +770,42 @@ def project(A: torch.Tensor, V: torch.Tensor, tensorcore: bool = False) -> torch
         return Cc
     with torch.cuda.device(A.device):
         check(lib().tnb_project(_dtype_code(A), _ptr(A), rows, n, _ptr(V), r, _ptr(Cc), _stream()))
+    return Cc
+
+
+def project_kblocked_out(A: torch.Tensor, V: torch.Tensor, inner: int) -> torch.Tensor:
+    """project(A, V, tensorcore=True) written K-blocked as the (rows/inner) x (inner*r) matrix whose row a holds rows
+    a*inner .. a*inner+inner-1 of the product (the sweep's carry for a next step with I = inner); returned flat."""
+    _require_cuda(A, "project_kblocked_out")
+    A, V = A.contiguous(), V.contiguous()
+    rows, n = A.shape
+    r = V.shape[1]
+    out = torch.empty(rows * r, dtype=torch.float32, device=A.device)
+    L = lib()
+    wsb = L.tnb_project_tc_workspace_bytes(n, r)
+    if wsb == 0 or A.dtype != torch.float32:
+        check(_lib.ERR_UNSUPPORTED)
+    ws = _ws(wsb, A.device)
+    with torch.cuda.device(A.device):
+        check(L.tnb_project_tc_kblocked_out_f32(_ptr(A), rows, n, _ptr(V), r, int(inner), _ptr(out), _ptr(ws), ws.numel(),
+                                                _stream()))
+    return out
+
+
+def project_kblocked_in(B: torch.Tensor, rows: int, V: torch.Tensor) -> torch.Tensor:
+    """project(A, V, tensorcore=True) for the (rows x n) fp32 matrix A stored K-blocked in B (to_kblocked)."""
+    _require_cuda(B, "project_kblocked_in")
+    V = V.contiguous()
+    n, r = V.shape
+    assert B.dtype == torch.float32 and B.is_contiguous() and B.numel() == rows * n
+    Cc = torch.empty(rows, r, dtype=torch.float32, device=B.device)
+    L = lib()
+    wsb = L.tnb_project_tc_workspace_bytes(n, r)
+    if wsb == 0:
+        check(_lib.ERR_UNSUPPORTED)
+    ws = _ws(wsb, B.device)
+    with torch.cuda.device(B.device):
+        check(L.tnb_project_tc_kblocked_in_f32(_ptr(B), rows, n, _ptr(V), r, _ptr(Cc), _ptr(ws), ws.numel(), _stream()))
     return Cc
 
 
