@@ -1,5 +1,6 @@
 // Generic CUDA-core GEMM used for every shape/dtype the tensor-core kernels do not cover:
-// fp64 everywhere, fp32 with fp32 or fp64 accumulation, ragged sizes, both storage orders.
+// fp64 everywhere, fp32 with fp32 or fp64 accumulation, bf16 operands (dense TT-SVD input), ragged sizes, both storage
+// orders.
 //
 //   C[M,N] = alpha * sum_k A(m,k) * B(k,n)  (+ beta * D + gamma * E)
 //
@@ -13,6 +14,16 @@
 namespace tnb {
 
 constexpr int GEMM_BM = 64, GEMM_BN = 64, GEMM_BK = 16, GEMM_THREADS = 256;
+
+// Operand load: the one place an element becomes the accumulation type (bf16 through fp32, exactly).
+template <typename TAcc, typename T>
+__device__ __forceinline__ TAcc gemm_ld(const T& v) {
+  return (TAcc)v;
+}
+template <typename TAcc>
+__device__ __forceinline__ TAcc gemm_ld(const __nv_bfloat16& v) {
+  return (TAcc)__bfloat162float(v);
+}
 
 template <typename TA, typename TB, typename TAcc, typename TC>
 struct GemmArgs {
@@ -85,7 +96,7 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tile_kernel(const GemmArgs<
       }
       const int64_t gm = m0 + mm, gk = k0 + kk;
       TAcc v = TAcc(0);
-      if (gm < p.M && gk < kend) v = (TAcc)(A_KMAJ ? Ab[gm * p.lda + gk] : Ab[gk * p.lda + gm]);
+      if (gm < p.M && gk < kend) v = gemm_ld<TAcc>(A_KMAJ ? Ab[gm * p.lda + gk] : Ab[gk * p.lda + gm]);
       As[kk][mm] = v;
     }
 #pragma unroll
@@ -101,7 +112,7 @@ __global__ void __launch_bounds__(GEMM_THREADS) gemm_tile_kernel(const GemmArgs<
       }
       const int64_t gn = n0 + nn, gk = k0 + kk;
       TAcc v = TAcc(0);
-      if (gn < p.N && gk < kend) v = (TAcc)(B_KMAJ ? Bb[gn * p.ldb + gk] : Bb[gk * p.ldb + gn]);
+      if (gn < p.N && gk < kend) v = gemm_ld<TAcc>(B_KMAJ ? Bb[gn * p.ldb + gk] : Bb[gk * p.ldb + gn]);
       Bs[kk][nn] = v;
     }
     __syncthreads();

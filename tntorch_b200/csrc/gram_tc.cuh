@@ -17,18 +17,29 @@
 // wgmma.mma_async m64n{tn}k8 .f32.tf32.tf32 with A from registers, accumulating in registers.  setmaxnreg moves the
 // register file to the consumers (TC_CONSUMER_REGS: 128 accumulators plus two stages of A fragments).
 //
-// K-blocked mode (gram_tc_f32(..., kblocked)): C is stored as wgmma's K-major core matrices, [rows/8][n/8][2][8][4]:
+// K-blocked mode (gram_tc(..., kblocked)): C is stored as wgmma's K-major core matrices, [rows/8][n/8][2][8][4]:
 // element (k, c) at (((k/8 * n/8 + c/8) * 2 + k%8/4) * 8 + c%8) * 4 + k%4, the layout the sweep's projection writes for
 // the next step.  Each 8 x 4 core matrix is 128 contiguous bytes and the 8 rows of a k8 step over 256 columns are one
 // contiguous 8 KB run, so TMA loads both operands (256-byte lines, no swizzle) straight into the layout tf32 wgmma reads
 // from shared memory: no transposers, A and B through descriptors, and the freed shared memory holds a
 // TC_BLK_STAGES-deep slab ring.  The 8 rows each k8 step sums are the same 8 rows as in the row-major mode.
 //
+// bf16 mode (gram_tc_bf16): C is a row-major bf16 matrix (the dense TT-SVD's input).  wgmma takes 16-bit operands from
+// shared memory MN-major, so TMA loads boxes of 64 bf16 columns x TC_KC rows (128-byte rows, 128-byte swizzle) and both
+// operands go through descriptors of those boxes as they are: no transposers, a TC_BF16_STAGES-deep ring of 24 KB
+// stages, wgmma.mma_async m64n128k16 .f32.bf16.bf16 on 128 x 128 tiles.  A product of two bf16 values is exact in
+// fp32, so G rounds only in the accumulation.  The tensor core's fp32 accumulation is biased toward zero: over a whole
+// 16384-row split it shrank G by ~5e-5 and left a non-uniform part of 8.5e-6 ||G|| on a rank-6 signal.  So each
+// consumer accumulates TC_BF16_FLUSH stages into a scratch accumulator (the first wgmma of a group overwrites it) and
+// adds that into its running sum with round-to-nearest fp32 adds, which needs the register room of 128-column tiles.
+// Plan (with tn capped at 128), split-K, tile set, fold, partial layout and finalize are those of the fp32 modes.
+//
 // Replaces, for large fp32 unfoldings, the QR of tensor.py:1816 / the Gram of round.py:104-110.
 #pragma once
 #include <cuda.h>
 
 #include <cstdlib>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -49,6 +60,12 @@ constexpr int TC_RING_BYTES = TC_STAGES * TC_STAGE_BYTES + TC_TB_STAGES * TC_TB_
 constexpr int TC_SMEM_BYTES = TC_RING_BYTES + 1024 /*align*/ + 256 /*barriers*/;
 constexpr int TC_BLK_STAGES = 4;                // slab ring depth of the K-blocked mode (no transposed-B buffers)
 static_assert(TC_BLK_STAGES * TC_STAGE_BYTES <= TC_RING_BYTES, "K-blocked ring must fit the row-major mode's buffers");
+constexpr int TC_BF16_STAGE_BYTES = 6 * TC_BOX_BYTES;  // bf16 mode: 4 B boxes (256 columns) + 2 A boxes, TC_KC rows each
+constexpr int TC_BF16_STAGES = 8;
+constexpr int TC_BF16_FLUSH = 16;               // stages (512 rows) per scratch accumulation of the bf16 mode
+static_assert(TC_BF16_STAGES * TC_BF16_STAGE_BYTES <= TC_RING_BYTES, "bf16 ring must fit the row-major mode's buffers");
+constexpr int TC_MAX_RING = 8;                  // mbarriers per ring
+constexpr int TC_ROWMAJOR = 0, TC_KBLOCKED = 1, TC_BF16 = 2;  // gram_tc_kernel modes
 // Longest run of rows one CTA accumulates in fp32 registers (512 stages = 16384 rows).  The diagonal of a Gram grows with
 // the row count while the rounding error of an fp32 sum grows faster; 16384-row partial sums keep that error well below
 // the TF32 operand noise the accept rule of the sweep budgets for.
@@ -387,6 +404,35 @@ __device__ __forceinline__ void wgmma_tf32<8>(float (&d)[128], const uint32_t (&
         "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc));
 }
+// MN-major operand of a 16-bit type with 128-byte swizzle, as TMA writes a box of 64 columns x TC_KC rows: each k is one
+// 128-byte row, 8 rows form a 1024-byte swizzle atom (stride byte offset 1024 between the 8-k groups), and the 64-column
+// blocks along M/N are `lbo` bytes apart (leading byte offset).  Adding 128 (2048 bytes) selects the next k16 slice.
+__device__ __forceinline__ uint64_t wgmma_desc_mn_sw128(const void* p, uint32_t lbo) {
+  return (uint64_t)((smem_u32(p) & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) |
+         ((uint64_t)1 << 62);
+}
+
+// D (64 x 128 fp32) = A (64 x 16) * B (16 x 128) + (accumulate ? D : 0), bf16, both operands MN-major through descriptors.
+__device__ __forceinline__ void wgmma_bf16_ss(float (&d)[64], uint64_t desc_a, uint64_t desc_b, int accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p, 1, 1, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+
 // The same m64n256k8 with A read from shared memory through `desc_a` as well (K-blocked mode).
 __device__ __forceinline__ void wgmma_tf32_ss(float (&d)[128], uint64_t desc_a, uint64_t desc_b) {
   asm volatile(
@@ -422,27 +468,39 @@ __device__ __forceinline__ void wgmma_tf32_ss(float (&d)[128], uint64_t desc_a, 
 // ---------------------------------------------------------------------------------------------
 // The kernel
 // ---------------------------------------------------------------------------------------------
+// Ring geometry of each mode.
+template <int MODE>
+struct TcRing {
+  static constexpr int STAGES = MODE == TC_KBLOCKED ? TC_BLK_STAGES : MODE == TC_BF16 ? TC_BF16_STAGES : TC_STAGES;
+  static constexpr int STAGE_BYTES = MODE == TC_BF16 ? TC_BF16_STAGE_BYTES : TC_STAGE_BYTES;
+  static constexpr int A_SLOT = MODE == TC_BF16 ? 4 : 8;  // first box of a separately loaded A operand
+  static constexpr int BOX_COLS = MODE == TC_BF16 ? 64 : 32;
+};
+static_assert(TcRing<TC_BF16>::STAGES <= TC_MAX_RING && TcRing<TC_KBLOCKED>::STAGES <= TC_MAX_RING, "mbarrier arrays");
+
 // Loads of pipeline iteration `it` (rows it_begin + it) into its ring slot, once the transposers and the consumers have
-// released it.  B first (slots 0..nbox_b), then A (slots 8..11).  Row-major: boxes of 32 columns.  K-blocked: one box
-// of (64, tn / 8 column groups, 4 row groups) for B and one of (64, 16, 4) for A, i.e. four k8 slices of tn (128)
-// columns x 32 bytes.
-template <bool BLOCKED>
+// released it.  B first (slots 0..nbox_b), then A (slots A_SLOT..).  Row-major: boxes of 32 columns.  bf16: boxes of 64
+// columns.  K-blocked: one box of (64, tn / 8 column groups, 4 row groups) for B and one of (64, 16, 4) for A, i.e.
+// four k8 slices of tn (128) columns x 32 bytes.
+template <int MODE>
 __device__ __forceinline__ void gram_tc_produce(const CUtensorMap* tmap, const CUtensorMap* tmap_b, unsigned char* stage_base,
                                                 uint64_t* full_bar, uint64_t* empty_bar, int64_t it, int64_t it_begin,
                                                 int nbox_a, int nbox_b, int a_col0, int b_col0) {
-  constexpr int STAGES = BLOCKED ? TC_BLK_STAGES : TC_STAGES;
-  const int stage = (int)(it % STAGES);
-  const uint32_t phase = (uint32_t)(it / STAGES) & 1u;
+  using R = TcRing<MODE>;
+  const int stage = (int)(it % R::STAGES);
+  const uint32_t phase = (uint32_t)(it / R::STAGES) & 1u;
   mbar_wait_quiet(&empty_bar[stage], phase ^ 1u);
-  unsigned char* sb = stage_base + stage * TC_STAGE_BYTES;
+  unsigned char* sb = stage_base + stage * R::STAGE_BYTES;
   mbar_expect_tx(&full_bar[stage], (uint32_t)(nbox_a + nbox_b) * TC_BOX_BYTES);
   const int row0 = (int)((it_begin + it) * TC_KC);
-  if constexpr (BLOCKED) {
+  if constexpr (MODE == TC_KBLOCKED) {
     tma_load_3d(sb, tmap_b, &full_bar[stage], 0, b_col0 / 8, row0 / 8);
     if (nbox_a) tma_load_3d(sb + 8 * TC_BOX_BYTES, tmap, &full_bar[stage], 0, a_col0 / 8, row0 / 8);
   } else {
-    for (int j = 0; j < nbox_b; ++j) tma_load_2d(sb + j * TC_BOX_BYTES, tmap_b, &full_bar[stage], b_col0 + 32 * j, row0);
-    for (int j = 0; j < nbox_a; ++j) tma_load_2d(sb + (8 + j) * TC_BOX_BYTES, tmap, &full_bar[stage], a_col0 + 32 * j, row0);
+    for (int j = 0; j < nbox_b; ++j)
+      tma_load_2d(sb + j * TC_BOX_BYTES, tmap_b, &full_bar[stage], b_col0 + R::BOX_COLS * j, row0);
+    for (int j = 0; j < nbox_a; ++j)
+      tma_load_2d(sb + (R::A_SLOT + j) * TC_BOX_BYTES, tmap, &full_bar[stage], a_col0 + R::BOX_COLS * j, row0);
   }
 }
 
@@ -581,6 +639,47 @@ __device__ __forceinline__ void gram_tc_consumer_blocked(const GramTcParams& p, 
   gram_tc_epilogue<8>(p, acc, cm, lane, tile_id, split, a_col0, b_col0);
 }
 
+// Consumer warpgroup cw of the bf16 mode (tn = 128): A (this warpgroup's 64 columns of C, box a_box + cw) and B (the
+// stage's two boxes, TC_BOX_BYTES apart) through MN-major descriptors, two k16 slices per stage, into the scratch
+// accumulator `part`; every TC_BF16_FLUSH stages (and at the end) `part` is added into `acc` with fp32 adds.  A slot is
+// released once the wgmma group that read it has completed, i.e. one stage later.
+__device__ __forceinline__ void gram_tc_consumer_bf16(const GramTcParams& p, const unsigned char* stage_base,
+                                                      uint64_t* full_bar, uint64_t* empty_bar, int64_t iters, int a_box,
+                                                      int tile_id, int split, int a_col0, int b_col0) {
+  using R = TcRing<TC_BF16>;
+  const int ct = threadIdx.x - 128;
+  const int lane = ct & 31, w = (ct >> 5) & 3, cw = ct >> 7;
+  const int cm = 64 * cw + 16 * w;
+  float acc[64], part[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) acc[i] = 0.f, part[i] = 0.f;
+  wgmma_fence_operand(part);
+  for (int64_t it = 0; it < iters; ++it) {
+    const int s = (int)(it % R::STAGES);
+    mbar_wait_spin(&full_bar[s], (uint32_t)(it / R::STAGES) & 1u);
+    const unsigned char* sb = stage_base + s * R::STAGE_BYTES;
+    const int first = it % TC_BF16_FLUSH == 0;
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < TC_KC / 16; ++kk)
+      wgmma_bf16_ss(part, wgmma_desc_mn_sw128(sb + (a_box + cw) * TC_BOX_BYTES + kk * 2048, TC_BOX_BYTES),
+                    wgmma_desc_mn_sw128(sb + kk * 2048, TC_BOX_BYTES), (first && kk == 0) ? 0 : 1);
+    wgmma_commit();
+    if ((it + 1) % TC_BF16_FLUSH == 0 || it + 1 == iters) {
+      wgmma_wait<0>();
+      wgmma_fence_operand(part);
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] += part[i];
+      wgmma_fence_operand(part);
+    } else {
+      wgmma_wait<1>();
+    }
+    __syncwarp();
+    if (it > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % R::STAGES]);
+  }
+  gram_tc_epilogue<4>(p, acc, cm, lane, tile_id, split, a_col0, b_col0);
+}
+
 // Output of one consumer warp: acc[4j + 2h + e] is (row cm + g + 8h, column 8j + 2t + e) of the 128 x tn tile.
 template <int NT>
 __device__ __forceinline__ void gram_tc_epilogue(const GramTcParams& p, const float (&acc)[NT * 16], int cm, int lane,
@@ -615,9 +714,10 @@ __device__ __forceinline__ void gram_tc_epilogue(const GramTcParams& p, const fl
   }
 }
 
-// BLOCKED: the operands are K-blocked (see the top of the file); tmap / tmap_b are 3-D maps with boxes (64, 16, 4) and
-// (64, 32, 4).  Otherwise row-major, 2-D maps with boxes of 32 columns x TC_KC rows.
-template <bool BLOCKED>
+// TC_KBLOCKED: the operands are K-blocked (see the top of the file); tmap / tmap_b are 3-D maps with boxes (64, 16, 4)
+// and (64, 32, 4).  TC_ROWMAJOR: row-major fp32, 2-D maps with boxes of 32 columns x TC_KC rows.  TC_BF16: row-major
+// bf16, 2-D maps with boxes of 64 columns x TC_KC rows.
+template <int MODE>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_b,
                const GramTcParams p) {
@@ -627,9 +727,10 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
   const uint32_t pad = (1024u - (raw_addr & 1023u)) & 1023u;
   unsigned char* stage_base = tc_smem_raw + pad;
   unsigned char* tb_base = stage_base + TC_STAGES * TC_STAGE_BYTES;  // row-major mode only
+  constexpr bool BLOCKED = MODE == TC_KBLOCKED, BF16 = MODE == TC_BF16;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(stage_base + TC_RING_BYTES);
-  uint64_t* empty_bar = full_bar + TC_BLK_STAGES;
-  uint64_t* tb_full = empty_bar + TC_BLK_STAGES;
+  uint64_t* empty_bar = full_bar + TC_MAX_RING;
+  uint64_t* tb_full = empty_bar + TC_MAX_RING;
   uint64_t* tb_empty = tb_full + TC_TB_STAGES;
   int* tile_smem = reinterpret_cast<int*>(tb_empty + TC_TB_STAGES);  // bm, bn
 
@@ -651,10 +752,10 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
     }
     tile_smem[0] = fbm;
     tile_smem[1] = fbn;
-    for (int s = 0; s < (BLOCKED ? TC_BLK_STAGES : TC_STAGES); ++s) {
+    for (int s = 0; s < TcRing<MODE>::STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      // per warp: transposers and consumers (K-blocked: consumers only)
-      mbar_init(&empty_bar[s], (BLOCKED ? 0 : TC_TRANSPOSE_THREADS / 32) + 8);
+      // per warp: transposers and consumers (K-blocked, bf16: consumers only)
+      mbar_init(&empty_bar[s], (MODE == TC_ROWMAJOR ? TC_TRANSPOSE_THREADS / 32 : 0) + 8);
     }
     for (int b = 0; b < TC_TB_STAGES; ++b) {
       mbar_init(&tb_full[b], TC_TRANSPOSE_THREADS);  // per thread: each orders its own stores for the async proxy
@@ -666,10 +767,11 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
 
   const int bm = tile_smem[0], bn = tile_smem[1];
   const int a_col0 = bm * 128, b_col0 = bn * p.tn;
-  const int nbox_b = p.tn / 32;
+  constexpr int BOX_COLS = TcRing<MODE>::BOX_COLS;
+  const int nbox_b = p.tn / BOX_COLS;
   const bool a_in_b = p.symmetric && (a_col0 >= b_col0) && (a_col0 + 128 <= b_col0 + p.tn);
-  const int nbox_a = a_in_b ? 0 : 4;
-  const int a_box = a_in_b ? (a_col0 - b_col0) / 32 : 8;  // first box of the A operand in a stage
+  const int nbox_a = a_in_b ? 0 : 128 / BOX_COLS;
+  const int a_box = a_in_b ? (a_col0 - b_col0) / BOX_COLS : TcRing<MODE>::A_SLOT;  // first box of the A operand in a stage
   const int64_t it_begin = (int64_t)split * p.iters_per_split;
   int64_t it_end = it_begin + p.iters_per_split;
   if (it_end > p.iters_total) it_end = p.iters_total;
@@ -679,15 +781,18 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
     setmaxnreg_dec<TC_PRODUCER_REGS>();
     if (threadIdx.x == 0) {
       for (int64_t it = 0; it < iters; ++it)
-        gram_tc_produce<BLOCKED>(&tmap, &tmap_b, stage_base, full_bar, empty_bar, it, it_begin, nbox_a, nbox_b, a_col0,
-                                 b_col0);
-    } else if (!BLOCKED && threadIdx.x >= 32) {
+        gram_tc_produce<MODE>(&tmap, &tmap_b, stage_base, full_bar, empty_bar, it, it_begin, nbox_a, nbox_b, a_col0,
+                              b_col0);
+    } else if (MODE == TC_ROWMAJOR && threadIdx.x >= 32) {
       gram_tc_transposer(stage_base, tb_base, full_bar, empty_bar, tb_full, tb_empty, iters, nbox_b);
     }
     return;
   }
   setmaxnreg_inc<TC_CONSUMER_REGS>();
-  if constexpr (BLOCKED) {  // tn == 256; A inside B: its k8 slices are rows of B's (8 KB apart), else 128-row slices in slot 8
+  if constexpr (BF16) {  // tn = 128
+    gram_tc_consumer_bf16(p, stage_base, full_bar, empty_bar, iters, a_box, tile_id, split, a_col0, b_col0);
+    return;
+  } else if constexpr (BLOCKED) {  // tn == 256; A inside B: its k8 slices are rows of B's (8 KB apart), else 128-row slices in slot 8
     gram_tc_consumer_blocked(p, stage_base, full_bar, empty_bar, iters,
                              a_in_b ? (a_col0 - b_col0) * 32 : 8 * TC_BOX_BYTES, a_in_b ? 256 * 32 : 128 * 32, tile_id,
                              split, a_col0, b_col0);
@@ -784,12 +889,13 @@ inline bool gram_tc_shape_ok(int64_t rows, int64_t n) {
   return n >= 16 && n % 4 == 0 && n <= 16384 && rows >= 1 && rows < ((int64_t)1 << 31) - 64;
 }
 
-inline void gram_tc_plan(int64_t rows, int64_t n, GramTcParams& p, int64_t m_cols = -1) {
+// max_tn: widest column tile (256; 128 for the bf16 mode)
+inline void gram_tc_plan(int64_t rows, int64_t n, GramTcParams& p, int64_t m_cols = -1, int max_tn = 256) {
   p.rows = rows;
   p.n = (int)n;
   p.symmetric = m_cols < 0 ? 1 : 0;
   p.m = p.symmetric ? (int)n : (int)m_cols;
-  int tn = n >= 256 ? 256 : (int)((n + 31) / 32 * 32);
+  int tn = n >= max_tn ? max_tn : (int)((n + 31) / 32 * 32);
   p.tn = tn;
   p.num_bm = (int)((p.m + 127) / 128);
   p.num_bn = (int)((n + tn - 1) / tn);
@@ -839,19 +945,22 @@ inline int gram_tc_fold(int64_t rows, int64_t n) {
   return (rows % f == 0) ? f : 1;
 }
 
-inline size_t gram_tc_workspace_bytes(int64_t rows, int64_t n) {
+inline size_t gram_tc_workspace_bytes(int64_t rows, int64_t n, int max_tn = 256) {
   GramTcParams p;
   const int f = gram_tc_fold(rows, n);
-  gram_tc_plan(rows / f, n * f, p);
+  gram_tc_plan(rows / f, n * f, p, -1, max_tn);
   return align_up((size_t)p.ksplit * p.num_tiles * 128 * p.tn * sizeof(float));
 }
 
-inline int encode_rowmajor_f32(CUtensorMap* tmap, const float* ptr, int64_t rows, int64_t cols, int box_rows = TC_KC) {
+// boxes of 128 bytes per row: 32 fp32 or 64 bf16 columns
+template <typename T = float>
+inline int encode_rowmajor_f32(CUtensorMap* tmap, const T* ptr, int64_t rows, int64_t cols, int box_rows = TC_KC) {
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)cols * sizeof(float)};
-  cuuint32_t box[2] = {32, (cuuint32_t)box_rows};
+  cuuint64_t gstride[1] = {(cuuint64_t)cols * sizeof(T)};
+  cuuint32_t box[2] = {128 / (cuuint32_t)sizeof(T), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult cr = get_encode_tiled()(tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), gdim, gstride, box,
+  CUresult cr = get_encode_tiled()(tmap, sizeof(T) == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+                                   2, const_cast<T*>(ptr), gdim, gstride, box,
                                    estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (cr != CUDA_SUCCESS) return fail(TNB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)cr);
@@ -876,12 +985,30 @@ inline bool gram_tc_kblocked_shape_ok(int64_t rows, int64_t n) {
   return gram_tc_shape_ok(rows, n) && n >= 256 && n % 8 == 0 && rows % 8 == 0;
 }
 
-// G (n x n fp64) and optionally Gf (fp32 copy) = A^T A, A: rows x n fp32 (device), row-major or, with kblocked, stored
-// K-blocked (then n >= 256, n % 8 == 0 and rows % 8 == 0).
-inline int gram_tc_f32(const float* A, int64_t rows, int64_t n, double* G, float* Gf, void* ws, size_t ws_bytes,
-                       cudaStream_t st, bool kblocked = false) {
+// bf16 input: 16-byte rows (n % 8 == 0) and 128-column tiles: a folded n = 32 / 64, n = 128, or n >= 256 (where the
+// upper-triangle tile set of 128 x 128 tiles covers no more than that of the fp32 modes' 128 x 256 tiles).
+inline bool gram_tc_bf16_shape_ok(int64_t rows, int64_t n) {
+  return gram_tc_shape_ok(rows, n) && n % 8 == 0 && (gram_tc_fold(rows, n) > 1 || n == 128 || n >= 256);
+}
+template <typename T>
+inline size_t gram_tc_input_workspace_bytes(int64_t rows, int64_t n) {
+  return gram_tc_workspace_bytes(rows, n, std::is_same<T, __nv_bfloat16>::value ? 128 : 256);
+}
+template <typename T>
+inline bool gram_tc_input_ok(int64_t rows, int64_t n) {
+  if (std::is_same<T, float>::value) return gram_tc_shape_ok(rows, n);
+  if (std::is_same<T, __nv_bfloat16>::value) return gram_tc_bf16_shape_ok(rows, n);
+  return false;
+}
+
+// G (n x n fp64) and optionally Gf (fp32 copy) = A^T A, A: rows x n fp32 or bf16 (device), row-major or, with kblocked
+// (fp32 only), stored K-blocked (then n >= 256, n % 8 == 0 and rows % 8 == 0).
+template <typename T>
+inline int gram_tc(const T* A, int64_t rows, int64_t n, double* G, float* Gf, void* ws, size_t ws_bytes,
+                   cudaStream_t st, bool kblocked = false) {
+  constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
   if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "gram_tc: TMA tensor-core path needs an sm_90 device");
-  if (!(kblocked ? gram_tc_kblocked_shape_ok(rows, n) : gram_tc_shape_ok(rows, n)))
+  if (!(kblocked ? !BF16 && gram_tc_kblocked_shape_ok(rows, n) : gram_tc_input_ok<T>(rows, n)))
     return fail(TNB_ERR_UNSUPPORTED, "gram_tc: unsupported shape rows=%lld n=%lld", (long long)rows, (long long)n);
   if ((reinterpret_cast<uintptr_t>(A) & 15u) != 0) return fail(TNB_ERR_INVALID, "gram_tc: input must be 16-byte aligned");
   GramTcParams p;
@@ -889,7 +1016,7 @@ inline int gram_tc_f32(const float* A, int64_t rows, int64_t n, double* G, float
   const int64_t n_in = n;
   rows /= fold;
   n *= fold;
-  gram_tc_plan(rows, n, p);
+  gram_tc_plan(rows, n, p, -1, BF16 ? 128 : 256);
   p.fold = fold;
   p.n_orig = (int)n_in;
   const size_t need = (size_t)p.ksplit * p.num_tiles * 128 * p.tn * sizeof(float);
@@ -897,19 +1024,25 @@ inline int gram_tc_f32(const float* A, int64_t rows, int64_t n, double* G, float
   p.partial = static_cast<float*>(ws);
 
   dim3 grid((unsigned)p.num_tiles, (unsigned)p.ksplit);
-  if (kblocked) {
+  if constexpr (BF16) {
+    CUtensorMap tmap;
+    TNB_TRY(encode_rowmajor_f32<T>(&tmap, A, rows, n));
+    static PerDeviceFlag attr_done;
+    TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel<TC_BF16>, TC_SMEM_BYTES));
+    gram_tc_kernel<TC_BF16><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(tmap, tmap, p);
+  } else if (kblocked) {
     CUtensorMap ta, tb;
     TNB_TRY(encode_kblocked_f32(&ta, A, rows, n, 128));
     TNB_TRY(encode_kblocked_f32(&tb, A, rows, n, 256));
     static PerDeviceFlag attr_done;
-    TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel<true>, TC_SMEM_BYTES));
-    gram_tc_kernel<true><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(ta, tb, p);
+    TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel<TC_KBLOCKED>, TC_SMEM_BYTES));
+    gram_tc_kernel<TC_KBLOCKED><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(ta, tb, p);
   } else {
     CUtensorMap tmap;
     TNB_TRY(encode_rowmajor_f32(&tmap, A, rows, n));
     static PerDeviceFlag attr_done;
-    TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel<false>, TC_SMEM_BYTES));
-    gram_tc_kernel<false><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(tmap, tmap, p);
+    TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel<TC_ROWMAJOR>, TC_SMEM_BYTES));
+    gram_tc_kernel<TC_ROWMAJOR><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(tmap, tmap, p);
   }
   TNB_LAUNCH_CHECK();
   const int64_t total = n_in * n_in * (p.fold > 1 ? 32 : 1);  // folded form: one warp per element
@@ -976,9 +1109,9 @@ inline int atb_tc_f32(const float* A, int64_t K, int64_t m, const float* B, int6
   TNB_TRY(encode_rowmajor_f32(&ta, A, K, m));
   TNB_TRY(encode_rowmajor_f32(&tb, B, K, n));
   static PerDeviceFlag attr_done;
-  TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel<false>, TC_SMEM_BYTES));
+  TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel<TC_ROWMAJOR>, TC_SMEM_BYTES));
   dim3 grid((unsigned)p.num_tiles, (unsigned)p.ksplit);
-  gram_tc_kernel<false><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(ta, tb, p);
+  gram_tc_kernel<TC_ROWMAJOR><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(ta, tb, p);
   TNB_LAUNCH_CHECK();
   if (narrow) return TNB_OK;
   const int64_t total = m * n;

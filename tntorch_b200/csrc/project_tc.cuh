@@ -19,7 +19,16 @@
 //     products are unchanged; its output is one contiguous 16 x r x 8 run of the carry, staged through shared memory past
 //     the ring (the ring keeps its depth) and stored with 16-byte writes.
 //   * PT_IN_KBLOCKED reads A in that layout (a 1 KB run per 8 rows and 32 columns, no swizzle) and writes C row-major.
+//
+// bf16 A (the dense TT-SVD's input, step 0 only), V and C fp32: V is split once into three bf16 terms v1 = bf16(v),
+// v2 = bf16(v - v1), v3 = bf16(v - v1 - v2), which together hold fp32's 24 significand bits, and every 16-wide k-step
+// issues mma.sync m16n8k16 .bf16 for C v3, C v2, C v1 in that order.  The products of two bf16 values are exact and
+// accumulate in fp32, so C comes out at fp32 accuracy without an fp32 image of A.  A chunk is 64 bf16 columns: the
+// same 128-byte swizzled rows as 32 fp32 columns, so the tiles, the ring, the schedule and both output layouts are
+// shared, and the 32-bit fragment words sit where the tf32 fragments sit.
 #pragma once
+#include <type_traits>
+
 #include "gram_tc.cuh"
 
 namespace tnb {
@@ -63,21 +72,38 @@ struct PtStage {
 };
 
 
+// D += A * B, m16n8k16, bf16 operands (two per 32-bit word, the lower k in the low half), fp32 accumulation.
+__device__ __forceinline__ void mma_bf16(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
+                                         uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+      "{%0, %1, %2, %3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
+// Per A element type: columns per 128-byte chunk row and the number of V terms (fp32: V_hi, V_lo; bf16: v1, v2, v3).
+template <typename TA>
+struct PtType {
+  static constexpr int KC = 128 / (int)sizeof(TA);
+  static constexpr int VTERMS = sizeof(TA) == 4 ? 2 : 3;
+};
+
 // element (row m, column k) of a K-major tile of 32 fp32 columns written by TMA with SWIZZLE_128B
 __device__ __forceinline__ uint32_t km_ld(const unsigned char* base, int m, int k) {
   return *reinterpret_cast<const uint32_t*>(base + m * 128 + ((((k >> 2) ^ (m & 7))) << 4) + ((k & 3) << 2));
 }
 
 // NT = npad / 8 n8 tiles
-template <int NT, int MODE>
+template <int NT, int MODE, typename TA>
 __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const unsigned char* stage_base,
                                                    const unsigned char* v_res, float* stg, uint64_t* full_bar,
                                                    uint64_t* empty_bar, uint64_t* v_bar, int64_t total_items) {
   const int w = (threadIdx.x >> 5) - 1, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
   const int m0 = 16 * w;
-  const int vchunk_bytes = 2 * p.npad * PT_KC * 4;
-  const int vlo_off = p.npad * PT_KC * 4;
+  const int vchunk_bytes = PtType<TA>::VTERMS * p.npad * 128;
+  const int vlo_off = p.npad * 128;  // between V terms
   if (p.vres && total_items > 0) mbar_wait(v_bar, 0);
   float out[NT][4];
 #pragma unroll
@@ -98,7 +124,7 @@ __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const 
 #pragma unroll
       for (int e = 0; e < 4; ++e) acc[j][e] = 0.f;
 #pragma unroll
-    for (int ks = 0; ks < PT_KC; ks += 8) {
+    for (int ks = 0; ks < PT_KC; ks += 8) {  // 8 fragment words: 8 fp32 or 16 bf16 columns
       uint32_t a[4], lo[4];
       if constexpr (MODE == PT_IN_KBLOCKED) {
         a[0] = kb_ld(sa, m0 + g, ks + t);
@@ -111,16 +137,26 @@ __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const 
         a[2] = km_ld(sa, m0 + g, ks + t + 4);
         a[3] = km_ld(sa, m0 + g + 8, ks + t + 4);
       }
+      if constexpr (PtType<TA>::VTERMS == 3) {
+        const unsigned char* v3 = vl + vlo_off;
 #pragma unroll
-      for (int i = 0; i < 4; ++i)
-        lo[i] = __float_as_uint(__uint_as_float(a[i]) - __uint_as_float(a[i] & 0xFFFFE000u));
+        for (int j = 0; j < NT; ++j) {
+          mma_bf16(acc[j], a[0], a[1], a[2], a[3], km_ld(v3, 8 * j + g, ks + t), km_ld(v3, 8 * j + g, ks + t + 4));  // C v3
+          mma_bf16(acc[j], a[0], a[1], a[2], a[3], km_ld(vl, 8 * j + g, ks + t), km_ld(vl, 8 * j + g, ks + t + 4));  // C v2
+          mma_bf16(acc[j], a[0], a[1], a[2], a[3], km_ld(vh, 8 * j + g, ks + t), km_ld(vh, 8 * j + g, ks + t + 4));  // C v1
+        }
+      } else {
 #pragma unroll
-      for (int j = 0; j < NT; ++j) {
-        const uint32_t bh0 = km_ld(vh, 8 * j + g, ks + t), bh1 = km_ld(vh, 8 * j + g, ks + t + 4);
-        const uint32_t bl0 = km_ld(vl, 8 * j + g, ks + t), bl1 = km_ld(vl, 8 * j + g, ks + t + 4);
-        mma_tf32(acc[j], a[0], a[1], a[2], a[3], bl0, bl1);      // A_hi V_lo
-        mma_tf32(acc[j], lo[0], lo[1], lo[2], lo[3], bh0, bh1);  // A_lo V_hi
-        mma_tf32(acc[j], a[0], a[1], a[2], a[3], bh0, bh1);      // A_hi V_hi
+        for (int i = 0; i < 4; ++i)
+          lo[i] = __float_as_uint(__uint_as_float(a[i]) - __uint_as_float(a[i] & 0xFFFFE000u));
+#pragma unroll
+        for (int j = 0; j < NT; ++j) {
+          const uint32_t bh0 = km_ld(vh, 8 * j + g, ks + t), bh1 = km_ld(vh, 8 * j + g, ks + t + 4);
+          const uint32_t bl0 = km_ld(vl, 8 * j + g, ks + t), bl1 = km_ld(vl, 8 * j + g, ks + t + 4);
+          mma_tf32(acc[j], a[0], a[1], a[2], a[3], bl0, bl1);      // A_hi V_lo
+          mma_tf32(acc[j], lo[0], lo[1], lo[2], lo[3], bh0, bh1);  // A_lo V_hi
+          mma_tf32(acc[j], a[0], a[1], a[2], a[3], bh0, bh1);      // A_hi V_hi
+        }
       }
     }
     __syncwarp();
@@ -179,10 +215,13 @@ __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const 
   }
 }
 
-template <int MODE>
+// tmap_v3: the third V term (bf16 A only).
+template <int MODE, typename TA>
 __global__ void __launch_bounds__(PT_THREADS, 1)
 project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_vhi,
-                  const __grid_constant__ CUtensorMap tmap_vlo, const ProjTcParams p) {
+                  const __grid_constant__ CUtensorMap tmap_vlo, const __grid_constant__ CUtensorMap tmap_v3,
+                  const ProjTcParams p) {
+  constexpr int VT = PtType<TA>::VTERMS;
   extern __shared__ unsigned char pt_smem_raw[];
   const uint32_t raw_addr = smem_u32(pt_smem_raw);
   const uint32_t pad = (1024u - (raw_addr & 1023u)) & 1023u;
@@ -192,7 +231,7 @@ project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(stage_base + PT_RING_BYTES + PT_STG_MAX_BYTES);
   uint64_t* empty_bar = full_bar + PT_MAX_STAGES;
   uint64_t* v_bar = empty_bar + PT_MAX_STAGES;
-  const int vchunk_bytes = 2 * p.npad * PT_KC * 4;
+  const int vchunk_bytes = VT * p.npad * 128;
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
@@ -214,8 +253,9 @@ project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       if (p.vres && total_items > 0) {
         mbar_expect_tx(v_bar, (uint32_t)(p.nk * vchunk_bytes));
         for (int kc = 0; kc < p.nk; ++kc) {
-          tma_load_2d(v_res + (size_t)kc * vchunk_bytes, &tmap_vhi, v_bar, kc * PT_KC, 0);
-          tma_load_2d(v_res + (size_t)kc * vchunk_bytes + p.npad * PT_KC * 4, &tmap_vlo, v_bar, kc * PT_KC, 0);
+          tma_load_2d(v_res + (size_t)kc * vchunk_bytes, &tmap_vhi, v_bar, kc * PtType<TA>::KC, 0);
+          tma_load_2d(v_res + (size_t)kc * vchunk_bytes + p.npad * 128, &tmap_vlo, v_bar, kc * PtType<TA>::KC, 0);
+          if (VT == 3) tma_load_2d(v_res + (size_t)kc * vchunk_bytes + 2 * p.npad * 128, &tmap_v3, v_bar, kc * PtType<TA>::KC, 0);
         }
       }
       const uint32_t tx_bytes = (uint32_t)PT_A_BYTES + (p.vres ? 0u : (uint32_t)vchunk_bytes);
@@ -227,15 +267,17 @@ project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         mbar_wait(&empty_bar[stage], phase ^ 1u);
         unsigned char* sb = stage_base + (size_t)stage * p.stage_bytes;
         mbar_expect_tx(&full_bar[stage], tx_bytes);
+        constexpr int KC = PtType<TA>::KC;
         if (MODE == PT_OUT_KBLOCKED)
-          tma_load_3d(sb, &tmap_a, &full_bar[stage], kc * PT_KC, (rb % p.inner16) * 16, (rb / p.inner16) * 8);
+          tma_load_3d(sb, &tmap_a, &full_bar[stage], kc * KC, (rb % p.inner16) * 16, (rb / p.inner16) * 8);
         else if (MODE == PT_IN_KBLOCKED)
-          tma_load_2d(sb, &tmap_a, &full_bar[stage], kc * PT_KC * 8, rb * (PT_BM / 8));
+          tma_load_2d(sb, &tmap_a, &full_bar[stage], kc * KC * 8, rb * (PT_BM / 8));
         else
-          tma_load_2d(sb, &tmap_a, &full_bar[stage], kc * PT_KC, rb * PT_BM);
+          tma_load_2d(sb, &tmap_a, &full_bar[stage], kc * KC, rb * PT_BM);
         if (!p.vres) {
-          tma_load_2d(sb + PT_A_BYTES, &tmap_vhi, &full_bar[stage], kc * PT_KC, 0);
-          tma_load_2d(sb + PT_A_BYTES + p.npad * PT_KC * 4, &tmap_vlo, &full_bar[stage], kc * PT_KC, 0);  // rows npad..2npad-1
+          tma_load_2d(sb + PT_A_BYTES, &tmap_vhi, &full_bar[stage], kc * KC, 0);
+          tma_load_2d(sb + PT_A_BYTES + p.npad * 128, &tmap_vlo, &full_bar[stage], kc * KC, 0);  // rows npad..2npad-1
+          if (VT == 3) tma_load_2d(sb + PT_A_BYTES + 2 * p.npad * 128, &tmap_v3, &full_bar[stage], kc * KC, 0);
         }
         if (++kc == p.nk) { kc = 0; rb += (int)gridDim.x; }
         if (++stage == p.nstages) { stage = 0; phase ^= 1u; }
@@ -244,12 +286,12 @@ project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     return;
   }
   switch (p.npad) {
-    case 16: project_tc_consume<2, MODE>(p, stage_base, v_res, stg, full_bar, empty_bar, v_bar, total_items); break;
-    case 32: project_tc_consume<4, MODE>(p, stage_base, v_res, stg, full_bar, empty_bar, v_bar, total_items); break;
-    case 48: project_tc_consume<6, MODE>(p, stage_base, v_res, stg, full_bar, empty_bar, v_bar, total_items); break;
-    default:  // r <= 48 with a K-blocked output (project_tc_f32)
+    case 16: project_tc_consume<2, MODE, TA>(p, stage_base, v_res, stg, full_bar, empty_bar, v_bar, total_items); break;
+    case 32: project_tc_consume<4, MODE, TA>(p, stage_base, v_res, stg, full_bar, empty_bar, v_bar, total_items); break;
+    case 48: project_tc_consume<6, MODE, TA>(p, stage_base, v_res, stg, full_bar, empty_bar, v_bar, total_items); break;
+    default:  // r <= 48 with a K-blocked output (project_tc)
       if constexpr (MODE != PT_OUT_KBLOCKED)
-        project_tc_consume<8, MODE>(p, stage_base, v_res, stg, full_bar, empty_bar, v_bar, total_items);
+        project_tc_consume<8, MODE, TA>(p, stage_base, v_res, stg, full_bar, empty_bar, v_bar, total_items);
       break;
   }
 }
@@ -268,95 +310,134 @@ __global__ void split_v_kernel(const float* __restrict__ V, int K, int r, int np
   }
 }
 
+// v1, v2, v3 (npad x K bf16 each, K contiguous) from V (K x r): three round-to-nearest bf16 terms of v.
+__global__ void split_v_bf16_kernel(const float* __restrict__ V, int K, int r, int npad, __nv_bfloat16* __restrict__ V1,
+                                    __nv_bfloat16* __restrict__ V2, __nv_bfloat16* __restrict__ V3) {
+  const int total = npad * K;
+  for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += gridDim.x * blockDim.x) {
+    const int j = idx / K, k = idx % K;
+    float v = 0.f;
+    if (j < r) v = V[(size_t)k * r + j];
+    const __nv_bfloat16 b1 = __float2bfloat16_rn(v);
+    const float r1 = v - __bfloat162float(b1);
+    const __nv_bfloat16 b2 = __float2bfloat16_rn(r1);
+    V1[idx] = b1;
+    V2[idx] = b2;
+    V3[idx] = __float2bfloat16_rn(r1 - __bfloat162float(b2));
+  }
+}
+
+// fp32 A: K % 4 == 0 and K >= 32; bf16 A: K % 8 == 0 and K >= 64 (16-byte rows, one full 128-byte chunk).
+template <typename TA = float>
 inline bool project_tc_shape_ok(int64_t rows, int64_t K, int64_t r, const void* A, const void* C) {
-  return r >= 1 && r <= PT_MAX_N && K % 4 == 0 && K >= 32 && K <= (1 << 24) && rows >= 128 &&
+  constexpr int KC = PtType<TA>::KC;
+  return r >= 1 && r <= PT_MAX_N && K % (16 / (int)sizeof(TA)) == 0 && K >= KC && K <= (1 << 24) && rows >= 128 &&
          rows < ((int64_t)1 << 31) - 256 && (reinterpret_cast<uintptr_t>(A) & 15u) == 0 &&
          (reinterpret_cast<uintptr_t>(C) & 15u) == 0;
 }
+template <typename TA = float>
 inline size_t project_tc_workspace_bytes(int64_t K, int64_t r) {
   const int64_t npad = (r + 15) / 16 * 16;
-  return 2 * align_up((size_t)npad * K * sizeof(float));
+  return PtType<TA>::VTERMS * align_up((size_t)npad * K * sizeof(TA));
 }
 
-inline int encode_kmajor_f32(CUtensorMap* tmap, const float* ptr, int64_t rows, int64_t cols, int box_rows) {
+template <typename T>
+inline CUtensorMapDataType tma_dtype() {
+  return sizeof(T) == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+}
+
+// boxes of 128 bytes (32 fp32 or 64 bf16 columns) x box_rows rows
+template <typename T = float>
+inline int encode_kmajor_f32(CUtensorMap* tmap, const T* ptr, int64_t rows, int64_t cols, int box_rows) {
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t gstride[1] = {(cuuint64_t)cols * sizeof(float)};
-  cuuint32_t box[2] = {(cuuint32_t)PT_KC, (cuuint32_t)box_rows};
+  cuuint64_t gstride[1] = {(cuuint64_t)cols * sizeof(T)};
+  cuuint32_t box[2] = {(cuuint32_t)PtType<T>::KC, (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult cr = get_encode_tiled()(tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), gdim, gstride, box,
+  CUresult cr = get_encode_tiled()(tmap, tma_dtype<T>(), 2, const_cast<T*>(ptr), gdim, gstride, box,
                                    estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (cr != CUDA_SUCCESS) return fail(TNB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)cr);
   return TNB_OK;
 }
 
-// C (rows x r) = A (rows x K) V (K x r); ws: project_tc_workspace_bytes(K, r).
+// C (rows x r) = A (rows x K) V (K x r); ws: project_tc_workspace_bytes<TA>(K, r).  TA: float or __nv_bfloat16.
 //   layout PT_ROWMAJOR:     A and C row-major;
 //   layout PT_OUT_KBLOCKED: A row-major, C stored as the K-blocked (gram_tc.cuh) (rows / inner) x (inner * r) matrix;
 //                           needs inner % 16 == 0, rows % (8 * inner) == 0, r % 16 == 0, r <= 48;
-//   layout PT_IN_KBLOCKED:  A stored K-blocked (rows % 8 == 0, K % 8 == 0), C row-major.
-inline int project_tc_f32(const float* A, int64_t rows, int64_t K, const float* V, int r, float* C, void* ws, size_t ws_bytes,
-                          cudaStream_t st, int layout = PT_ROWMAJOR, int64_t inner = 0) {
+//   layout PT_IN_KBLOCKED:  A stored K-blocked (rows % 8 == 0, K % 8 == 0), C row-major (fp32 A only).
+template <typename TA>
+inline int project_tc(const TA* A, int64_t rows, int64_t K, const float* V, int r, float* C, void* ws, size_t ws_bytes,
+                      cudaStream_t st, int layout = PT_ROWMAJOR, int64_t inner = 0) {
+  constexpr bool BF16 = std::is_same<TA, __nv_bfloat16>::value;
+  constexpr int KC = PtType<TA>::KC, VT = PtType<TA>::VTERMS;
   if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "project_tc: needs an sm_90 device");
-  if (!project_tc_shape_ok(rows, K, r, A, C)) return fail(TNB_ERR_UNSUPPORTED, "project_tc: unsupported shape");
+  if (!project_tc_shape_ok<TA>(rows, K, r, A, C)) return fail(TNB_ERR_UNSUPPORTED, "project_tc: unsupported shape");
   if (layout == PT_OUT_KBLOCKED && !(inner >= 16 && inner % 16 == 0 && rows % (8 * inner) == 0 && r % 16 == 0 && r <= 48))
     return fail(TNB_ERR_UNSUPPORTED,
                 "project_tc: K-blocked output needs inner %% 16 == 0, rows %% (8 inner) == 0, r %% 16 == 0, r <= 48");
-  if (layout == PT_IN_KBLOCKED && (rows % 8 != 0 || K % 8 != 0))
-    return fail(TNB_ERR_UNSUPPORTED, "project_tc: K-blocked input needs rows %% 8 == 0 and K %% 8 == 0");
-  if (ws_bytes < project_tc_workspace_bytes(K, r)) return fail(TNB_ERR_WORKSPACE, "project_tc: workspace too small");
+  if (layout == PT_IN_KBLOCKED && (BF16 || rows % 8 != 0 || K % 8 != 0))
+    return fail(TNB_ERR_UNSUPPORTED, "project_tc: K-blocked input needs fp32, rows %% 8 == 0 and K %% 8 == 0");
+  if (ws_bytes < project_tc_workspace_bytes<TA>(K, r)) return fail(TNB_ERR_WORKSPACE, "project_tc: workspace too small");
   ProjTcParams p;
   p.rows = rows; p.K = (int)K; p.r = r; p.npad = (r + 15) / 16 * 16;
   p.num_row_blocks = (rows + PT_BM - 1) / PT_BM;
-  p.nk = (int)((K + PT_KC - 1) / PT_KC);
+  p.nk = (int)((K + KC - 1) / KC);
   p.C = C;
   p.inner16 = layout == PT_OUT_KBLOCKED ? (int)(inner / 16) : 1;
   p.out_ld = layout == PT_OUT_KBLOCKED ? inner * r : 0;
-  const int vchunk = 2 * p.npad * PT_KC * 4;
+  const int vchunk = VT * p.npad * 128;
   p.vres = ((int64_t)p.nk * vchunk <= PT_VRES_MAX_BYTES) ? 1 : 0;
   p.stage_bytes = PT_A_BYTES + (p.vres ? 0 : vchunk);
   p.nstages = (PT_RING_BYTES - (p.vres ? p.nk * vchunk : 0)) / p.stage_bytes;
   if (p.nstages > PT_MAX_STAGES) p.nstages = PT_MAX_STAGES;
-  float* Vhi = static_cast<float*>(ws);
-  float* Vlo = reinterpret_cast<float*>(static_cast<char*>(ws) + align_up((size_t)p.npad * K * sizeof(float)));
-  split_v_kernel<<<grid_for((int64_t)p.npad * K), 256, 0, st>>>(V, (int)K, r, p.npad, Vhi, Vlo);
+  const size_t term_bytes = align_up((size_t)p.npad * K * sizeof(TA));
+  TA* Vt[3];
+  for (int q = 0; q < 3; ++q) Vt[q] = reinterpret_cast<TA*>(static_cast<char*>(ws) + (q < VT ? q : 0) * term_bytes);
+  if constexpr (BF16)
+    split_v_bf16_kernel<<<grid_for((int64_t)p.npad * K), 256, 0, st>>>(V, (int)K, r, p.npad, Vt[0], Vt[1], Vt[2]);
+  else
+    split_v_kernel<<<grid_for((int64_t)p.npad * K), 256, 0, st>>>(V, (int)K, r, p.npad, Vt[0], Vt[1]);
   TNB_LAUNCH_CHECK();
-  CUtensorMap ta, th, tl;
+  CUtensorMap ta, th, tl, t3;
   CUresult cr = CUDA_SUCCESS;
-  if (layout == PT_OUT_KBLOCKED) {  // (K, inner, rows / inner), box (32, 16, 8): the 128 x 32 tile of 8 rows of M
+  if (layout == PT_OUT_KBLOCKED) {  // (K, inner, rows / inner), box (KC, 16, 8): the 128 x KC tile of 8 rows of M
     cuuint64_t gdim[3] = {(cuuint64_t)K, (cuuint64_t)inner, (cuuint64_t)(rows / inner)};
-    cuuint64_t gstride[2] = {(cuuint64_t)K * sizeof(float), (cuuint64_t)(inner * K) * sizeof(float)};
-    cuuint32_t box[3] = {(cuuint32_t)PT_KC, 16, 8}, estr[3] = {1, 1, 1};
-    cr = get_encode_tiled()(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(A), gdim, gstride, box, estr,
+    cuuint64_t gstride[2] = {(cuuint64_t)K * sizeof(TA), (cuuint64_t)(inner * K) * sizeof(TA)};
+    cuuint32_t box[3] = {(cuuint32_t)KC, 16, 8}, estr[3] = {1, 1, 1};
+    cr = get_encode_tiled()(&ta, tma_dtype<TA>(), 3, const_cast<TA*>(A), gdim, gstride, box, estr,
                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   } else if (layout == PT_IN_KBLOCKED) {  // (8 K, rows / 8), box (8 x 32 columns, 16 row groups), no swizzle
     cuuint64_t gdim[2] = {(cuuint64_t)(8 * K), (cuuint64_t)(rows / 8)};
     cuuint64_t gstride[1] = {(cuuint64_t)(8 * K) * sizeof(float)};
     cuuint32_t box[2] = {8 * PT_KC, PT_BM / 8}, estr[2] = {1, 1};
-    cr = get_encode_tiled()(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(A), gdim, gstride, box, estr,
+    cr = get_encode_tiled()(&ta, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<TA*>(A), gdim, gstride, box, estr,
                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   } else {
-    TNB_TRY(encode_kmajor_f32(&ta, A, rows, K, PT_BM));
+    TNB_TRY(encode_kmajor_f32<TA>(&ta, A, rows, K, PT_BM));
   }
   if (cr != CUDA_SUCCESS) return fail(TNB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)cr);
-  TNB_TRY(encode_kmajor_f32(&th, Vhi, p.npad, K, p.npad));
-  TNB_TRY(encode_kmajor_f32(&tl, Vlo, p.npad, K, p.npad));
+  TNB_TRY(encode_kmajor_f32<TA>(&th, Vt[0], p.npad, K, p.npad));
+  TNB_TRY(encode_kmajor_f32<TA>(&tl, Vt[1], p.npad, K, p.npad));
+  t3 = th;
+  if (VT == 3) TNB_TRY(encode_kmajor_f32<TA>(&t3, Vt[2], p.npad, K, p.npad));
   const int sms = usable_sms();
   const int64_t grid = p.num_row_blocks < sms ? p.num_row_blocks : sms;
   if (layout == PT_OUT_KBLOCKED) {
     static PerDeviceFlag attr_done;
-    TNB_CUDA(ensure_dyn_smem(attr_done, project_tc_kernel<PT_OUT_KBLOCKED>, PT_SMEM_BYTES));
-    project_tc_kernel<PT_OUT_KBLOCKED><<<(unsigned)grid, PT_THREADS, PT_SMEM_BYTES, st>>>(ta, th, tl, p);
+    TNB_CUDA(ensure_dyn_smem(attr_done, project_tc_kernel<PT_OUT_KBLOCKED, TA>, PT_SMEM_BYTES));
+    project_tc_kernel<PT_OUT_KBLOCKED, TA><<<(unsigned)grid, PT_THREADS, PT_SMEM_BYTES, st>>>(ta, th, tl, t3, p);
   } else if (layout == PT_IN_KBLOCKED) {
-    static PerDeviceFlag attr_done;
-    TNB_CUDA(ensure_dyn_smem(attr_done, project_tc_kernel<PT_IN_KBLOCKED>, PT_SMEM_BYTES));
-    project_tc_kernel<PT_IN_KBLOCKED><<<(unsigned)grid, PT_THREADS, PT_SMEM_BYTES, st>>>(ta, th, tl, p);
+    if constexpr (!BF16) {
+      static PerDeviceFlag attr_done;
+      TNB_CUDA(ensure_dyn_smem(attr_done, project_tc_kernel<PT_IN_KBLOCKED, TA>, PT_SMEM_BYTES));
+      project_tc_kernel<PT_IN_KBLOCKED, TA><<<(unsigned)grid, PT_THREADS, PT_SMEM_BYTES, st>>>(ta, th, tl, t3, p);
+    }
   } else {
     static PerDeviceFlag attr_done;
-    TNB_CUDA(ensure_dyn_smem(attr_done, project_tc_kernel<PT_ROWMAJOR>, PT_SMEM_BYTES));
-    project_tc_kernel<PT_ROWMAJOR><<<(unsigned)grid, PT_THREADS, PT_SMEM_BYTES, st>>>(ta, th, tl, p);
+    TNB_CUDA(ensure_dyn_smem(attr_done, project_tc_kernel<PT_ROWMAJOR, TA>, PT_SMEM_BYTES));
+    project_tc_kernel<PT_ROWMAJOR, TA><<<(unsigned)grid, PT_THREADS, PT_SMEM_BYTES, st>>>(ta, th, tl, t3, p);
   }
   TNB_LAUNCH_CHECK();
   return TNB_OK;

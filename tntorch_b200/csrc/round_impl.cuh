@@ -186,7 +186,7 @@ inline int tt_round_impl(ArenaT& ar, bool dry, const T* const* cores_in, const R
     const int64_t n = d.shape[mu] * (dry ? d.rcap[mu + 1] : r_next);
     const bool have_rmax = rmax && rmax[mu - 1] > 0;
     int64_t rank = d.rcap[mu];
-    TNB_TRY((truncate_step<T>(ar, dry, cx, M, rows, n, d.rcap[mu], have_rmax, have_rmax ? rmax[mu - 1] : 0, t == 0,
+    TNB_TRY((truncate_step<T, T>(ar, dry, cx, M, rows, n, d.rcap[mu], have_rmax, have_rmax ? rmax[mu - 1] : 0, t == 0,
                               dry ? nullptr : cores_out + d.slot[mu], left, &rank)));
     if (!dry) {
       ranks_host[mu] = (int32_t)rank;
@@ -305,7 +305,7 @@ inline int tt_round_spec_enqueue(ArenaT& ar, bool dry, const T* const* cores_in,
     const size_t mark = ar.off;
     const int64_t rows = d.ra[mu];
     const int64_t n = d.shape[mu] * d.rcap[mu + 1];
-    spec_step_carve<T>(ar, cx, rows, n, d.rcap[mu], step);
+    spec_step_carve<T, T>(ar, cx, rows, n, d.rcap[mu], step);
     if (ar.off > peak) peak = ar.off;
     if (!dry) {
       if (!ar.ok) return fail(TNB_ERR_WORKSPACE, "tt_round: workspace too small (need > %zu bytes)", ar.off);
@@ -639,10 +639,10 @@ inline int truncated_svd_impl(ArenaT& ar, bool dry, const T* M, int64_t m, int64
 // || T - TT(cores) ||_F / || T ||_F  with the last contraction fused with the difference and the
 // two squared norms (fp64 accumulation).  Tensor.torch() tensor.py:1639-1687 + metrics.py:135-151.
 // ---------------------------------------------------------------------------------------------
-template <typename T>
+template <typename T, typename TD>
 __global__ void __launch_bounds__(256) recon_diff_kernel(const T* __restrict__ F, int64_t rows, int r,
                                                          const T* __restrict__ core, int ncols,
-                                                         const T* __restrict__ data, double* __restrict__ acc) {
+                                                         const TD* __restrict__ data, double* __restrict__ acc) {
   // each block handles a strip of rows; thread computes dot(F[row,:], core[:,col]) for its (row, col)
   __shared__ double red[32];
   double d2 = 0.0, t2 = 0.0;
@@ -653,8 +653,8 @@ __global__ void __launch_bounds__(256) recon_diff_kernel(const T* __restrict__ F
     const int col = (int)(idx % ncols);
     double s = 0.0;
     for (int k = 0; k < r; ++k) s += (double)F[row * r + k] * (double)core[(size_t)k * ncols + col];
-    const double t = (double)data[idx];
-    const double diff = t - (double)(T)s;  // reconstruct in the data precision, like the reference
+    const double t = gemm_ld<double>(data[idx]);
+    const double diff = t - (double)(T)s;  // reconstruct in the cores' precision (the data's, like the reference, or fp32)
     d2 += diff * diff;
     t2 += t * t;
   }
@@ -666,8 +666,9 @@ __global__ void __launch_bounds__(256) recon_diff_kernel(const T* __restrict__ F
   }
 }
 
-template <typename T, class ArenaT>
-inline int tt_relative_error_impl(ArenaT& ar, bool dry, const T* data, const T* const* cores, int N,
+// TD: the data's element type (T, or bf16 with fp32 cores)
+template <typename T, typename TD, class ArenaT>
+inline int tt_relative_error_impl(ArenaT& ar, bool dry, const TD* data, const T* const* cores, int N,
                                   const int64_t* shape, const int32_t* ranks, double* result_host, cudaStream_t st) {
   if (N < 2) return fail(TNB_ERR_UNSUPPORTED, "tt_relative_error: needs at least 2 modes");
   double* acc = ar.template take<double>(2);
@@ -694,7 +695,7 @@ inline int tt_relative_error_impl(ArenaT& ar, bool dry, const T* data, const T* 
     rows *= shape[k];
   }
   const int ncols = (int)shape[N - 1];
-  recon_diff_kernel<T><<<grid_for(rows * ncols, 256, 1184), 256, 0, st>>>(Fc, rows, ranks[N - 1], cores[N - 1], ncols,
+  recon_diff_kernel<T, TD><<<grid_for(rows * ncols, 256, 1184), 256, 0, st>>>(Fc, rows, ranks[N - 1], cores[N - 1], ncols,
                                                                          data, acc);
   TNB_LAUNCH_CHECK();
   double* h = static_cast<double*>(pinned_scratch(2 * sizeof(double)));

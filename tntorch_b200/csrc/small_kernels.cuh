@@ -1,6 +1,7 @@
 // Glue kernels around the GEMM / eigen kernels: rank rule, factor extraction, traces, fills.
 #pragma once
 #include "common.cuh"
+#include "gemm_generic.cuh"
 #include "jacobi.cuh"
 
 namespace tnb {
@@ -27,11 +28,17 @@ struct SweepScalars {
 // (half the 1e-5 parity bar), with the tail taken at the low end of what the noisy values resolve.  A flat spectrum
 // (random data: lambda_0 << trace, tail ~ trace) passes on the first bound; signal + noise with a clear gap passes on the
 // second; a tensor whose discarded tail is below ~1e-4 of its norm does not, and takes the exact Gram.
-__device__ inline int tf32_gram_rejected(const double* w, int nvals, int L, int rank, double trace) {
+// `noise` is the measured ||E|| / ||G|| of the kernel that produced G (TF32_GRAM_NOISE, BF16_GRAM_NOISE).  The bf16
+// Gram has exact products and adds its 512-row partial sums with round-to-nearest (gram_tc.cuh): on bf16-rounded
+// randn(2^24, 64), randn(262144, 2048) and a rank-6 signal plus 1e-3 noise of 2^24 x 64, ||G_bf16 - (1 - c) G_fp64||_2 /
+// ||G_fp64||_2 measured 7.3e-9, 9.2e-8 and 6.3e-8, with shrinks c of 9.3e-7, 9.2e-7 and 5.9e-7 (H100 80GB HBM3, 700 W).
+constexpr double TF32_GRAM_NOISE = 2e-6;
+constexpr double BF16_GRAM_NOISE = 1e-7;
+__device__ inline int tf32_gram_rejected(const double* w, int nvals, int L, int rank, double trace, double noise) {
   if (rank >= L) return 0;  // nothing discarded
   const double lam0 = w[0] > 0.0 ? w[0] : 0.0;
   if (!(trace > 0.0) || !(lam0 > 0.0)) return 0;
-  const double normE = 4e-6 * lam0;  // twice the measured 2e-6
+  const double normE = 2.0 * noise * lam0;  // twice the measured level
   double head = 0.0;
   for (int i = 0; i < rank && i < nvals; ++i) head += w[i] > 0.0 ? w[i] : 0.0;
   const double first = 2.0 * rank * normE;
@@ -79,7 +86,7 @@ __global__ void set_delta2_kernel(SweepScalars* sc, double delta_abs, double eps
 //   leading values only (topk == 1): w holds kk >= min(rmax, L) leading Ritz values; the tail energy
 //   behind index k is trace - sum_{i<=k} w_i.
 __global__ void rank_rule_kernel(const double* __restrict__ w, int L, int kk, int rmax, int topk, int batch_mode,
-                                 SweepScalars* sc, int used_tf32 = 0, int nvals = 0) {
+                                 SweepScalars* sc, double gram_noise = 0.0, int nvals = 0) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   sc->tf32_reject = 0;
   const double w0 = w[0] > 0.0 ? w[0] : 0.0;
@@ -117,7 +124,8 @@ __global__ void rank_rule_kernel(const double* __restrict__ w, int L, int kk, in
   }
   if (rank < 1) rank = 1;
   sc->rank = rank;
-  if (used_tf32 && !sc->zero_flag && !sc->undecided) sc->tf32_reject = tf32_gram_rejected(w, nvals > 0 ? nvals : (topk ? kk : L), L, rank, sc->trace);
+  if (gram_noise > 0.0 && !sc->zero_flag && !sc->undecided)
+    sc->tf32_reject = tf32_gram_rejected(w, nvals > 0 ? nvals : (topk ? kk : L), L, rank, sc->trace, gram_noise);
 }
 
 // Speculative sweep (sweep.cuh): the step was enqueued assuming rank == expect; record the rank the rule chose and raise
@@ -131,6 +139,13 @@ __global__ void spec_check_kernel(const SweepScalars* sc, int expect, int32_t* r
   if (sc->rank != expect) f |= 16;
   if (sc->zero_flag) f |= 32;
   if (f) atomicOr(flags, f);
+}
+
+// out[i] = in[i] in the output type (a bf16 input's single core, N = 1)
+template <typename TOut, typename TIn>
+__global__ void convert_kernel(const TIn* __restrict__ in, int64_t n, TOut* __restrict__ out) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+    out[i] = gemm_ld<TOut>(in[i]);
 }
 
 // out[i][j] (or out[j][i] when transpose) = V[i][j] * f(w_j) for j < rank, i < rows.

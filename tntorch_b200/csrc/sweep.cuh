@@ -25,22 +25,36 @@
 
 namespace tnb {
 
-// C (rows x r) = A (rows x n) * V (n x r) in the data precision: streaming FFMA kernel for fp32 when the
-// shape allows, generic tiled GEMM otherwise.
-constexpr int64_t PROJ_TC_MIN_ROWS = 16384;
-inline bool project_use_tc(int64_t rows, int64_t n, int64_t r, const void* A, const void* C) {
-  return rows >= PROJ_TC_MIN_ROWS && project_tc_shape_ok(rows, n, r, A, C);
+// The input of the dense TT-SVD may be bf16 (TIn); only step 0 reads it, every carry and core is T (fp32 for bf16 input).
+template <typename TIn>
+constexpr bool tc_input() {
+  return std::is_same<TIn, float>::value || std::is_same<TIn, __nv_bfloat16>::value;
 }
-template <typename T>
-inline int project_any(const T* A, int64_t rows, int64_t n, const T* V, int64_t r, T* C, cudaStream_t st,
+
+// C (rows x r) = A (rows x n) * V (n x r) in the data precision (fp32 for bf16 A): tensor-core kernel, streaming FFMA
+// kernel for fp32 when the shape allows, generic tiled GEMM otherwise.
+constexpr int64_t PROJ_TC_MIN_ROWS = 16384;
+template <typename TIn = float>
+inline bool project_use_tc(int64_t rows, int64_t n, int64_t r, const void* A, const void* C) {
+  return tc_input<TIn>() && rows >= PROJ_TC_MIN_ROWS && project_tc_shape_ok<TIn>(rows, n, r, A, C);
+}
+template <typename T, typename TIn = T>
+inline int project_any(const TIn* A, int64_t rows, int64_t n, const T* V, int64_t r, T* C, cudaStream_t st,
                        void* tc_ws = nullptr, size_t tc_ws_bytes = 0) {
-  if (std::is_same<T, float>::value && tc_ws && tc_path_available() && project_use_tc(rows, n, r, A, C))
-    return project_tc_f32(reinterpret_cast<const float*>(A), rows, n, reinterpret_cast<const float*>(V), (int)r,
-                          reinterpret_cast<float*>(C), tc_ws, tc_ws_bytes, st);
-  if (std::is_same<T, float>::value && project_f32_fast_ok(rows, n, r, A, C))
+  if constexpr (tc_input<TIn>())
+    if (tc_ws && tc_path_available() && project_use_tc<TIn>(rows, n, r, A, C))
+      return project_tc<TIn>(A, rows, n, reinterpret_cast<const float*>(V), (int)r, reinterpret_cast<float*>(C), tc_ws,
+                             tc_ws_bytes, st);
+  if (std::is_same<TIn, float>::value && project_f32_fast_ok(rows, n, r, A, C))
     return project_f32_fast(reinterpret_cast<const float*>(A), rows, n, reinterpret_cast<const float*>(V), (int)r,
                             reinterpret_cast<float*>(C), st);
-  return gemm_direct<T, T, T, T>(rows, r, n, A, n, true, V, r, false, C, r, (T)1, nullptr, 0, (T)0, nullptr, 0, (T)0, st);
+  return gemm_direct<TIn, T, T, T>(rows, r, n, A, n, true, V, r, false, C, r, (T)1, nullptr, 0, (T)0, nullptr, 0, (T)0, st);
+}
+// Workspace of the tensor-core projection of a step (0: the step projects elsewhere).
+template <typename TIn>
+inline size_t project_tc_carve_bytes(bool allow_tc, int64_t rows, int64_t n, int64_t kcap) {
+  if (!allow_tc || !tc_input<TIn>() || rows < n || !project_use_tc<TIn>(rows, n, kcap, nullptr, nullptr)) return 0;
+  return project_tc_workspace_bytes<TIn>(n, kcap);
 }
 
 constexpr int64_t TC_MIN_ROWS = 2048;  // below this the generic fp64-accumulating Gram is used
@@ -88,24 +102,24 @@ inline int make_dims(int ndim, const int64_t* shape, const int32_t* rmax, SweepD
 // step mu takes the tensor-core Gram unfolded (n' >= 256) and the tensor-core projection, and step mu + 1 projects on the
 // tensor cores with an epilogue that can write it (rcap[mu+1] % 16 == 0 and <= 48, shape[mu] % 16 == 0).  Its Gram then loads
 // K-major operands directly instead of transposing every slab in shared memory.  The writer's own input must be
-// row-major, and the last carry (step mu = 0's core) stays row-major.
-template <typename T>
+// row-major (fp32, or the bf16 input when the writer is step 0), and the last carry (step mu = 0's core) stays row-major.
+template <typename T, typename TIn = T>
 inline bool carry_kblocked(const SweepDims& d, int mu, bool allow_tc) {
   if (!std::is_same<T, float>::value || !allow_tc || mu < 1 || mu + 1 > d.N - 1) return false;
   const int64_t rows = d.rows[mu], n = d.shape[mu] * d.rcap[mu + 1], k = std::min<int64_t>(d.rcap[mu], n);
   const bool reader = rows >= n && rows >= std::max(TC_MIN_ROWS, PROJ_TC_MIN_ROWS) && gram_tc_kblocked_shape_ok(rows, n) &&
                       k <= PT_MAX_N && project_tc_shape_ok(rows, n, k, nullptr, nullptr);
   const int64_t wrows = d.rows[mu + 1], wn = d.shape[mu + 1] * d.rcap[mu + 2], r = d.rcap[mu + 1];
-  const bool writer = wrows >= wn && wrows >= PROJ_TC_MIN_ROWS && wn >= 32 && project_tc_shape_ok(wrows, wn, r, nullptr, nullptr) &&
-                      r % 16 == 0 && r <= 48 && d.shape[mu] % 16 == 0;
-  return reader && writer && !carry_kblocked<T>(d, mu + 1, allow_tc);
+  const bool wtc = mu + 1 == d.N - 1 ? project_use_tc<TIn>(wrows, wn, r, nullptr, nullptr)
+                                     : project_use_tc<T>(wrows, wn, r, nullptr, nullptr);
+  const bool writer = wrows >= wn && wn >= 32 && wtc && r % 16 == 0 && r <= 48 && d.shape[mu] % 16 == 0;
+  return reader && writer && !carry_kblocked<T, TIn>(d, mu + 1, allow_tc);
 }
 
 // ---------------------------------------------------------------------------------------------
 // Gram of a (rows x n) row-major matrix on whichever side is smaller, into fp64 G (L x L).
 // ---------------------------------------------------------------------------------------------
-template <typename T>
-struct GramWork {
+struct GramWork {  // untyped buffers: the same for every input type
   double* partial = nullptr;
   size_t partial_elems = 0;
   void* tc_ws = nullptr;
@@ -113,7 +127,7 @@ struct GramWork {
 };
 
 template <typename T, class ArenaT>
-inline void gram_carve(ArenaT& ar, int64_t rows, int64_t n, bool allow_tc, GramWork<T>& w) {
+inline void gram_carve(ArenaT& ar, int64_t rows, int64_t n, bool allow_tc, GramWork& w) {  // T: the input type
   const bool tall = rows >= n;
   const int64_t L = tall ? n : rows;
   const int64_t K = tall ? rows : n;
@@ -122,22 +136,24 @@ inline void gram_carve(ArenaT& ar, int64_t rows, int64_t n, bool allow_tc, GramW
   w.partial = ar.template take<double>(pl.partial_elems);
   w.tc_bytes = 0;
   w.tc_ws = nullptr;
-  if (allow_tc && std::is_same<T, float>::value && tall && rows >= TC_MIN_ROWS && gram_tc_shape_ok(rows, n)) {
-    w.tc_bytes = gram_tc_workspace_bytes(rows, n);
+  if (allow_tc && tall && rows >= TC_MIN_ROWS && gram_tc_input_ok<T>(rows, n)) {
+    w.tc_bytes = gram_tc_input_workspace_bytes<T>(rows, n);
     w.tc_ws = ar.template take<char>(w.tc_bytes);
   }
 }
 
+// *used_tc: 0 exact-product Gram, 1 TF32 tensor-core Gram, 2 bf16 tensor-core Gram (gram_noise)
 template <typename T>
-inline int gram_small_side(const T* C, int64_t rows, int64_t n, double* G, float* Gf, GramWork<T>& w, bool use_tc,
+inline int gram_small_side(const T* C, int64_t rows, int64_t n, double* G, float* Gf, GramWork& w, bool use_tc,
                            int* used_tc, cudaStream_t st) {
   const bool tall = rows >= n;
   if (used_tc) *used_tc = 0;
   if (tall) {
-    if (use_tc && w.tc_ws && std::is_same<T, float>::value) {
-      if (used_tc) *used_tc = 1;
-      return gram_tc_f32(reinterpret_cast<const float*>(C), rows, n, G, Gf, w.tc_ws, w.tc_bytes, st);
-    }
+    if constexpr (tc_input<T>())
+      if (use_tc && w.tc_ws) {
+        if (used_tc) *used_tc = std::is_same<T, __nv_bfloat16>::value ? 2 : 1;
+        return gram_tc<T>(C, rows, n, G, Gf, w.tc_ws, w.tc_bytes, st);
+      }
     GemmPlan pl = plan_gemm(n, n, rows, true);
     return gemm_splitk<T, T, double, double, float>(pl, n, n, rows, C, n, false, C, n, false, w.partial, G, n, 1.0,
                                                     nullptr, 0, 0.0, nullptr, 0, 0.0, true, Gf, n, st);
@@ -145,6 +161,13 @@ inline int gram_small_side(const T* C, int64_t rows, int64_t n, double* G, float
   GemmPlan pl = plan_gemm(rows, rows, n, true);
   return gemm_splitk<T, T, double, double, float>(pl, rows, rows, n, C, n, true, C, n, true, w.partial, G, rows, 1.0,
                                                   nullptr, 0, 0.0, nullptr, 0, 0.0, true, Gf, rows, st);
+}
+
+// The accept rule's noise level for a Gram made as gram_small_side's *used_tc says (0: exact, nothing to guard), and,
+// when its eigenpairs come from an fp32 solve, at least the TF32 level that covers the solve (spec_step_eig_begin).
+inline double gram_noise(int used_tc, bool fp32_solve = false) {
+  const double g = used_tc == 2 ? BF16_GRAM_NOISE : used_tc ? TF32_GRAM_NOISE : 0.0;
+  return fp32_solve ? std::max(g, TF32_GRAM_NOISE) : g;
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -220,7 +243,7 @@ inline int eig_run(const double* G, const TBk* Gb_in, int64_t L, EigWork<TBk>& e
 template <typename TBk>
 inline int eig_solve_and_rank(const double* G, const TBk* Gb, int64_t L, EigWork<TBk>& ew, SweepScalars* sc, int* h_sc,
                               int32_t rm, int batch_mode, ChfsiStats* total, int* solves, cudaStream_t st, bool allow_tc,
-                              bool shared_gpu, int used_tf32 = 0) {
+                              bool shared_gpu, int used_tc = 0) {
   const SweepScalars* hs = reinterpret_cast<const SweepScalars*>(h_sc);
   const bool adaptive = ew.chfsi && ew.adaptive;
   int k_try = adaptive ? 32 : 0;
@@ -239,7 +262,7 @@ inline int eig_solve_and_rank(const double* G, const TBk* Gb, int64_t L, EigWork
           total->rr_sweeps += cs.rr_sweeps;
     if (solves) *solves += 1;
     rank_rule_kernel<<<1, 32, 0, st>>>(ew.w, (int)L, ew.chfsi ? ew.k_run : (int)L, rm, ew.chfsi ? 1 : 0, batch_mode, sc,
-                                       used_tf32, ew.chfsi ? ew.b_run : (int)L);
+                                       gram_noise(used_tc), ew.chfsi ? ew.b_run : (int)L);
     TNB_LAUNCH_CHECK();
     TNB_CUDA(cudaMemcpyAsync(h_sc, sc, sizeof(SweepScalars), cudaMemcpyDeviceToHost, st));
     TNB_CUDA(cudaStreamSynchronize(st));
@@ -310,35 +333,31 @@ struct StepCtx {
   int32_t* d_ranks = nullptr;   // device copy of the ranks the rule chose, [N + 1]
 };
 
-template <typename T, class ArenaT>
-inline int truncate_step(ArenaT& ar, bool dry, const StepCtx& cx, const T* C, int64_t rows, int64_t n, int64_t rank_cap,
+// TIn: the element type of C (the dense input at step 0, else T).
+template <typename T, typename TIn, class ArenaT>
+inline int truncate_step(ArenaT& ar, bool dry, const StepCtx& cx, const TIn* C, int64_t rows, int64_t n, int64_t rank_cap,
                          bool have_rmax, int32_t rm, bool first_step, T* core, T* Cn, int64_t* rank_out) {
   typedef T TBk;  // block precision of the subspace eigensolver follows the data
   const bool tall = rows >= n;
   const int64_t L = tall ? n : rows;
   const int batch_mode = (cx.flags & TNB_FLAG_BATCH_MODE) ? 1 : 0;
   cudaStream_t st = cx.st;
-  GramWork<T> gw;
+  GramWork gw;
   EigWork<TBk> ew;
   // The TF32 Gram equals (1 - c) * G, c ~ 7e-4 (operand truncation shrinks every product alike: harmless, the rank
   // rule works on ratios) plus noise of ~1.6e-6 * ||G|| (measured, tests/test_model.py) — a floor under the tail
   // energies the rank rule can resolve.  An eps budget between "inactive" and 1e-4 of the trace needs finer
   // resolution than that: those sweeps take the exact-product fp64-accumulating Gram instead.
   const bool tc_gram = cx.allow_tc && !cx.exact_gram && (dry || cx.eps_scaled2 < 1e-20 || cx.eps_scaled2 >= 1e-4);
-  gram_carve<T>(ar, rows, n, tc_gram, gw);
+  gram_carve<TIn>(ar, rows, n, tc_gram, gw);
   double* G = ar.template take<double>((size_t)L * L);
   float* Gf = nullptr;
   const int64_t kcap = std::min<int64_t>(rank_cap, L);
   TNB_TRY(eig_carve<TBk>(ar, L, kcap, have_rmax, ew));
   if (ew.chfsi && std::is_same<TBk, float>::value) Gf = reinterpret_cast<float*>(ew.Gb);
   T* fac = ar.template take<T>((size_t)L * (size_t)kcap);  // V_r or U_r/s
-  void* ptc_ws = nullptr;
-  size_t ptc_bytes = 0;
-  if (cx.allow_tc && std::is_same<T, float>::value && tall && rows >= PROJ_TC_MIN_ROWS && kcap <= PT_MAX_N && n % 4 == 0 &&
-      n >= 32) {
-    ptc_bytes = project_tc_workspace_bytes(n, kcap);
-    ptc_ws = ar.template take<char>(ptc_bytes);
-  }
+  const size_t ptc_bytes = project_tc_carve_bytes<TIn>(cx.allow_tc, rows, n, kcap);
+  void* ptc_ws = ptc_bytes ? ar.template take<char>(ptc_bytes) : nullptr;
   if (dry) return TNB_OK;
   if (!ar.ok) return fail(TNB_ERR_WORKSPACE, "workspace too small (need > %zu bytes)", ar.off);
   Prof& prof = Prof::get();
@@ -347,9 +366,9 @@ inline int truncate_step(ArenaT& ar, bool dry, const StepCtx& cx, const T* C, in
   const bool concurrent = (cx.flags & TNB_FLAG_CONCURRENT) != 0;
   {
     BigKernelGate gate(st, concurrent && gw.tc_ws != nullptr);
-    TNB_TRY(gram_small_side<T>(C, rows, n, G, Gf, gw, tc_gram, &used_tc, st));
+    TNB_TRY(gram_small_side<TIn>(C, rows, n, G, Gf, gw, tc_gram, &used_tc, st));
   }
-  if (cx.info) cx.info->tc_grams += used_tc;
+  if (cx.info) cx.info->tc_grams += used_tc ? 1 : 0;
   trace_kernel<<<1, 256, 0, st>>>(G, (int)L, (int)L, cx.sc, first_step ? 1 : 0, cx.eps_scaled2);
   TNB_LAUNCH_CHECK();
   prof.mark(st);
@@ -362,7 +381,7 @@ inline int truncate_step(ArenaT& ar, bool dry, const StepCtx& cx, const T* C, in
     // the exact-product, fp64-accumulated Gram
     if (cx.info) cx.info->tc_grams -= 1;
     used_tc = 0;
-    TNB_TRY(gram_small_side<T>(C, rows, n, G, Gf, gw, false, nullptr, st));
+    TNB_TRY(gram_small_side<TIn>(C, rows, n, G, Gf, gw, false, nullptr, st));
     trace_kernel<<<1, 256, 0, st>>>(G, (int)L, (int)L, cx.sc, first_step ? 1 : 0, cx.eps_scaled2);
     TNB_LAUNCH_CHECK();
     TNB_TRY(eig_solve_and_rank<TBk>(G, reinterpret_cast<const TBk*>(Gf), L, ew, cx.sc, cx.h_sc, rm, batch_mode, &cs, &solves,
@@ -389,14 +408,14 @@ inline int truncate_step(ArenaT& ar, bool dry, const StepCtx& cx, const T* C, in
     TNB_LAUNCH_CHECK();
     {
       BigKernelGate gate(st, concurrent && rows >= PROJ_TC_MIN_ROWS);
-      TNB_TRY(project_any<T>(C, rows, n, fac, rank, Cn, st, ptc_ws, ptc_bytes));
+      TNB_TRY((project_any<T, TIn>(C, rows, n, fac, rank, Cn, st, ptc_ws, ptc_bytes)));
     }
   } else {
     // core = diag(1/s) U_r^T C (rank x n);  Cn = U_r diag(s)
     scale_extract_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(ew.V, ew.ldv, (int)rows, (int)rank, ew.w, fac, 1, 0);
     TNB_LAUNCH_CHECK();
-    TNB_TRY((gemm_direct<T, T, T, T>(rank, n, rows, fac, rank, false, C, n, false, core, n, (T)1, nullptr, 0, (T)0,
-                                     nullptr, 0, (T)0, st)));
+    TNB_TRY((gemm_direct<T, TIn, T, T>(rank, n, rows, fac, rank, false, C, n, false, core, n, (T)1, nullptr, 0, (T)0,
+                                       nullptr, 0, (T)0, st)));
     scale_extract_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(ew.V, ew.ldv, (int)rows, (int)rank, ew.w, Cn, 2, 0);
     TNB_LAUNCH_CHECK();
   }
@@ -428,7 +447,7 @@ inline bool spec_step_ok(int64_t rows, int64_t n, int64_t rank_cap, bool allow_t
 // back to back while the latency-bound eigen chains of the other tensors run beside them on their own streams.
 template <typename T>
 struct SpecStep {
-  GramWork<T> gw;
+  GramWork gw;
   double *G = nullptr, *w = nullptr, *V = nullptr, *jscratch = nullptr;
   int* jinfo = nullptr;
   float* Gf = nullptr;
@@ -438,19 +457,20 @@ struct SpecStep {
   size_t ptc_bytes = 0;
   int ldv = 0, b = 0, used_tc = 0;
   bool chfsi = false, tc_gram = false;
+  bool fp32_solve = false;    // the small Gram's eigenpairs come from fp32 Jacobi rotations
   bool in_kblocked = false;   // C is K-blocked (carry_kblocked of this step)
   int64_t out_inner = 0;      // > 0: write Cn K-blocked for the next step, whose rows hold out_inner rows of Cn each
   int64_t L = 0, kcap = 0;
   CdRun cd;  // the subspace solve of this step, enqueued stage by stage
 };
 
-template <typename T, class ArenaT>
+template <typename T, typename TIn, class ArenaT>
 inline void spec_step_carve(ArenaT& ar, const StepCtx& cx, int64_t rows, int64_t n, int64_t rank_cap, SpecStep<T>& s) {
   const bool tall = rows >= n;
   s.L = tall ? n : rows;
   const int64_t L = s.L;
   s.tc_gram = cx.allow_tc && !cx.exact_gram;
-  gram_carve<T>(ar, rows, n, s.tc_gram, s.gw);
+  gram_carve<TIn>(ar, rows, n, s.tc_gram, s.gw);
   s.G = ar.template take<double>((size_t)L * L);
   s.kcap = std::min<int64_t>(rank_cap, L);
   s.chfsi = L > JACOBI_MAX_N;
@@ -471,18 +491,13 @@ inline void spec_step_carve(ArenaT& ar, const StepCtx& cx, int64_t rows, int64_t
     chfsi_dev_carve<float>(ar, (int)L, s.b, s.cw);
   }
   s.fac = ar.template take<T>((size_t)L * (size_t)s.kcap);
-  s.ptc_ws = nullptr;
-  s.ptc_bytes = 0;
-  if (cx.allow_tc && std::is_same<T, float>::value && tall && rows >= PROJ_TC_MIN_ROWS && s.kcap <= PT_MAX_N && n % 4 == 0 &&
-      n >= 32) {
-    s.ptc_bytes = project_tc_workspace_bytes(n, s.kcap);
-    s.ptc_ws = ar.template take<char>(s.ptc_bytes);
-  }
+  s.ptc_bytes = project_tc_carve_bytes<TIn>(cx.allow_tc, rows, n, s.kcap);
+  s.ptc_ws = s.ptc_bytes ? ar.template take<char>(s.ptc_bytes) : nullptr;
 }
 
 // phase 1: Gram + trace
-template <typename T>
-inline int spec_step_gram(const StepCtx& cx, const T* C, int64_t rows, int64_t n, bool first_step, SpecStep<T>& s, bool prof_on) {
+template <typename T, typename TIn>
+inline int spec_step_gram(const StepCtx& cx, const TIn* C, int64_t rows, int64_t n, bool first_step, SpecStep<T>& s, bool prof_on) {
   cudaStream_t st = cx.st;
   Prof& prof = Prof::get();
   if (prof_on) prof.mark(st);
@@ -491,12 +506,12 @@ inline int spec_step_gram(const StepCtx& cx, const T* C, int64_t rows, int64_t n
     BigKernelGate gate(st, concurrent && s.gw.tc_ws != nullptr);
     if (s.in_kblocked) {
       s.used_tc = 1;
-      TNB_TRY(gram_tc_f32(reinterpret_cast<const float*>(C), rows, n, s.G, s.Gf, s.gw.tc_ws, s.gw.tc_bytes, st, true));
+      TNB_TRY(gram_tc(reinterpret_cast<const float*>(C), rows, n, s.G, s.Gf, s.gw.tc_ws, s.gw.tc_bytes, st, true));
     } else {
-      TNB_TRY(gram_small_side<T>(C, rows, n, s.G, s.Gf, s.gw, s.tc_gram, &s.used_tc, st));
+      TNB_TRY(gram_small_side<TIn>(C, rows, n, s.G, s.Gf, s.gw, s.tc_gram, &s.used_tc, st));
     }
   }
-  if (cx.info) cx.info->tc_grams += s.used_tc, cx.info->kblocked_steps += s.in_kblocked ? 1 : 0;
+  if (cx.info) cx.info->tc_grams += s.used_tc ? 1 : 0, cx.info->kblocked_steps += s.in_kblocked ? 1 : 0;
   trace_kernel<<<1, 256, 0, st>>>(s.G, (int)s.L, (int)s.L, cx.sc, first_step ? 1 : 0, cx.eps_scaled2);
   TNB_LAUNCH_CHECK();
   if (prof_on) prof.mark(st);
@@ -518,8 +533,9 @@ inline int spec_step_eig_begin(const StepCtx& cx, SpecStep<T>& s) {
     // The same holds for fp32 DATA whatever Gram kernel produced G, as long as the accept rule — which then guards the
     // fp32 solve instead of the TF32 Gram, same noise allowance — finds the spectrum benign; a rejected step is repeated
     // on the host-driven path with fp64 rotations.
+    // The rule then allows for the larger of the Gram kernel's noise and the fp32 solve's (gram_noise).
     const bool single = std::is_same<T, float>::value && (cx.allow_tc && !cx.exact_gram) && jacobi2_ok((int)L, true);
-    s.used_tc = (s.used_tc || single) ? 1 : 0;
+    s.fp32_solve = single;
     return jacobi2_eigh(s.G, (int)L, (int)L, s.w, s.V, s.jscratch, s.jinfo, st, single, single ? 2e-7 : 0.0);
   }
   if (cx.info) cx.info->eig_solves += 1;
@@ -531,8 +547,8 @@ inline int spec_step_eig_stage(SpecStep<T>& s, int stage) {
 }
 
 // phase 2b: end of the eigen stage, rank rule + speculation check, factor extraction, projection
-template <typename T>
-inline int spec_step_rest(const StepCtx& cx, const T* C, int64_t rows, int64_t n, int32_t rm, T* core, T* Cn, int mu,
+template <typename T, typename TIn>
+inline int spec_step_rest(const StepCtx& cx, const TIn* C, int64_t rows, int64_t n, int32_t rm, T* core, T* Cn, int mu,
                           SpecStep<T>& s, bool prof_on) {
   const bool tall = rows >= n;
   const int64_t L = s.L;
@@ -541,10 +557,11 @@ inline int spec_step_rest(const StepCtx& cx, const T* C, int64_t rows, int64_t n
   Prof& prof = Prof::get();
   const bool concurrent = (cx.flags & TNB_FLAG_CONCURRENT) != 0;
   if (!s.chfsi) {
-    rank_rule_kernel<<<1, 32, 0, st>>>(s.w, (int)L, (int)L, rm, 0, batch_mode, cx.sc, s.used_tc, (int)L);
+    rank_rule_kernel<<<1, 32, 0, st>>>(s.w, (int)L, (int)L, rm, 0, batch_mode, cx.sc, gram_noise(s.used_tc, s.fp32_solve),
+                                       (int)L);
   } else {
     TNB_TRY(cd_end(s.cd));
-    rank_rule_kernel<<<1, 32, 0, st>>>(s.w, (int)L, (int)s.kcap, rm, 1, batch_mode, cx.sc, s.used_tc, s.b);
+    rank_rule_kernel<<<1, 32, 0, st>>>(s.w, (int)L, (int)s.kcap, rm, 1, batch_mode, cx.sc, gram_noise(s.used_tc), s.b);
   }
   TNB_LAUNCH_CHECK();
   spec_check_kernel<<<1, 32, 0, st>>>(cx.sc, (int)s.kcap, cx.d_ranks + mu, cx.d_flags);
@@ -558,18 +575,20 @@ inline int spec_step_rest(const StepCtx& cx, const T* C, int64_t rows, int64_t n
     TNB_LAUNCH_CHECK();
     {
       BigKernelGate gate(st, concurrent && rows >= PROJ_TC_MIN_ROWS);
-      if (s.in_kblocked || s.out_inner > 0)
-        TNB_TRY(project_tc_f32(reinterpret_cast<const float*>(C), rows, n, reinterpret_cast<const float*>(s.fac), (int)rank,
-                               reinterpret_cast<float*>(Cn), s.ptc_ws, s.ptc_bytes, st,
-                               s.in_kblocked ? PT_IN_KBLOCKED : PT_OUT_KBLOCKED, s.out_inner));
-      else
-        TNB_TRY(project_any<T>(C, rows, n, s.fac, rank, Cn, st, s.ptc_ws, s.ptc_bytes));
+      bool blocked = false;
+      if constexpr (tc_input<TIn>()) {
+        blocked = s.in_kblocked || s.out_inner > 0;
+        if (blocked)
+          TNB_TRY(project_tc<TIn>(C, rows, n, reinterpret_cast<const float*>(s.fac), (int)rank, reinterpret_cast<float*>(Cn),
+                                  s.ptc_ws, s.ptc_bytes, st, s.in_kblocked ? PT_IN_KBLOCKED : PT_OUT_KBLOCKED, s.out_inner));
+      }
+      if (!blocked) TNB_TRY((project_any<T, TIn>(C, rows, n, s.fac, rank, Cn, st, s.ptc_ws, s.ptc_bytes)));
     }
   } else {
     scale_extract_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(s.V, s.ldv, (int)rows, (int)rank, s.w, s.fac, 1, 0);
     TNB_LAUNCH_CHECK();
-    TNB_TRY((gemm_direct<T, T, T, T>(rank, n, rows, s.fac, rank, false, C, n, false, core, n, (T)1, nullptr, 0, (T)0,
-                                     nullptr, 0, (T)0, st)));
+    TNB_TRY((gemm_direct<T, TIn, T, T>(rank, n, rows, s.fac, rank, false, C, n, false, core, n, (T)1, nullptr, 0, (T)0,
+                                       nullptr, 0, (T)0, st)));
     scale_extract_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(s.V, s.ldv, (int)rows, (int)rank, s.w, Cn, 2, 0);
     TNB_LAUNCH_CHECK();
   }
@@ -580,8 +599,9 @@ inline int spec_step_rest(const StepCtx& cx, const T* C, int64_t rows, int64_t n
 // ---------------------------------------------------------------------------------------------
 // Dense TT-SVD
 // ---------------------------------------------------------------------------------------------
-template <typename T, class ArenaT>
-inline int ttsvd_sync_impl(ArenaT& ar, bool dry, const T* data, const SweepDims& d, const int32_t* rmax, double eps,
+// T: carries and cores; TIn: the dense input (T, or bf16 with T = float), read by step 0 only.
+template <typename T, typename TIn, class ArenaT>
+inline int ttsvd_sync_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d, const int32_t* rmax, double eps,
                            uint32_t flags, T* cores, int32_t* ranks_host, SweepInfo* info, cudaStream_t st,
                            bool exact_gram = false) {
   const int N = d.N;
@@ -605,7 +625,12 @@ inline int ttsvd_sync_impl(ArenaT& ar, bool dry, const T* data, const SweepDims&
   }
   if (N == 1) {
     if (!dry) {
-      TNB_CUDA(cudaMemcpyAsync(cores + d.slot[0], data, sizeof(T) * d.shape[0], cudaMemcpyDeviceToDevice, st));
+      if (std::is_same<T, TIn>::value) {
+        TNB_CUDA(cudaMemcpyAsync(cores + d.slot[0], data, sizeof(T) * d.shape[0], cudaMemcpyDeviceToDevice, st));
+      } else {  // the single core is the data, converted
+        convert_kernel<T, TIn><<<grid_for(d.shape[0]), 256, 0, st>>>(data, d.shape[0], cores + d.slot[0]);
+        TNB_LAUNCH_CHECK();
+      }
       TNB_CUDA(cudaStreamSynchronize(st));
       if (info) info->norm = 0;
     }
@@ -618,7 +643,7 @@ inline int ttsvd_sync_impl(ArenaT& ar, bool dry, const T* data, const SweepDims&
     if (e > carry_elems[t & 1]) carry_elems[t & 1] = e;
   }
   T* carry[2] = {ar.template take<T>(carry_elems[0]), ar.template take<T>(carry_elems[1])};
-  const T* C = data;
+  const T* C = nullptr;  // the carry step t > 0 reads; step 0 reads data
   int64_t r_next = 1;
   size_t peak = ar.off;
   for (int mu = N - 1, t = 0; mu >= 1; --mu, ++t) {
@@ -627,8 +652,12 @@ inline int ttsvd_sync_impl(ArenaT& ar, bool dry, const T* data, const SweepDims&
     const bool have_rmax = rmax && rmax[mu - 1] > 0;
     const size_t mark = ar.off;
     int64_t rank = d.rcap[mu];
-    TNB_TRY((truncate_step<T>(ar, dry, cx, C, rows, n, d.rcap[mu], have_rmax, have_rmax ? rmax[mu - 1] : 0, t == 0,
-                              dry ? nullptr : cores + d.slot[mu], carry[t & 1], &rank)));
+    T* core = dry ? nullptr : cores + d.slot[mu];
+    const int32_t rm = have_rmax ? rmax[mu - 1] : 0;
+    if (t == 0)
+      TNB_TRY((truncate_step<T, TIn>(ar, dry, cx, data, rows, n, d.rcap[mu], have_rmax, rm, true, core, carry[0], &rank)));
+    else
+      TNB_TRY((truncate_step<T, T>(ar, dry, cx, C, rows, n, d.rcap[mu], have_rmax, rm, false, core, carry[t & 1], &rank)));
     if (!dry) {
       ranks_host[mu] = (int32_t)rank;
       r_next = rank;
@@ -688,12 +717,13 @@ struct SpecHostBack {  // pinned read-back of one speculative sweep
 };
 
 // One tensor of a speculative sweep (or of a batch of them): its arena, device scalars, carries and position.
-template <typename T, class ArenaT>
+template <typename T, typename TIn, class ArenaT>
 struct SpecRun {
   ArenaT* ar = nullptr;
   StepCtx cx;
   SweepInfo info_local;
-  const T* C = nullptr;
+  const TIn* data = nullptr;  // read by step 0
+  const T* C = nullptr;       // the carry later steps read
   T* carry[2] = {nullptr, nullptr};
   T* cores = nullptr;
   SpecStep<T> step;
@@ -701,8 +731,8 @@ struct SpecRun {
   SpecHostBack* hb = nullptr;
 };
 
-template <typename T, class ArenaT>
-inline int spec_begin(SpecRun<T, ArenaT>& r, ArenaT& ar, bool dry, const T* data, const SweepDims& d, double eps,
+template <typename T, typename TIn, class ArenaT>
+inline int spec_begin(SpecRun<T, TIn, ArenaT>& r, ArenaT& ar, bool dry, const TIn* data, const SweepDims& d, double eps,
                       uint32_t flags, T* cores, SweepInfo* info, cudaStream_t st, SpecHostBack* hb) {
   const int N = d.N;
   r.ar = &ar;
@@ -723,7 +753,8 @@ inline int spec_begin(SpecRun<T, ArenaT>& r, ArenaT& ar, bool dry, const T* data
   }
   r.carry[0] = ar.template take<T>(carry_elems[0]);
   r.carry[1] = ar.template take<T>(carry_elems[1]);
-  r.C = data;
+  r.data = data;
+  r.C = nullptr;
   r.cores = cores;
   r.peak = ar.off;
   r.hb = hb;
@@ -733,46 +764,58 @@ inline int spec_begin(SpecRun<T, ArenaT>& r, ArenaT& ar, bool dry, const T* data
 
 // the step scratch of step t+1 reuses that of step t: the kernels of one stream run in order, and every kernel of
 // step t+1 that writes scratch is enqueued after every kernel of step t that reads it
-template <typename T, class ArenaT>
-inline int spec_phase1(SpecRun<T, ArenaT>& r, bool dry, const SweepDims& d, int mu, int t, bool prof_on) {
+template <typename T, typename TIn, class ArenaT>
+inline int spec_phase1(SpecRun<T, TIn, ArenaT>& r, bool dry, const SweepDims& d, int mu, int t, bool prof_on) {
   ArenaT& ar = *r.ar;
   r.mark = ar.off;
-  spec_step_carve<T>(ar, r.cx, d.rows[mu], d.shape[mu] * d.rcap[mu + 1], d.rcap[mu], r.step);
-  r.step.in_kblocked = carry_kblocked<T>(d, mu, r.cx.allow_tc);
-  r.step.out_inner = carry_kblocked<T>(d, mu - 1, r.cx.allow_tc) ? d.shape[mu - 1] : 0;
+  const int64_t rows = d.rows[mu], n = d.shape[mu] * d.rcap[mu + 1];
+  if (t == 0)
+    spec_step_carve<T, TIn>(ar, r.cx, rows, n, d.rcap[mu], r.step);
+  else
+    spec_step_carve<T, T>(ar, r.cx, rows, n, d.rcap[mu], r.step);
+  r.step.in_kblocked = carry_kblocked<T, TIn>(d, mu, r.cx.allow_tc);
+  r.step.out_inner = carry_kblocked<T, TIn>(d, mu - 1, r.cx.allow_tc) ? d.shape[mu - 1] : 0;
   if (ar.off > r.peak) r.peak = ar.off;
   if (dry) return TNB_OK;
   if (!ar.ok) return fail(TNB_ERR_WORKSPACE, "workspace too small (need > %zu bytes)", ar.off);
-  return spec_step_gram<T>(r.cx, r.C, d.rows[mu], d.shape[mu] * d.rcap[mu + 1], t == 0, r.step, prof_on);
+  if (t == 0) return spec_step_gram<T, TIn>(r.cx, r.data, rows, n, true, r.step, prof_on);
+  return spec_step_gram<T, T>(r.cx, r.C, rows, n, false, r.step, prof_on);
 }
-template <typename T, class ArenaT>
-inline int spec_phase2a(SpecRun<T, ArenaT>& r, bool dry) {
+template <typename T, typename TIn, class ArenaT>
+inline int spec_phase2a(SpecRun<T, TIn, ArenaT>& r, bool dry) {
   return dry ? TNB_OK : spec_step_eig_begin<T>(r.cx, r.step);
 }
-template <typename T, class ArenaT>
-inline int spec_phase2s(SpecRun<T, ArenaT>& r, bool dry, int stage) {
+template <typename T, typename TIn, class ArenaT>
+inline int spec_phase2s(SpecRun<T, TIn, ArenaT>& r, bool dry, int stage) {
   return dry ? TNB_OK : spec_step_eig_stage<T>(r.step, stage);
 }
-template <typename T, class ArenaT>
-inline int spec_phase2b(SpecRun<T, ArenaT>& r, bool dry, const SweepDims& d, const int32_t* rmax, int mu, int t, bool prof_on) {
+template <typename T, typename TIn, class ArenaT>
+inline int spec_phase2b(SpecRun<T, TIn, ArenaT>& r, bool dry, const SweepDims& d, const int32_t* rmax, int mu, int t,
+                        bool prof_on) {
   ArenaT& ar = *r.ar;
   if (!dry) {
-    TNB_TRY(spec_step_rest<T>(r.cx, r.C, d.rows[mu], d.shape[mu] * d.rcap[mu + 1], rmax[mu - 1], r.cores + d.slot[mu],
-                              r.carry[t & 1], mu, r.step, prof_on));
+    const int64_t rows = d.rows[mu], n = d.shape[mu] * d.rcap[mu + 1];
+    if (t == 0)
+      TNB_TRY((spec_step_rest<T, TIn>(r.cx, r.data, rows, n, rmax[mu - 1], r.cores + d.slot[mu], r.carry[0], mu, r.step,
+                                      prof_on)));
+    else
+      TNB_TRY((spec_step_rest<T, T>(r.cx, r.C, rows, n, rmax[mu - 1], r.cores + d.slot[mu], r.carry[t & 1], mu, r.step,
+                                    prof_on)));
     r.C = r.carry[t & 1];
   }
   ar.off = r.mark;
   return TNB_OK;
 }
 // the whole phase 2 of one tensor
-template <typename T, class ArenaT>
-inline int spec_phase2(SpecRun<T, ArenaT>& r, bool dry, const SweepDims& d, const int32_t* rmax, int mu, int t, bool prof_on) {
-  TNB_TRY((spec_phase2a<T, ArenaT>(r, dry)));
-  for (int stage = 0; stage <= CD_MAX_STAGES; ++stage) TNB_TRY((spec_phase2s<T, ArenaT>(r, dry, stage)));
-  return spec_phase2b<T, ArenaT>(r, dry, d, rmax, mu, t, prof_on);
+template <typename T, typename TIn, class ArenaT>
+inline int spec_phase2(SpecRun<T, TIn, ArenaT>& r, bool dry, const SweepDims& d, const int32_t* rmax, int mu, int t,
+                       bool prof_on) {
+  TNB_TRY(spec_phase2a(r, dry));
+  for (int stage = 0; stage <= CD_MAX_STAGES; ++stage) TNB_TRY(spec_phase2s(r, dry, stage));
+  return spec_phase2b(r, dry, d, rmax, mu, t, prof_on);
 }
-template <typename T, class ArenaT>
-inline int spec_end(SpecRun<T, ArenaT>& r, const SweepDims& d) {
+template <typename T, typename TIn, class ArenaT>
+inline int spec_end(SpecRun<T, TIn, ArenaT>& r, const SweepDims& d) {
   cudaStream_t st = r.cx.st;
   const int N = d.N;
   TNB_CUDA(cudaMemcpyAsync(r.cores + d.slot[0], r.C, sizeof(T) * (size_t)d.shape[0] * (size_t)d.rcap[1],
@@ -799,8 +842,8 @@ inline void spec_collect(const SpecHostBack* hb, const SweepDims& d, int32_t* ra
   }
 }
 
-template <typename T, class ArenaT>
-inline int ttsvd_spec_impl(ArenaT& ar, bool dry, const T* data, const SweepDims& d, const int32_t* rmax, double eps,
+template <typename T, typename TIn, class ArenaT>
+inline int ttsvd_spec_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d, const int32_t* rmax, double eps,
                            uint32_t flags, T* cores, int32_t* ranks_host, SweepInfo* info, cudaStream_t st,
                            SpecOutcome* out) {
   const int N = d.N;
@@ -813,11 +856,11 @@ inline int ttsvd_spec_impl(ArenaT& ar, bool dry, const T* data, const SweepDims&
     hb = static_cast<SpecHostBack*>(pinned_scratch(sizeof(SpecHostBack)));
     if (!hb) return fail(TNB_ERR_CUDA, "pinned scratch allocation failed");
   }
-  SpecRun<T, ArenaT> r;
-  TNB_TRY((spec_begin<T, ArenaT>(r, ar, dry, data, d, eps, flags, cores, info, st, hb)));
+  SpecRun<T, TIn, ArenaT> r;
+  TNB_TRY(spec_begin(r, ar, dry, data, d, eps, flags, cores, info, st, hb));
   for (int mu = N - 1, t = 0; mu >= 1; --mu, ++t) {
-    int rc = spec_phase1<T, ArenaT>(r, dry, d, mu, t, prof_on);
-    if (rc == TNB_OK) rc = spec_phase2<T, ArenaT>(r, dry, d, rmax, mu, t, prof_on);
+    int rc = spec_phase1(r, dry, d, mu, t, prof_on);
+    if (rc == TNB_OK) rc = spec_phase2(r, dry, d, rmax, mu, t, prof_on);
     if (rc != TNB_OK) {
       if (!dry) cudaStreamSynchronize(st);  // part of the sweep is enqueued: drain it before the host-driven path
       prof.on = false;
@@ -828,7 +871,7 @@ inline int ttsvd_spec_impl(ArenaT& ar, bool dry, const T* data, const SweepDims&
     ar.off = r.peak;
     return TNB_OK;
   }
-  TNB_TRY((spec_end<T, ArenaT>(r, d)));
+  TNB_TRY(spec_end(r, d));
   TNB_CUDA(cudaStreamSynchronize(st));
   spec_collect(hb, d, ranks_host, info, out);
   if (prof_on && info) {
@@ -849,8 +892,8 @@ inline int ttsvd_spec_impl(ArenaT& ar, bool dry, const T* data, const SweepDims&
 }
 
 // Dispatcher: speculative sweep when a rank cap decides every bond, host-driven sweep otherwise and as the fallback.
-template <typename T, class ArenaT>
-inline int ttsvd_impl(ArenaT& ar, bool dry, const T* data, const SweepDims& d, const int32_t* rmax, double eps,
+template <typename T, typename TIn, class ArenaT>
+inline int ttsvd_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d, const int32_t* rmax, double eps,
                       uint32_t flags, T* cores, int32_t* ranks_host, SweepInfo* info, cudaStream_t st) {
   const bool allow_tc = !(flags & TNB_FLAG_NO_TENSORCORE) && (dry || tc_path_available());
   // the sizing pass cannot ask the device what it supports: size for both paths
@@ -863,7 +906,7 @@ inline int ttsvd_impl(ArenaT& ar, bool dry, const T* data, const SweepDims& d, c
       for (int mu = 1; mu < d.N; ++mu) all_caps = all_caps && rmax[mu - 1] > 0;
       if (all_caps) {
         SpecOutcome o;
-        const int rc = ttsvd_spec_impl<T>(ar, true, data, d, rmax, eps, flags, cores, ranks_host, info, st, &o);
+        const int rc = ttsvd_spec_impl<T, TIn>(ar, true, data, d, rmax, eps, flags, cores, ranks_host, info, st, &o);
         if (rc == TNB_OK) need_spec = ar.off - base;
         ar.off = base;
       }
@@ -871,7 +914,7 @@ inline int ttsvd_impl(ArenaT& ar, bool dry, const T* data, const SweepDims& d, c
       SpecOutcome o;
       SweepInfo saved;
       if (info) saved = *info;
-      const int rc = ttsvd_spec_impl<T>(ar, false, data, d, rmax, eps, flags, cores, ranks_host, info, st, &o);
+      const int rc = ttsvd_spec_impl<T, TIn>(ar, false, data, d, rmax, eps, flags, cores, ranks_host, info, st, &o);
       if (rc == TNB_OK && o.ran && o.flags == 0) {
         if (info) info->speculative = 1;
         return TNB_OK;
@@ -882,10 +925,10 @@ inline int ttsvd_impl(ArenaT& ar, bool dry, const T* data, const SweepDims& d, c
       if (info) { *info = saved; info->spec_flags = o.flags; }
       ar.off = base;
       ar.ok = true;
-      return ttsvd_sync_impl<T>(ar, false, data, d, rmax, eps, flags, cores, ranks_host, info, st, (o.flags & 1) != 0);
+      return ttsvd_sync_impl<T, TIn>(ar, false, data, d, rmax, eps, flags, cores, ranks_host, info, st, (o.flags & 1) != 0);
     }
   }
-  const int rc = ttsvd_sync_impl<T>(ar, dry, data, d, rmax, eps, flags, cores, ranks_host, info, st);
+  const int rc = ttsvd_sync_impl<T, TIn>(ar, dry, data, d, rmax, eps, flags, cores, ranks_host, info, st);
   if (dry && rc == TNB_OK && need_spec > ar.off - base) ar.off = base + need_spec;
   return rc;
 }
@@ -916,8 +959,8 @@ struct StreamPool {
   }
 };
 
-template <typename T>
-inline int ttsvd_batch_impl(void* workspace, size_t per_tensor_bytes, int inflight, const T* const* data, int batch,
+template <typename T, typename TIn>
+inline int ttsvd_batch_impl(void* workspace, size_t per_tensor_bytes, int inflight, const TIn* const* data, int batch,
                             const SweepDims& d, const int32_t* rmax, double eps, uint32_t flags, T* const* cores,
                             int32_t* ranks_host, double* norms_host, int32_t* spec_host, cudaStream_t st) {
   const int N = d.N;
@@ -928,7 +971,8 @@ inline int ttsvd_batch_impl(void* workspace, size_t per_tensor_bytes, int inflig
     for (int i = 0; i < batch; ++i) {
       Arena ar(ws, per_tensor_bytes);
       SweepInfo info;
-      TNB_TRY((ttsvd_impl<T, Arena>(ar, false, data[i], d, rmax, eps, flags, cores[i], ranks_host + (size_t)i * (N + 1), &info, st)));
+      TNB_TRY((ttsvd_impl<T, TIn, Arena>(ar, false, data[i], d, rmax, eps, flags, cores[i], ranks_host + (size_t)i * (N + 1), &info,
+                                         st)));
       if (norms_host) norms_host[i] = info.norm;
       if (spec_host) spec_host[i] = info.speculative;
     }
@@ -951,11 +995,11 @@ inline int ttsvd_batch_impl(void* workspace, size_t per_tensor_bytes, int inflig
     const int g = std::min(inflight, batch - g0);
     std::vector<Arena> arenas;
     arenas.reserve(g);
-    std::vector<SpecRun<T, Arena>> runs(g);
+    std::vector<SpecRun<T, TIn, Arena>> runs(g);
     for (int s = 0; s < g; ++s) arenas.emplace_back(ws + (size_t)s * per_tensor_bytes, per_tensor_bytes);
     for (int s = 0; s < g && rc == TNB_OK; ++s)
-      rc = spec_begin<T, Arena>(runs[s], arenas[s], false, data[g0 + s], d, eps, bflags, cores[g0 + s], &infos[g0 + s],
-                                pool.st[s], hbs + g0 + s);
+      rc = spec_begin(runs[s], arenas[s], false, data[g0 + s], d, eps, bflags, cores[g0 + s], &infos[g0 + s], pool.st[s],
+                      hbs + g0 + s);
     // Enqueue order (TNB_BATCH_ORDER):
     //   "stage" (default): step by step; all Gram kernels of a step, then the eigen stages of all tensors INTERLEAVED
     //            stage by stage (the resident filter kernels of all streams run one after the other, cheb_filter.cuh:
@@ -971,27 +1015,27 @@ inline int ttsvd_batch_impl(void* workspace, size_t per_tensor_bytes, int inflig
       for (int w = 0; w < steps + g - 1 && rc == TNB_OK; ++w) {
         for (int s = 0; s < g && rc == TNB_OK; ++s) {
           const int t = w - s;
-          if (t >= 0 && t < steps) rc = spec_phase1<T, Arena>(runs[s], false, d, N - 1 - t, t, false);
+          if (t >= 0 && t < steps) rc = spec_phase1(runs[s], false, d, N - 1 - t, t, false);
         }
         for (int s = 0; s < g && rc == TNB_OK; ++s) {
           const int t = w - s;
-          if (t >= 0 && t < steps) rc = spec_phase2<T, Arena>(runs[s], false, d, rmax, N - 1 - t, t, false);
+          if (t >= 0 && t < steps) rc = spec_phase2(runs[s], false, d, rmax, N - 1 - t, t, false);
         }
       }
     } else {
       for (int mu = N - 1, t = 0; mu >= 1 && rc == TNB_OK; --mu, ++t) {
-        for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase1<T, Arena>(runs[s], false, d, mu, t, false);
+        for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase1(runs[s], false, d, mu, t, false);
         if (order_phase) {
-          for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase2<T, Arena>(runs[s], false, d, rmax, mu, t, false);
+          for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase2(runs[s], false, d, rmax, mu, t, false);
         } else {
-          for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase2a<T, Arena>(runs[s], false);
+          for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase2a(runs[s], false);
           for (int stage = 0; stage <= CD_MAX_STAGES && rc == TNB_OK; ++stage)
-            for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase2s<T, Arena>(runs[s], false, stage);
-          for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase2b<T, Arena>(runs[s], false, d, rmax, mu, t, false);
+            for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase2s(runs[s], false, stage);
+          for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase2b(runs[s], false, d, rmax, mu, t, false);
         }
       }
     }
-    for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_end<T, Arena>(runs[s], d);
+    for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_end(runs[s], d);
   }
   // join: the caller's stream continues after every internal stream; then the one host synchronisation
   for (int s = 0; s < inflight; ++s) {
@@ -1014,7 +1058,7 @@ inline int ttsvd_batch_impl(void* workspace, size_t per_tensor_bytes, int inflig
     // repeat this tensor on the host-driven path (exact Gram when the TF32 one was rejected)
     Arena ar(ws, per_tensor_bytes);
     SweepInfo info;
-    TNB_TRY((ttsvd_sync_impl<T, Arena>(ar, false, data[i], d, rmax, eps, flags & ~TNB_FLAG_PROFILE, cores[i], rk, &info, st,
+    TNB_TRY((ttsvd_sync_impl<T, TIn, Arena>(ar, false, data[i], d, rmax, eps, flags & ~TNB_FLAG_PROFILE, cores[i], rk, &info, st,
                                        (outs[i].flags & 1) != 0)));
     if (norms_host) norms_host[i] = info.norm;
     if (spec_host) spec_host[i] = 0;

@@ -22,6 +22,13 @@ inline int check_dtype(int dtype) {
   if (dtype != TNB_F32 && dtype != TNB_F64) return fail(TNB_ERR_INVALID, "dtype must be TNB_F32 or TNB_F64, got %d", dtype);
   return TNB_OK;
 }
+// The dense TT-SVD entry points also take bf16 input (fp32 cores).
+inline int check_ttsvd_dtype(int dtype) {
+  if (dtype != TNB_F32 && dtype != TNB_F64 && dtype != TNB_BF16)
+    return fail(TNB_ERR_INVALID, "dtype must be TNB_F32, TNB_F64 or TNB_BF16, got %d", dtype);
+  return TNB_OK;
+}
+inline size_t dtype_bytes(int dtype) { return dtype == TNB_F64 ? 8 : dtype == TNB_F32 ? 4 : 2; }
 inline int require_device() {
   int dev = -1;
   if (cudaGetDevice(&dev) != cudaSuccess || !device_info().valid) {
@@ -53,13 +60,16 @@ int64_t tnb_ttsvd_cores_capacity(int ndim, const int64_t* shape, const int32_t* 
 
 size_t tnb_ttsvd_workspace_bytes(int dtype, int ndim, const int64_t* shape, const int32_t* rmax, uint32_t flags) {
   SweepDims d;
-  if (check_dtype(dtype) != TNB_OK || make_dims(ndim, shape, rmax, d) != TNB_OK) return 0;
+  if (check_ttsvd_dtype(dtype) != TNB_OK || make_dims(ndim, shape, rmax, d) != TNB_OK) return 0;
   ArenaSizer ar;
   int rc;
   if (dtype == TNB_F32)
-    rc = ttsvd_impl<float>(ar, true, nullptr, d, rmax, 0.0, flags, nullptr, nullptr, nullptr, 0);
+    rc = ttsvd_impl<float, float>(ar, true, (const float*)nullptr, d, rmax, 0.0, flags, nullptr, nullptr, nullptr, 0);
+  else if (dtype == TNB_BF16)
+    rc = ttsvd_impl<float, __nv_bfloat16>(ar, true, (const __nv_bfloat16*)nullptr, d, rmax, 0.0, flags, nullptr, nullptr,
+                                          nullptr, 0);
   else
-    rc = ttsvd_impl<double>(ar, true, nullptr, d, rmax, 0.0, flags, nullptr, nullptr, nullptr, 0);
+    rc = ttsvd_impl<double, double>(ar, true, (const double*)nullptr, d, rmax, 0.0, flags, nullptr, nullptr, nullptr, 0);
   if (rc != TNB_OK) return 0;
   return with_slack(ar.off);
 }
@@ -67,7 +77,7 @@ size_t tnb_ttsvd_workspace_bytes(int dtype, int ndim, const int64_t* shape, cons
 int tnb_ttsvd(int dtype, const void* data, int ndim, const int64_t* shape, const int32_t* rmax, double eps,
               uint32_t flags, void* workspace, size_t workspace_bytes, void* cores, int64_t cores_capacity,
               int32_t* ranks_host, double* info_host, void* stream) {
-  TNB_TRY(check_dtype(dtype));
+  TNB_TRY(check_ttsvd_dtype(dtype));
   TNB_TRY(require_device());
   if (!data || !shape || !cores || !ranks_host || !workspace) return fail(TNB_ERR_INVALID, "tnb_ttsvd: null argument");
   if (rmax)
@@ -82,11 +92,14 @@ int tnb_ttsvd(int dtype, const void* data, int ndim, const int64_t* shape, const
   SweepInfo info;
   int rc;
   if (dtype == TNB_F32)
-    rc = ttsvd_impl<float>(ar, false, static_cast<const float*>(data), d, rmax, eps, flags, static_cast<float*>(cores),
-                           ranks_host, &info, as_stream(stream));
+    rc = ttsvd_impl<float, float>(ar, false, static_cast<const float*>(data), d, rmax, eps, flags, static_cast<float*>(cores),
+                                  ranks_host, &info, as_stream(stream));
+  else if (dtype == TNB_BF16)
+    rc = ttsvd_impl<float, __nv_bfloat16>(ar, false, static_cast<const __nv_bfloat16*>(data), d, rmax, eps, flags,
+                                          static_cast<float*>(cores), ranks_host, &info, as_stream(stream));
   else
-    rc = ttsvd_impl<double>(ar, false, static_cast<const double*>(data), d, rmax, eps, flags,
-                            static_cast<double*>(cores), ranks_host, &info, as_stream(stream));
+    rc = ttsvd_impl<double, double>(ar, false, static_cast<const double*>(data), d, rmax, eps, flags,
+                                    static_cast<double*>(cores), ranks_host, &info, as_stream(stream));
   if (info_host) {
     for (int i = 0; i < 32; ++i) info_host[i] = 0.0;
     info_host[0] = info.norm;
@@ -125,7 +138,7 @@ int tnb_ttsvd_batch(int dtype, const void* const* data, int batch, int ndim, con
                     double eps, uint32_t flags, void* workspace, size_t workspace_bytes, void* const* cores,
                     int64_t cores_capacity, int32_t* ranks_host, double* norms_host, int32_t* speculative_host,
                     void* stream) {
-  TNB_TRY(check_dtype(dtype));
+  TNB_TRY(check_ttsvd_dtype(dtype));
   TNB_TRY(require_device());
   if (batch < 0 || (batch > 0 && (!data || !cores)) || !shape || !ranks_host || !workspace)
     return fail(TNB_ERR_INVALID, "tnb_ttsvd_batch: null argument");
@@ -144,10 +157,14 @@ int tnb_ttsvd_batch(int dtype, const void* const* data, int batch, int ndim, con
   if (workspace_bytes < one) return fail(TNB_ERR_WORKSPACE, "tnb_ttsvd_batch: workspace %zu < %zu", workspace_bytes, one);
   const int inflight = (int)std::min<size_t>(workspace_bytes / one, (size_t)TNB_BATCH_MAX_INFLIGHT);
   if (dtype == TNB_F32)
-    return ttsvd_batch_impl<float>(workspace, one, inflight, reinterpret_cast<const float* const*>(data), batch, d, rmax, eps,
-                                   flags, reinterpret_cast<float* const*>(cores), ranks_host, norms_host, speculative_host,
-                                   as_stream(stream));
-  return ttsvd_batch_impl<double>(workspace, one, inflight, reinterpret_cast<const double* const*>(data), batch, d, rmax, eps,
+    return ttsvd_batch_impl<float, float>(workspace, one, inflight, reinterpret_cast<const float* const*>(data), batch, d, rmax,
+                                          eps, flags, reinterpret_cast<float* const*>(cores), ranks_host, norms_host,
+                                          speculative_host, as_stream(stream));
+  if (dtype == TNB_BF16)
+    return ttsvd_batch_impl<float, __nv_bfloat16>(workspace, one, inflight, reinterpret_cast<const __nv_bfloat16* const*>(data),
+                                                  batch, d, rmax, eps, flags, reinterpret_cast<float* const*>(cores), ranks_host,
+                                                  norms_host, speculative_host, as_stream(stream));
+  return ttsvd_batch_impl<double, double>(workspace, one, inflight, reinterpret_cast<const double* const*>(data), batch, d, rmax, eps,
                                   flags, reinterpret_cast<double* const*>(cores), ranks_host, norms_host, speculative_host,
                                   as_stream(stream));
 }
@@ -155,13 +172,13 @@ int tnb_ttsvd_batch(int dtype, const void* const* data, int batch, int ndim, con
 int tnb_ttsvd_host(int dtype, const void* data_host, int ndim, const int64_t* shape, const int32_t* rmax, double eps,
                    uint32_t flags, void* device_buffer, void* workspace, size_t workspace_bytes, void* cores_dev,
                    int64_t cores_capacity, void* cores_host, int32_t* ranks_host, double* info_host, void* stream) {
-  TNB_TRY(check_dtype(dtype));
+  TNB_TRY(check_ttsvd_dtype(dtype));
   TNB_TRY(require_device());
   if (!data_host || !device_buffer || !cores_host) return fail(TNB_ERR_INVALID, "tnb_ttsvd_host: null argument");
   SweepDims d;
   TNB_TRY(make_dims(ndim, shape, rmax, d));
-  const size_t esz = dtype == TNB_F32 ? 4 : 8;
-  const size_t total = (size_t)d.rows[ndim] * esz;
+  const size_t total = (size_t)d.rows[ndim] * dtype_bytes(dtype);
+  const size_t core_esz = dtype == TNB_F64 ? 8 : 4;  // bf16 input: fp32 cores
   cudaStream_t st = as_stream(stream);
   // chunked so that a pageable source still overlaps its staging copies with the DMA
   const size_t chunk = (size_t)256 << 20;
@@ -172,7 +189,7 @@ int tnb_ttsvd_host(int dtype, const void* data_host, int ndim, const int64_t* sh
   }
   TNB_TRY(tnb_ttsvd(dtype, device_buffer, ndim, shape, rmax, eps, flags, workspace, workspace_bytes, cores_dev,
                     cores_capacity, ranks_host, info_host, stream));
-  TNB_CUDA(cudaMemcpyAsync(cores_host, cores_dev, (size_t)d.capacity * esz, cudaMemcpyDeviceToHost, st));
+  TNB_CUDA(cudaMemcpyAsync(cores_host, cores_dev, (size_t)d.capacity * core_esz, cudaMemcpyDeviceToHost, st));
   TNB_CUDA(cudaStreamSynchronize(st));
   return TNB_OK;
 }
@@ -601,14 +618,30 @@ int tnb_gram_tc_f32(const float* A, int64_t rows, int64_t n, double* G, void* wo
                     void* stream) {
   TNB_TRY(require_device());
   if (!A || !G || !workspace) return fail(TNB_ERR_INVALID, "tnb_gram_tc_f32: null argument");
-  return gram_tc_f32(A, rows, n, G, nullptr, workspace, workspace_bytes, as_stream(stream));
+  return gram_tc(A, rows, n, G, nullptr, workspace, workspace_bytes, as_stream(stream));
 }
 
 int tnb_gram_tc_kblocked_f32(const float* A, int64_t rows, int64_t n, double* G, void* workspace, size_t workspace_bytes,
                              void* stream) {
   TNB_TRY(require_device());
   if (!A || !G || !workspace) return fail(TNB_ERR_INVALID, "tnb_gram_tc_kblocked_f32: null argument");
-  return gram_tc_f32(A, rows, n, G, nullptr, workspace, workspace_bytes, as_stream(stream), true);
+  return gram_tc(A, rows, n, G, nullptr, workspace, workspace_bytes, as_stream(stream), true);
+}
+
+size_t tnb_gram_tc_bf16_workspace_bytes(int64_t rows, int64_t n) {
+  if (!gram_tc_bf16_shape_ok(rows, n)) return 0;
+  return gram_tc_input_workspace_bytes<__nv_bfloat16>(rows, n) + 256;
+}
+
+double tnb_gram_noise_level(int dtype) {
+  return dtype == TNB_F32 ? TF32_GRAM_NOISE : dtype == TNB_BF16 ? BF16_GRAM_NOISE : 0.0;
+}
+
+int tnb_gram_tc_bf16(const void* A, int64_t rows, int64_t n, double* G, void* workspace, size_t workspace_bytes,
+                     void* stream) {
+  TNB_TRY(require_device());
+  if (!A || !G || !workspace) return fail(TNB_ERR_INVALID, "tnb_gram_tc_bf16: null argument");
+  return gram_tc(static_cast<const __nv_bfloat16*>(A), rows, n, G, nullptr, workspace, workspace_bytes, as_stream(stream));
 }
 
 size_t tnb_atb_tc_workspace_bytes(int64_t K, int64_t m, int64_t n) {
@@ -662,21 +695,29 @@ int tnb_project_tc_f32(const float* A, int64_t rows, int64_t n, const float* V, 
                        size_t workspace_bytes, void* stream) {
   TNB_TRY(require_device());
   if (!A || !V || !C || !workspace) return fail(TNB_ERR_INVALID, "tnb_project_tc_f32: null argument");
-  return project_tc_f32(A, rows, n, V, r, C, workspace, workspace_bytes, as_stream(stream));
+  return project_tc(A, rows, n, V, r, C, workspace, workspace_bytes, as_stream(stream));
 }
 
 int tnb_project_tc_kblocked_out_f32(const float* A, int64_t rows, int64_t n, const float* V, int32_t r, int64_t inner,
                                     float* C, void* workspace, size_t workspace_bytes, void* stream) {
   TNB_TRY(require_device());
   if (!A || !V || !C || !workspace) return fail(TNB_ERR_INVALID, "tnb_project_tc_kblocked_out_f32: null argument");
-  return project_tc_f32(A, rows, n, V, r, C, workspace, workspace_bytes, as_stream(stream), PT_OUT_KBLOCKED, inner);
+  return project_tc(A, rows, n, V, r, C, workspace, workspace_bytes, as_stream(stream), PT_OUT_KBLOCKED, inner);
 }
 
 int tnb_project_tc_kblocked_in_f32(const float* A, int64_t rows, int64_t n, const float* V, int32_t r, float* C,
                                    void* workspace, size_t workspace_bytes, void* stream) {
   TNB_TRY(require_device());
   if (!A || !V || !C || !workspace) return fail(TNB_ERR_INVALID, "tnb_project_tc_kblocked_in_f32: null argument");
-  return project_tc_f32(A, rows, n, V, r, C, workspace, workspace_bytes, as_stream(stream), PT_IN_KBLOCKED);
+  return project_tc(A, rows, n, V, r, C, workspace, workspace_bytes, as_stream(stream), PT_IN_KBLOCKED);
+}
+
+int tnb_project_tc_bf16(const void* A, int64_t rows, int64_t n, const float* V, int32_t r, int64_t inner, float* C,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  TNB_TRY(require_device());
+  if (!A || !V || !C || !workspace) return fail(TNB_ERR_INVALID, "tnb_project_tc_bf16: null argument");
+  return project_tc(static_cast<const __nv_bfloat16*>(A), rows, n, V, r, C, workspace, workspace_bytes, as_stream(stream),
+                    inner > 0 ? PT_OUT_KBLOCKED : PT_ROWMAJOR, inner);
 }
 
 size_t tnb_eigh_workspace_bytes(int32_t n) {
@@ -734,29 +775,33 @@ int tnb_eig_topk(const double* G, int32_t n, int32_t k, int32_t b, double tol, d
 }
 
 size_t tnb_tt_relative_error_workspace_bytes(int dtype, int ndim, const int64_t* shape, const int32_t* ranks) {
-  if (check_dtype(dtype) != TNB_OK || ndim < 2) return 0;
+  if (check_ttsvd_dtype(dtype) != TNB_OK || ndim < 2) return 0;
   ArenaSizer ar;
   int rc;
-  if (dtype == TNB_F32)
-    rc = tt_relative_error_impl<float>(ar, true, nullptr, nullptr, ndim, shape, ranks, nullptr, 0);
-  else
-    rc = tt_relative_error_impl<double>(ar, true, nullptr, nullptr, ndim, shape, ranks, nullptr, 0);
+  if (dtype == TNB_F64)
+    rc = tt_relative_error_impl<double, double>(ar, true, nullptr, nullptr, ndim, shape, ranks, nullptr, 0);
+  else  // fp32 cores for fp32 and bf16 data
+    rc = tt_relative_error_impl<float, float>(ar, true, nullptr, nullptr, ndim, shape, ranks, nullptr, 0);
   return rc == TNB_OK ? ar.off + 4096 : 0;
 }
 
 int tnb_tt_relative_error(int dtype, const void* data, const void* const* cores, int ndim, const int64_t* shape,
                           const int32_t* ranks, void* workspace, size_t workspace_bytes, double* result_host,
                           void* stream) {
-  TNB_TRY(check_dtype(dtype));
+  TNB_TRY(check_ttsvd_dtype(dtype));
   TNB_TRY(require_device());
   if (!data || !cores || !shape || !ranks || !workspace || !result_host)
     return fail(TNB_ERR_INVALID, "tnb_tt_relative_error: null argument");
   Arena ar(workspace, workspace_bytes);
   if (dtype == TNB_F32)
-    return tt_relative_error_impl<float>(ar, false, static_cast<const float*>(data),
-                                         reinterpret_cast<const float* const*>(cores), ndim, shape, ranks, result_host,
-                                         as_stream(stream));
-  return tt_relative_error_impl<double>(ar, false, static_cast<const double*>(data),
+    return tt_relative_error_impl<float, float>(ar, false, static_cast<const float*>(data),
+                                                reinterpret_cast<const float* const*>(cores), ndim, shape, ranks, result_host,
+                                                as_stream(stream));
+  if (dtype == TNB_BF16)
+    return tt_relative_error_impl<float, __nv_bfloat16>(ar, false, static_cast<const __nv_bfloat16*>(data),
+                                                        reinterpret_cast<const float* const*>(cores), ndim, shape, ranks,
+                                                        result_host, as_stream(stream));
+  return tt_relative_error_impl<double, double>(ar, false, static_cast<const double*>(data),
                                         reinterpret_cast<const double* const*>(cores), ndim, shape, ranks, result_host,
                                         as_stream(stream));
 }

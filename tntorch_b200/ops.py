@@ -22,6 +22,20 @@ def _dtype_code(t: torch.Tensor) -> int:
     return _DT[t.dtype]
 
 
+# The dense TT-SVD (ttsvd, ttsvd_batch, their plans, tt_relative_error) also reads bfloat16 data; its cores are float32.
+_DT_DENSE = {**_DT, torch.bfloat16: _lib.TNB_BF16}
+
+
+def _dense_code(dtype: torch.dtype) -> int:
+    if dtype not in _DT_DENSE:
+        raise ValueError(f"the dense TT-SVD supports float32/float64/bfloat16 tensors, got {dtype}")
+    return _DT_DENSE[dtype]
+
+
+def _core_dtype(dtype: torch.dtype) -> torch.dtype:
+    return torch.float32 if dtype == torch.bfloat16 else dtype
+
+
 def _require_cuda(t: torch.Tensor, what: str):
     if not t.is_cuda:
         raise RuntimeError(f"{what}: tensor must live on a CUDA device (tntorch_b200 has no CPU path)")
@@ -88,7 +102,7 @@ def ttsvd(data: torch.Tensor, rmax=None, eps: float = 1e-14, batch_mode: bool = 
     """Dense tensor -> list of TT cores [r_{k-1}, I_k, r_k] (tn.Tensor(data, ranks_tt=...), tensor.py:401-408)."""
     _require_cuda(data, "ttsvd")
     data = data.contiguous()
-    code = _dtype_code(data)
+    code = _dense_code(data.dtype)
     N = data.dim()
     shape = list(data.shape)
     rm = _rmax_list(rmax, max(N - 1, 0))
@@ -105,7 +119,7 @@ def ttsvd(data: torch.Tensor, rmax=None, eps: float = 1e-14, batch_mode: bool = 
     if wsb == 0:
         check(_lib.ERR_UNSUPPORTED if L.tnb_last_error() else _lib.ERR_INVALID)
     ws = _ws(wsb, data.device)
-    cores_buf = torch.empty(int(cap), dtype=data.dtype, device=data.device)
+    cores_buf = torch.empty(int(cap), dtype=_core_dtype(data.dtype), device=data.device)
     ranks = (C.c_int32 * (N + 1))()
     info = (C.c_double * 32)()
     with torch.cuda.device(data.device):
@@ -131,7 +145,7 @@ class TTSVDPlan:
         self.N = len(self.shape)
         self.dtype = dtype
         self.device = torch.device(device)
-        self.code = _DT[dtype]
+        self.code = _dense_code(dtype)
         self.rm = _rmax_list(rmax, max(self.N - 1, 0))
         # concurrent: several plans run at once on different streams (TNB_FLAG_CONCURRENT, include/tnb200.h)
         self.flags = ((0 if use_tensorcore else _lib.FLAG_NO_TENSORCORE) | (_lib.FLAG_PROFILE if profile else 0) |
@@ -145,7 +159,7 @@ class TTSVDPlan:
         if self.cap < 0 or wsb == 0:
             check(_lib.ERR_UNSUPPORTED)
         self.ws = _ws(wsb, self.device)
-        self.cores_buf = torch.empty(int(self.cap), dtype=dtype, device=self.device)
+        self.cores_buf = torch.empty(int(self.cap), dtype=_core_dtype(dtype), device=self.device)
         self.ranks = (C.c_int32 * (self.N + 1))()
         self.info = (C.c_double * 32)()
         self.numel = 1
@@ -155,7 +169,7 @@ class TTSVDPlan:
         self.cores_host = None
         if host_io:
             self.dev_in = torch.empty(self.numel, dtype=dtype, device=self.device)
-            self.cores_host = torch.empty(int(self.cap), dtype=dtype, pin_memory=True)
+            self.cores_host = torch.empty(int(self.cap), dtype=_core_dtype(dtype), pin_memory=True)
 
     def run(self, data: torch.Tensor, eps: float = 1e-14):
         with torch.cuda.device(self.device):
@@ -193,7 +207,7 @@ class TTSVDBatchPlan:
         self.batch = int(batch)
         self.dtype = dtype
         self.device = torch.device(device)
-        self.code = _DT[dtype]
+        self.code = _dense_code(dtype)
         self.rm = _rmax_list(rmax, max(self.N - 1, 0))
         self.flags = (0 if use_tensorcore else _lib.FLAG_NO_TENSORCORE) | (_lib.FLAG_BATCH_MODE if batch_mode else 0)
         L = lib()
@@ -208,7 +222,7 @@ class TTSVDBatchPlan:
         self.per_tensor_bytes = int(one.value)
         self.inflight = max(1, min(int(inflight), self.batch, 8))
         self.ws = _ws(self.per_tensor_bytes * self.inflight, self.device)
-        self.cores_buf = torch.empty(self.batch, int(self.cap), dtype=dtype, device=self.device)
+        self.cores_buf = torch.empty(self.batch, int(self.cap), dtype=_core_dtype(dtype), device=self.device)
         self.ranks = (C.c_int32 * (self.batch * (self.N + 1)))()
         self.norms = (C.c_double * self.batch)()
         self.spec = (C.c_int32 * self.batch)()
@@ -220,7 +234,7 @@ class TTSVDBatchPlan:
         self.cores_host = None
         if host_io:
             self.dev_in = torch.empty(self.batch, self.numel, dtype=dtype, device=self.device)
-            self.cores_host = torch.empty(self.batch, int(self.cap), dtype=dtype, pin_memory=True)
+            self.cores_host = torch.empty(self.batch, int(self.cap), dtype=_core_dtype(dtype), pin_memory=True)
 
     def run(self, tensors, eps: float = 1e-14):
         """tensors: a [batch, ...] tensor or a sequence of `batch` contiguous device tensors.  Returns, per tensor, the
@@ -715,6 +729,49 @@ def gram_kblocked(B: torch.Tensor, rows: int, n: int) -> torch.Tensor:
     return G
 
 
+def gram_bf16(A: torch.Tensor) -> torch.Tensor:
+    """fp64 A^T A of a row-major bfloat16 (rows x n) matrix on the bf16 tensor-core Gram kernel (exact products, fp32
+    accumulation): n % 8 == 0 and n = 32 / 64 (rows divisible by 128 / n), 128 or >= 256."""
+    _require_cuda(A, "gram_bf16")
+    assert A.dtype == torch.bfloat16
+    A = A.contiguous()
+    rows, n = A.shape
+    G = torch.empty(n, n, dtype=torch.float64, device=A.device)
+    L = lib()
+    wsb = L.tnb_gram_tc_bf16_workspace_bytes(rows, n)
+    if wsb == 0:
+        check(_lib.ERR_UNSUPPORTED)
+    ws = _ws(wsb, A.device)
+    with torch.cuda.device(A.device):
+        check(L.tnb_gram_tc_bf16(_ptr(A), rows, n, _ptr(G), _ptr(ws), ws.numel(), _stream()))
+    return G
+
+
+def gram_noise_level(dtype: torch.dtype) -> float:
+    """||G_tc - (1 - c) G|| / ||G|| the TT-SVD's accept rule allows for the tensor-core Gram of float32 (TF32) or
+    bfloat16 input."""
+    return float(lib().tnb_gram_noise_level(_dense_code(dtype)))
+
+
+def project_bf16(A: torch.Tensor, V: torch.Tensor, inner: int = 0) -> torch.Tensor:
+    """A (rows x n, bfloat16) @ V (n x r, float32) at fp32 accuracy on the tensor cores, float32 result.  inner > 0
+    writes it K-blocked like project_kblocked_out (returned flat)."""
+    _require_cuda(A, "project_bf16")
+    assert A.dtype == torch.bfloat16 and V.dtype == torch.float32
+    A, V = A.contiguous(), V.contiguous()
+    rows, n = A.shape
+    r = V.shape[1]
+    out = torch.empty(rows * r if inner > 0 else (rows, r), dtype=torch.float32, device=A.device)
+    L = lib()
+    wsb = L.tnb_project_tc_workspace_bytes(n, r)
+    if wsb == 0:
+        check(_lib.ERR_UNSUPPORTED)
+    ws = _ws(wsb, A.device)
+    with torch.cuda.device(A.device):
+        check(L.tnb_project_tc_bf16(_ptr(A), rows, n, _ptr(V), r, int(inner), _ptr(out), _ptr(ws), ws.numel(), _stream()))
+    return out
+
+
 def atb_tensorcore(A: torch.Tensor, B: torch.Tensor, alpha: float = 1.0, D: Optional[torch.Tensor] = None,
                    beta: float = 0.0) -> torch.Tensor:
     """alpha * A^T B + beta * D on the tensor-core kernel (A: K x m, B: K x n, fp32)."""
@@ -846,12 +903,15 @@ def eig_topk(G: torch.Tensor, k: int, b: int = 0, tol: float = 1e-6):
 
 
 def tt_relative_error(data: torch.Tensor, cores: Sequence[torch.Tensor]) -> float:
-    """‖data − TT(cores)‖_F / ‖data‖_F, fp64 accumulation on the device (metrics.py:135-151)."""
+    """‖data − TT(cores)‖_F / ‖data‖_F, fp64 accumulation on the device (metrics.py:135-151).  bfloat16 data takes
+    float32 cores (what ttsvd returns for it)."""
     _require_cuda(data, "tt_relative_error")
     data = data.contiguous()
     cores = [c.contiguous() for c in cores]
     N = data.dim()
-    code = _dtype_code(data)
+    code = _dense_code(data.dtype)
+    if data.dtype == torch.bfloat16 and any(c.dtype != torch.float32 for c in cores):
+        raise ValueError("tt_relative_error: bfloat16 data needs float32 cores")
     ranks = [cores[0].shape[0]] + [c.shape[2] for c in cores]
     L = lib()
     sh, rk = i64(list(data.shape)), i32(ranks)
