@@ -60,18 +60,41 @@ inline int make_round_dims(int ndim, const int64_t* shape, const int32_t* ranks_
   return TNB_OK;
 }
 
+// Phase A, core k: G = A^T A with A = cur viewed (rowsA x cols), then, when `pivot` is given, the Cholesky-QR of A in
+// fp64 from G (chol_orth_kernel): A fac has orthonormal columns and A = (A fac) Rf; a breakdown pivot (rank-deficient
+// or short core) raises *pivot.  fits: the factorisation keeps L and L^-1 in shared memory.
+template <typename T>
+inline int round_gram_chol(const GemmPlan& pl, const T* cur, int64_t rowsA, int64_t cols, double* partial, double* G,
+                           double* js, T* fac, T* Rf, int* pivot, bool fits, cudaStream_t st) {
+  TNB_TRY((gemm_splitk<T, T, double, double, float>(pl, cols, cols, rowsA, cur, cols, false, cur, cols, false, partial, G,
+                                                    cols, 1.0, nullptr, 0, 0.0, nullptr, 0, 0.0, true, (float*)nullptr, 0,
+                                                    st)));
+  if (!pivot) return TNB_OK;
+  const size_t csm = (size_t)2 * cols * (cols | 1) * sizeof(double);
+  static PerDeviceFlag attr_done;
+  TNB_CUDA(ensure_dyn_smem(attr_done, chol_orth_kernel<T>, 180 * 1024));
+  chol_orth_kernel<T><<<1, 1024, fits ? csm : 0, st>>>(G, (int)cols, js, fac, pivot, fits ? 1 : 0, Rf);
+  TNB_LAUNCH_CHECK();
+  return TNB_OK;
+}
+
+// Phase A, core k, from the Cholesky-QR factors (q = cols): Q_k = A fac (rowsA x q);  next = Rf * unfold(core_{k+1}).
+template <typename T>
+inline int round_apply_qr(const T* cur, int64_t rowsA, int64_t cols, const T* fac, const T* Rf, const T* core_next,
+                          int64_t ncols, T* Qk, T* nxt, cudaStream_t st) {
+  TNB_TRY((gemm_direct<T, T, T, T>(rowsA, cols, cols, cur, cols, true, fac, cols, false, Qk, cols, (T)1, nullptr, 0, (T)0,
+                                   nullptr, 0, (T)0, st)));
+  return gemm_direct<T, T, T, T>(cols, ncols, cols, Rf, cols, true, core_next, ncols, false, nxt, ncols, (T)1, nullptr, 0,
+                                 (T)0, nullptr, 0, (T)0, st);
+}
+
 // Phase A + phase B of Tensor.round_tt (tensor.py:2008-2083) on device-resident cores.
 template <typename T, class ArenaT>
 inline int tt_round_impl(ArenaT& ar, bool dry, const T* const* cores_in, const RoundDims& d, const int32_t* rmax,
                          double eps, uint32_t flags, T* cores_out, int32_t* ranks_host, cudaStream_t st) {
   const int N = d.N;
-  StepCtx cx;
-  cx.flags = flags;
-  cx.allow_tc = false;  // TT cores are small: the generic fp64-accumulating kernels are used throughout
-  cx.st = st;
-  const double epsN = eps / std::max(1.0, std::sqrt((double)(N - 1)));
-  cx.eps_scaled2 = epsN * epsN;
-  cx.sc = ar.template take<SweepScalars>(1);
+  // TT cores are small: the generic fp64-accumulating kernels are used throughout
+  StepCtx cx = make_step_ctx(ar, N, eps, flags, false, nullptr, st, false);
   if (!dry) {
     cx.h_sc = static_cast<int*>(pinned_scratch(sizeof(SweepScalars)));
     if (!cx.h_sc) return fail(TNB_ERR_CUDA, "pinned scratch allocation failed");
@@ -117,33 +140,22 @@ inline int tt_round_impl(ArenaT& ar, bool dry, const T* const* cores_in, const R
     T* Rf = ar.template take<T>((size_t)cols * cols);    // sqrt(lambda) V_q^T   (q x cols)
     if (!dry) {
       if (!ar.ok) return fail(TNB_ERR_WORKSPACE, "tt_round: workspace too small (need > %zu bytes)", ar.off);
-      // G = A^T A with A = cur viewed (rowsA x cols)
-      TNB_TRY((gemm_splitk<T, T, double, double, float>(pl, cols, cols, rowsA, cur, cols, false, cur, cols, false, partial,
-                                                        G, cols, 1.0, nullptr, 0, 0.0, nullptr, 0, 0.0, true,
-                                                        (float*)nullptr, 0, st)));
-      // fast path: Cholesky-QR in fp64 (A = Q R with R = L^T from G = L L^T); a breakdown pivot (rank-deficient
-      // or short core) raises the flag and the eigen-decomposition path below takes over for this core
+      // fast path: Cholesky-QR, on a core with at least as many rows as columns; a raised pivot flag sends this core
+      // to the eigen-decomposition path below
+      const bool try_chol = rowsA >= cols;
+      if (try_chol) TNB_CUDA(cudaMemsetAsync(jinfo, 0, 4 * sizeof(int), st));
+      const bool fits = (size_t)2 * cols * (cols | 1) * sizeof(double) <= (size_t)180 * 1024;
+      TNB_TRY(round_gram_chol<T>(pl, cur, rowsA, cols, partial, G, js, fac, Rf, try_chol ? jinfo + 1 : nullptr, fits, st));
       bool chol_ok = false;
-      if (rowsA >= cols) {
-        TNB_CUDA(cudaMemsetAsync(jinfo, 0, 4 * sizeof(int), st));
-        const size_t csm = (size_t)2 * cols * (cols | 1) * sizeof(double);
-        const bool fits = csm <= (size_t)180 * 1024;
-        static PerDeviceFlag attr_done;
-  TNB_CUDA(ensure_dyn_smem(attr_done, chol_orth_kernel<T>, 180 * 1024));
-        chol_orth_kernel<T><<<1, 1024, fits ? csm : 0, st>>>(G, (int)cols, js, fac, jinfo + 1, fits ? 1 : 0, Rf);
-        TNB_LAUNCH_CHECK();
+      if (try_chol) {
         TNB_CUDA(cudaMemcpyAsync(cx.h_sc, jinfo, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
         TNB_CUDA(cudaStreamSynchronize(st));
         chol_ok = (cx.h_sc[1] == 0);
       }
+      const int64_t ncols = d.shape[k + 1] * d.rin[k + 2];
       if (chol_ok) {
-        const int64_t q = cols;
-        r[k + 1] = q;
-        TNB_TRY((gemm_direct<T, T, T, T>(rowsA, q, cols, cur, cols, true, fac, q, false, Q[k], q, (T)1, nullptr, 0, (T)0,
-                                         nullptr, 0, (T)0, st)));
-        const int64_t ncols = d.shape[k + 1] * d.rin[k + 2];
-        TNB_TRY((gemm_direct<T, T, T, T>(q, ncols, cols, Rf, cols, true, cores_in[k + 1], ncols, false, nxt, ncols, (T)1,
-                                         nullptr, 0, (T)0, nullptr, 0, (T)0, st)));
+        r[k + 1] = cols;
+        TNB_TRY(round_apply_qr<T>(cur, rowsA, cols, fac, Rf, cores_in[k + 1], ncols, Q[k], nxt, st));
         T* t = cur; cur = nxt; nxt = t;
         if (ar.off > peak) peak = ar.off;
         ar.off = mark;
@@ -166,7 +178,6 @@ inline int tt_round_impl(ArenaT& ar, bool dry, const T* const* cores_in, const R
       // R' = lambda^1/2 V_q^T (q x cols);  next <- R' * unfold(core_{k+1})  (q x I r'')
       scale_extract_kernel<T><<<grid_for(cols * q), 256, 0, st>>>(V, (int)cols, (int)cols, (int)q, w, Rf, 2, 1);
       TNB_LAUNCH_CHECK();
-      const int64_t ncols = d.shape[k + 1] * d.rin[k + 2];
       TNB_TRY((gemm_direct<T, T, T, T>(q, ncols, cols, Rf, cols, true, cores_in[k + 1], ncols, false, nxt, ncols, (T)1,
                                        nullptr, 0, (T)0, nullptr, 0, (T)0, st)));
       T* t = cur; cur = nxt; nxt = t;
@@ -222,8 +233,7 @@ __global__ void or_flag_kernel(const int* src, int* flags, int bit) {
 
 template <typename T>
 inline bool tt_round_spec_eligible(const RoundDims& d, const int32_t* rmax, double eps, uint32_t flags) {
-  static const bool disabled = getenv("TNB_NO_SPECULATE") != nullptr;
-  if (disabled || (flags & TNB_FLAG_NO_SPECULATE) || d.N < 2 || !rmax) return false;
+  if ((flags & TNB_FLAG_NO_SPECULATE) || d.N < 2 || !rmax) return false;
   const double epsN = eps / std::max(1.0, std::sqrt((double)(d.N - 1)));
   if (!(epsN * epsN < 1e-20)) return false;
   for (int k = 0; k < d.N - 1; ++k) {
@@ -240,15 +250,7 @@ template <typename T, class ArenaT>
 inline int tt_round_spec_enqueue(ArenaT& ar, bool dry, const T* const* cores_in, const RoundDims& d, const int32_t* rmax,
                                  double eps, uint32_t flags, T* cores_out, SpecHostBack* hb, cudaStream_t st) {
   const int N = d.N;
-  StepCtx cx;
-  cx.flags = flags;
-  cx.allow_tc = false;
-  cx.st = st;
-  const double epsN = eps / std::max(1.0, std::sqrt((double)(N - 1)));
-  cx.eps_scaled2 = epsN * epsN;
-  cx.sc = ar.template take<SweepScalars>(1);
-  cx.d_flags = ar.template take<int>(4);
-  cx.d_ranks = ar.template take<int32_t>(N + 1);
+  StepCtx cx = make_step_ctx(ar, N, eps, flags, false, nullptr, st, true);
   int* d_chol = ar.template take<int>(4);
   size_t maxcore = 0;
   for (int k = 0; k < N; ++k) maxcore = std::max<size_t>(maxcore, (size_t)d.ra[k] * d.shape[k] * d.rin[k + 1]);
@@ -276,19 +278,8 @@ inline int tt_round_spec_enqueue(ArenaT& ar, bool dry, const T* const* cores_in,
     if (ar.off > peak) peak = ar.off;
     if (!dry) {
       if (!ar.ok) return fail(TNB_ERR_WORKSPACE, "tt_round: workspace too small (need > %zu bytes)", ar.off);
-      TNB_TRY((gemm_splitk<T, T, double, double, float>(pl, cols, cols, rowsA, cur, cols, false, cur, cols, false, partial, G,
-                                                        cols, 1.0, nullptr, 0, 0.0, nullptr, 0, 0.0, true, (float*)nullptr, 0,
-                                                        st)));
-      const size_t csm = (size_t)2 * cols * (cols | 1) * sizeof(double);
-      static PerDeviceFlag attr_done;
-      TNB_CUDA(ensure_dyn_smem(attr_done, chol_orth_kernel<T>, 180 * 1024));
-      chol_orth_kernel<T><<<1, 1024, csm, st>>>(G, (int)cols, js, fac, d_chol, 1, Rf);
-      TNB_LAUNCH_CHECK();
-      TNB_TRY((gemm_direct<T, T, T, T>(rowsA, cols, cols, cur, cols, true, fac, cols, false, Q[k], cols, (T)1, nullptr, 0,
-                                       (T)0, nullptr, 0, (T)0, st)));
-      const int64_t ncols = d.shape[k + 1] * d.rin[k + 2];
-      TNB_TRY((gemm_direct<T, T, T, T>(cols, ncols, cols, Rf, cols, true, cores_in[k + 1], ncols, false, nxt, ncols, (T)1,
-                                       nullptr, 0, (T)0, nullptr, 0, (T)0, st)));
+      TNB_TRY(round_gram_chol<T>(pl, cur, rowsA, cols, partial, G, js, fac, Rf, d_chol, true, st));  // eligible: cols <= 104
+      TNB_TRY(round_apply_qr<T>(cur, rowsA, cols, fac, Rf, cores_in[k + 1], d.shape[k + 1] * d.rin[k + 2], Q[k], nxt, st));
       T* t = cur; cur = nxt; nxt = t;
     }
     ar.off = mark;
@@ -398,18 +389,14 @@ inline int tt_round_batch_impl(void* workspace, size_t per_tensor_bytes, int inf
   TNB_TRY(pool.ensure());
   SpecHostBack* hbs = static_cast<SpecHostBack*>(pinned_scratch((size_t)batch * sizeof(SpecHostBack)));
   if (!hbs) return fail(TNB_ERR_CUDA, "pinned scratch allocation failed");
-  TNB_CUDA(cudaEventRecord(pool.ev[TNB_BATCH_MAX_INFLIGHT], st));
-  for (int s = 0; s < inflight; ++s) TNB_CUDA(cudaStreamWaitEvent(pool.st[s], pool.ev[TNB_BATCH_MAX_INFLIGHT], 0));
+  TNB_TRY(pool.fork(st, inflight));
   int rc = TNB_OK;
   for (int i = 0; i < batch && rc == TNB_OK; ++i) {
     const int s = i % inflight;  // tensor i + inflight reuses workspace slice s on the same stream: ordered
     Arena ar(ws + (size_t)s * per_tensor_bytes, per_tensor_bytes);
     rc = tt_round_spec_enqueue<T>(ar, false, cores_in + (size_t)i * N, d, rmax, eps, flags, cores_out[i], hbs + i, pool.st[s]);
   }
-  for (int s = 0; s < inflight; ++s) {
-    cudaEventRecord(pool.ev[s], pool.st[s]);
-    cudaStreamWaitEvent(st, pool.ev[s], 0);
-  }
+  pool.join(st, inflight);
   TNB_CUDA(cudaStreamSynchronize(st));
   if (rc != TNB_OK && rc != TNB_ERR_UNSUPPORTED) return rc;
   std::vector<int> bad(batch, 0);

@@ -313,6 +313,24 @@ struct Prof {
   void mark(cudaStream_t st) {
     if (on) cudaEventRecord(next(), st);
   }
+  // after the stream has been synchronised; 4 events per step: start, after Gram, after eigen+rank, after
+  // factor/projection
+  void collect(SweepInfo* info) {
+    if (on && info) {
+      const int steps = used / 4;
+      info->nsteps = steps;
+      for (int t = 0; t < steps && t < 8; ++t) {
+        float a = 0, b = 0, c = 0;
+        cudaEventElapsedTime(&a, ev[4 * t], ev[4 * t + 1]);
+        cudaEventElapsedTime(&b, ev[4 * t + 1], ev[4 * t + 2]);
+        cudaEventElapsedTime(&c, ev[4 * t + 2], ev[4 * t + 3]);
+        info->gram_ms[t] = a;
+        info->eig_ms[t] = b;
+        info->factor_ms[t] = c;
+      }
+    }
+    on = false;
+  }
   static Prof& get() {
     static thread_local Prof p;
     return p;
@@ -332,6 +350,56 @@ struct StepCtx {
   int* d_flags = nullptr;       // device flags raised by spec_check_kernel / cd_finish_kernel
   int32_t* d_ranks = nullptr;   // device copy of the ranks the rule chose, [N + 1]
 };
+
+// The context of a sweep over N modes.  Carves the device scalars and, for a speculative sweep, then its flags and ranks.
+template <class ArenaT>
+inline StepCtx make_step_ctx(ArenaT& ar, int N, double eps, uint32_t flags, bool allow_tc, SweepInfo* info,
+                             cudaStream_t st, bool speculative) {
+  StepCtx cx;
+  cx.flags = flags;
+  cx.allow_tc = allow_tc;
+  cx.info = info;
+  cx.st = st;
+  const double epsN = eps / std::max(1.0, std::sqrt((double)(N - 1)));
+  cx.eps_scaled2 = epsN * epsN;
+  cx.sc = ar.template take<SweepScalars>(1);
+  if (speculative) {
+    cx.d_flags = ar.template take<int>(4);
+    cx.d_ranks = ar.template take<int32_t>(N + 1);
+  }
+  return cx;
+}
+
+// The end of a truncation step at rank `rank`, from the step's eigenpairs (w descending, V with leading dimension ldv):
+//   tall (rows >= n): core = V_r^T (rank x n);  Cn = C V_r;
+//   wide:             core = diag(1/s) U_r^T C (rank x n);  Cn = U_r diag(s).
+// fac (L x rank) is scratch; ptc_ws the tensor-core projection's workspace (project_tc_carve_bytes).  `layout` is
+// PT_ROWMAJOR unless the speculative sweep reads (PT_IN_KBLOCKED) or writes (PT_OUT_KBLOCKED, out_inner) a K-blocked carry.
+template <typename T, typename TIn>
+inline int step_factors(const StepCtx& cx, const TIn* C, int64_t rows, int64_t n, int64_t rank, const double* w,
+                        const double* V, int ldv, T* fac, void* ptc_ws, size_t ptc_bytes, T* core, T* Cn,
+                        int layout = PT_ROWMAJOR, int64_t out_inner = 0) {
+  cudaStream_t st = cx.st;
+  if (rows >= n) {
+    scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(V, ldv, (int)n, (int)rank, w, core, 0, 1);
+    TNB_LAUNCH_CHECK();
+    scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(V, ldv, (int)n, (int)rank, w, fac, 0, 0);
+    TNB_LAUNCH_CHECK();
+    BigKernelGate gate(st, (cx.flags & TNB_FLAG_CONCURRENT) && rows >= PROJ_TC_MIN_ROWS);
+    if constexpr (tc_input<TIn>())
+      if (layout != PT_ROWMAJOR)
+        return project_tc<TIn>(C, rows, n, reinterpret_cast<const float*>(fac), (int)rank, reinterpret_cast<float*>(Cn),
+                               ptc_ws, ptc_bytes, st, layout, out_inner);
+    return project_any<T, TIn>(C, rows, n, fac, rank, Cn, st, ptc_ws, ptc_bytes);
+  }
+  scale_extract_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(V, ldv, (int)rows, (int)rank, w, fac, 1, 0);
+  TNB_LAUNCH_CHECK();
+  TNB_TRY((gemm_direct<T, TIn, T, T>(rank, n, rows, fac, rank, false, C, n, false, core, n, (T)1, nullptr, 0, (T)0,
+                                     nullptr, 0, (T)0, st)));
+  scale_extract_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(V, ldv, (int)rows, (int)rank, w, Cn, 2, 0);
+  TNB_LAUNCH_CHECK();
+  return TNB_OK;
+}
 
 // TIn: the element type of C (the dense input at step 0, else T).
 template <typename T, typename TIn, class ArenaT>
@@ -400,24 +468,8 @@ inline int truncate_step(ArenaT& ar, bool dry, const StepCtx& cx, const TIn* C, 
     TNB_LAUNCH_CHECK();
     fill_kernel<T><<<grid_for(rows), 256, 0, st>>>(Cn, rows, (T)0);
     TNB_LAUNCH_CHECK();
-  } else if (tall) {
-    // core = V_r^T (rank x n);  Cn = C V_r
-    scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(ew.V, ew.ldv, (int)n, (int)rank, ew.w, core, 0, 1);
-    TNB_LAUNCH_CHECK();
-    scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(ew.V, ew.ldv, (int)n, (int)rank, ew.w, fac, 0, 0);
-    TNB_LAUNCH_CHECK();
-    {
-      BigKernelGate gate(st, concurrent && rows >= PROJ_TC_MIN_ROWS);
-      TNB_TRY((project_any<T, TIn>(C, rows, n, fac, rank, Cn, st, ptc_ws, ptc_bytes)));
-    }
   } else {
-    // core = diag(1/s) U_r^T C (rank x n);  Cn = U_r diag(s)
-    scale_extract_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(ew.V, ew.ldv, (int)rows, (int)rank, ew.w, fac, 1, 0);
-    TNB_LAUNCH_CHECK();
-    TNB_TRY((gemm_direct<T, TIn, T, T>(rank, n, rows, fac, rank, false, C, n, false, core, n, (T)1, nullptr, 0, (T)0,
-                                       nullptr, 0, (T)0, st)));
-    scale_extract_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(ew.V, ew.ldv, (int)rows, (int)rank, ew.w, Cn, 2, 0);
-    TNB_LAUNCH_CHECK();
+    TNB_TRY((step_factors<T, TIn>(cx, C, rows, n, rank, ew.w, ew.V, ew.ldv, fac, ptc_ws, ptc_bytes, core, Cn)));
   }
   prof.mark(st);
   *rank_out = rank;
@@ -442,9 +494,10 @@ inline bool spec_step_ok(int64_t rows, int64_t n, int64_t rank_cap, bool allow_t
   return chfsi_dev_ok((int)L, chfsi_dev_block((int)L, (int)k));
 }
 
-// The step is split in two enqueue phases so that a batch of tensors can be interleaved phase by phase (all Gram
-// kernels of a step first, then every tensor's eigen chain + projection): the whole-GPU kernels of the batch then run
-// back to back while the latency-bound eigen chains of the other tensors run beside them on their own streams.
+// The step is split in enqueue phases so that a batch of tensors can be interleaved phase by phase (spec_enqueue: all
+// Gram kernels of a step first, then every tensor's eigen stages, then every tensor's projection): the whole-GPU kernels
+// of the batch then run back to back while the latency-bound eigen chains of the other tensors run beside them on their
+// own streams.
 template <typename T>
 struct SpecStep {
   GramWork gw;
@@ -550,12 +603,10 @@ inline int spec_step_eig_stage(SpecStep<T>& s, int stage) {
 template <typename T, typename TIn>
 inline int spec_step_rest(const StepCtx& cx, const TIn* C, int64_t rows, int64_t n, int32_t rm, T* core, T* Cn, int mu,
                           SpecStep<T>& s, bool prof_on) {
-  const bool tall = rows >= n;
   const int64_t L = s.L;
   const int batch_mode = (cx.flags & TNB_FLAG_BATCH_MODE) ? 1 : 0;
   cudaStream_t st = cx.st;
   Prof& prof = Prof::get();
-  const bool concurrent = (cx.flags & TNB_FLAG_CONCURRENT) != 0;
   if (!s.chfsi) {
     rank_rule_kernel<<<1, 32, 0, st>>>(s.w, (int)L, (int)L, rm, 0, batch_mode, cx.sc, gram_noise(s.used_tc, s.fp32_solve),
                                        (int)L);
@@ -567,31 +618,9 @@ inline int spec_step_rest(const StepCtx& cx, const TIn* C, int64_t rows, int64_t
   spec_check_kernel<<<1, 32, 0, st>>>(cx.sc, (int)s.kcap, cx.d_ranks + mu, cx.d_flags);
   TNB_LAUNCH_CHECK();
   if (prof_on) prof.mark(st);
-  const int64_t rank = s.kcap;
-  if (tall) {
-    scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(s.V, s.ldv, (int)n, (int)rank, s.w, core, 0, 1);
-    TNB_LAUNCH_CHECK();
-    scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(s.V, s.ldv, (int)n, (int)rank, s.w, s.fac, 0, 0);
-    TNB_LAUNCH_CHECK();
-    {
-      BigKernelGate gate(st, concurrent && rows >= PROJ_TC_MIN_ROWS);
-      bool blocked = false;
-      if constexpr (tc_input<TIn>()) {
-        blocked = s.in_kblocked || s.out_inner > 0;
-        if (blocked)
-          TNB_TRY(project_tc<TIn>(C, rows, n, reinterpret_cast<const float*>(s.fac), (int)rank, reinterpret_cast<float*>(Cn),
-                                  s.ptc_ws, s.ptc_bytes, st, s.in_kblocked ? PT_IN_KBLOCKED : PT_OUT_KBLOCKED, s.out_inner));
-      }
-      if (!blocked) TNB_TRY((project_any<T, TIn>(C, rows, n, s.fac, rank, Cn, st, s.ptc_ws, s.ptc_bytes)));
-    }
-  } else {
-    scale_extract_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(s.V, s.ldv, (int)rows, (int)rank, s.w, s.fac, 1, 0);
-    TNB_LAUNCH_CHECK();
-    TNB_TRY((gemm_direct<T, TIn, T, T>(rank, n, rows, s.fac, rank, false, C, n, false, core, n, (T)1, nullptr, 0, (T)0,
-                                       nullptr, 0, (T)0, st)));
-    scale_extract_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(s.V, s.ldv, (int)rows, (int)rank, s.w, Cn, 2, 0);
-    TNB_LAUNCH_CHECK();
-  }
+  const int layout = s.in_kblocked ? PT_IN_KBLOCKED : s.out_inner > 0 ? PT_OUT_KBLOCKED : PT_ROWMAJOR;
+  TNB_TRY((step_factors<T, TIn>(cx, C, rows, n, s.kcap, s.w, s.V, s.ldv, s.fac, s.ptc_ws, s.ptc_bytes, core, Cn, layout,
+                                s.out_inner)));
   if (prof_on) prof.mark(st);
   return TNB_OK;
 }
@@ -599,21 +628,27 @@ inline int spec_step_rest(const StepCtx& cx, const TIn* C, int64_t rows, int64_t
 // ---------------------------------------------------------------------------------------------
 // Dense TT-SVD
 // ---------------------------------------------------------------------------------------------
+// The two ping-pong carries, sized by the rank caps: step t writes carry[t & 1] (rows[mu] x rcap[mu]).
+template <typename T, class ArenaT>
+inline void carve_carries(ArenaT& ar, const SweepDims& d, T* carry[2]) {
+  size_t elems[2] = {0, 0};
+  for (int mu = d.N - 1, t = 0; mu >= 1; --mu, ++t) {
+    const size_t e = (size_t)d.rows[mu] * (size_t)d.rcap[mu];
+    if (e > elems[t & 1]) elems[t & 1] = e;
+  }
+  carry[0] = ar.template take<T>(elems[0]);
+  carry[1] = ar.template take<T>(elems[1]);
+}
+
 // T: carries and cores; TIn: the dense input (T, or bf16 with T = float), read by step 0 only.
 template <typename T, typename TIn, class ArenaT>
 inline int ttsvd_sync_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d, const int32_t* rmax, double eps,
                            uint32_t flags, T* cores, int32_t* ranks_host, SweepInfo* info, cudaStream_t st,
                            bool exact_gram = false) {
   const int N = d.N;
-  StepCtx cx;
-  cx.flags = flags;
+  StepCtx cx = make_step_ctx(ar, N, eps, flags, !(flags & TNB_FLAG_NO_TENSORCORE) && (dry || tc_path_available()), info,
+                             st, false);
   cx.exact_gram = exact_gram;
-  cx.allow_tc = !(flags & TNB_FLAG_NO_TENSORCORE) && (dry || tc_path_available());
-  cx.info = info;
-  cx.st = st;
-  const double epsN = eps / std::max(1.0, std::sqrt((double)(N - 1)));
-  cx.eps_scaled2 = epsN * epsN;
-  cx.sc = ar.template take<SweepScalars>(1);
   Prof& prof = Prof::get();
   prof.on = !dry && (flags & TNB_FLAG_PROFILE);
   prof.used = 0;
@@ -636,13 +671,8 @@ inline int ttsvd_sync_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDim
     }
     return TNB_OK;
   }
-  // carry buffers (ping-pong), sized by the rank caps
-  size_t carry_elems[2] = {0, 0};
-  for (int mu = N - 1, t = 0; mu >= 1; --mu, ++t) {
-    const size_t e = (size_t)d.rows[mu] * (size_t)d.rcap[mu];
-    if (e > carry_elems[t & 1]) carry_elems[t & 1] = e;
-  }
-  T* carry[2] = {ar.template take<T>(carry_elems[0]), ar.template take<T>(carry_elems[1])};
+  T* carry[2];
+  carve_carries(ar, d, carry);
   const T* C = nullptr;  // the carry step t > 0 reads; step 0 reads data
   int64_t r_next = 1;
   size_t peak = ar.off;
@@ -671,20 +701,7 @@ inline int ttsvd_sync_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDim
     TNB_CUDA(cudaMemcpyAsync(cores + d.slot[0], C, sizeof(T) * (size_t)d.shape[0] * (size_t)r_next,
                              cudaMemcpyDeviceToDevice, st));
     TNB_CUDA(cudaStreamSynchronize(st));
-    if (prof.on && info) {  // 4 events per step: start, after Gram, after eigen+rank, after factor/projection
-      const int steps = prof.used / 4;
-      info->nsteps = steps;
-      for (int t = 0; t < steps && t < 8; ++t) {
-        float a = 0, b = 0, c = 0;
-        cudaEventElapsedTime(&a, prof.ev[4 * t], prof.ev[4 * t + 1]);
-        cudaEventElapsedTime(&b, prof.ev[4 * t + 1], prof.ev[4 * t + 2]);
-        cudaEventElapsedTime(&c, prof.ev[4 * t + 2], prof.ev[4 * t + 3]);
-        info->gram_ms[t] = a;
-        info->eig_ms[t] = b;
-        info->factor_ms[t] = c;
-      }
-    }
-    prof.on = false;
+    prof.collect(info);
   }
   return TNB_OK;
 }
@@ -694,8 +711,7 @@ inline int ttsvd_sync_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDim
 // ---------------------------------------------------------------------------------------------
 template <typename T>
 inline bool spec_eligible(const SweepDims& d, const int32_t* rmax, double eps, uint32_t flags, bool allow_tc) {
-  static const bool disabled = getenv("TNB_NO_SPECULATE") != nullptr;  // A/B switch (profiling, debugging)
-  if (disabled || (flags & TNB_FLAG_NO_SPECULATE) || d.N < 2 || !rmax) return false;
+  if ((flags & TNB_FLAG_NO_SPECULATE) || d.N < 2 || !rmax) return false;
   const double epsN = eps / std::max(1.0, std::sqrt((double)(d.N - 1)));
   if (!(epsN * epsN < 1e-20)) return false;  // an active eps budget decides ranks: host-driven path
   for (int mu = d.N - 1; mu >= 1; --mu) {
@@ -704,11 +720,6 @@ inline bool spec_eligible(const SweepDims& d, const int32_t* rmax, double eps, u
   }
   return true;
 }
-
-struct SpecOutcome {
-  int flags = 0;
-  bool ran = false;
-};
 
 struct SpecHostBack {  // pinned read-back of one speculative sweep
   SweepScalars sc;
@@ -734,25 +745,10 @@ struct SpecRun {
 template <typename T, typename TIn, class ArenaT>
 inline int spec_begin(SpecRun<T, TIn, ArenaT>& r, ArenaT& ar, bool dry, const TIn* data, const SweepDims& d, double eps,
                       uint32_t flags, T* cores, SweepInfo* info, cudaStream_t st, SpecHostBack* hb) {
-  const int N = d.N;
   r.ar = &ar;
-  r.cx = StepCtx();
-  r.cx.flags = flags;
-  r.cx.allow_tc = !(flags & TNB_FLAG_NO_TENSORCORE) && (dry || tc_path_available());
-  r.cx.info = info;
-  r.cx.st = st;
-  const double epsN = eps / std::max(1.0, std::sqrt((double)(N - 1)));
-  r.cx.eps_scaled2 = epsN * epsN;
-  r.cx.sc = ar.template take<SweepScalars>(1);
-  r.cx.d_flags = ar.template take<int>(4);
-  r.cx.d_ranks = ar.template take<int32_t>(N + 1);
-  size_t carry_elems[2] = {0, 0};
-  for (int mu = N - 1, t = 0; mu >= 1; --mu, ++t) {
-    const size_t e = (size_t)d.rows[mu] * (size_t)d.rcap[mu];
-    if (e > carry_elems[t & 1]) carry_elems[t & 1] = e;
-  }
-  r.carry[0] = ar.template take<T>(carry_elems[0]);
-  r.carry[1] = ar.template take<T>(carry_elems[1]);
+  r.cx = make_step_ctx(ar, d.N, eps, flags, !(flags & TNB_FLAG_NO_TENSORCORE) && (dry || tc_path_available()), info, st,
+                       true);
+  carve_carries(ar, d, r.carry);
   r.data = data;
   r.C = nullptr;
   r.cores = cores;
@@ -782,14 +778,6 @@ inline int spec_phase1(SpecRun<T, TIn, ArenaT>& r, bool dry, const SweepDims& d,
   return spec_step_gram<T, T>(r.cx, r.C, rows, n, false, r.step, prof_on);
 }
 template <typename T, typename TIn, class ArenaT>
-inline int spec_phase2a(SpecRun<T, TIn, ArenaT>& r, bool dry) {
-  return dry ? TNB_OK : spec_step_eig_begin<T>(r.cx, r.step);
-}
-template <typename T, typename TIn, class ArenaT>
-inline int spec_phase2s(SpecRun<T, TIn, ArenaT>& r, bool dry, int stage) {
-  return dry ? TNB_OK : spec_step_eig_stage<T>(r.step, stage);
-}
-template <typename T, typename TIn, class ArenaT>
 inline int spec_phase2b(SpecRun<T, TIn, ArenaT>& r, bool dry, const SweepDims& d, const int32_t* rmax, int mu, int t,
                         bool prof_on) {
   ArenaT& ar = *r.ar;
@@ -806,13 +794,24 @@ inline int spec_phase2b(SpecRun<T, TIn, ArenaT>& r, bool dry, const SweepDims& d
   ar.off = r.mark;
   return TNB_OK;
 }
-// the whole phase 2 of one tensor
+// Enqueues the whole sweep of g >= 1 runs, each on its own stream, step by step: every run's Gram (phase 1), then every
+// run's eigen start (phase 2a), then the subspace-solver stages interleaved run by run, then every run's rank rule and
+// projection (phase 2b).  Interleaving the stages makes the resident filter kernels of the streams run one after the
+// other (cheb_filter.cuh), so one run's Rayleigh-Ritz step is in flight while another run's filter runs.  With dry it
+// only sizes the step scratch.
 template <typename T, typename TIn, class ArenaT>
-inline int spec_phase2(SpecRun<T, TIn, ArenaT>& r, bool dry, const SweepDims& d, const int32_t* rmax, int mu, int t,
-                       bool prof_on) {
-  TNB_TRY(spec_phase2a(r, dry));
-  for (int stage = 0; stage <= CD_MAX_STAGES; ++stage) TNB_TRY(spec_phase2s(r, dry, stage));
-  return spec_phase2b(r, dry, d, rmax, mu, t, prof_on);
+inline int spec_enqueue(SpecRun<T, TIn, ArenaT>* runs, int g, bool dry, const SweepDims& d, const int32_t* rmax,
+                        bool prof_on) {
+  for (int mu = d.N - 1, t = 0; mu >= 1; --mu, ++t) {
+    for (int s = 0; s < g; ++s) TNB_TRY(spec_phase1(runs[s], dry, d, mu, t, prof_on));
+    if (!dry) {
+      for (int s = 0; s < g; ++s) TNB_TRY(spec_step_eig_begin<T>(runs[s].cx, runs[s].step));
+      for (int stage = 0; stage <= CD_MAX_STAGES; ++stage)
+        for (int s = 0; s < g; ++s) TNB_TRY(spec_step_eig_stage<T>(runs[s].step, stage));
+    }
+    for (int s = 0; s < g; ++s) TNB_TRY(spec_phase2b(runs[s], dry, d, rmax, mu, t, prof_on));
+  }
+  return TNB_OK;
 }
 template <typename T, typename TIn, class ArenaT>
 inline int spec_end(SpecRun<T, TIn, ArenaT>& r, const SweepDims& d) {
@@ -825,11 +824,9 @@ inline int spec_end(SpecRun<T, TIn, ArenaT>& r, const SweepDims& d) {
   TNB_CUDA(cudaMemcpyAsync(r.hb->ranks, r.cx.d_ranks, (size_t)(N + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   return TNB_OK;
 }
-// after the stream has been synchronised
-inline void spec_collect(const SpecHostBack* hb, const SweepDims& d, int32_t* ranks_host, SweepInfo* info, SpecOutcome* out) {
+// after the stream has been synchronised; returns the speculation flags (spec_check_kernel bits, 0: accepted)
+inline int spec_collect(const SpecHostBack* hb, const SweepDims& d, int32_t* ranks_host, SweepInfo* info) {
   const int N = d.N;
-  out->ran = true;
-  out->flags = hb->flags[0];
   ranks_host[0] = 1;
   ranks_host[N] = 1;
   for (int mu = 1; mu < N; ++mu) ranks_host[mu] = (int32_t)d.rcap[mu];  // the flags say whether the rule agreed
@@ -840,13 +837,14 @@ inline void spec_collect(const SpecHostBack* hb, const SweepDims& d, int32_t* ra
     info->rr_sweeps += hb->flags[3];
     info->fused_filters += hb->flags[2] - info->eig_solves;  // every Rayleigh-Ritz step but the first of a solve follows a filter
   }
+  return hb->flags[0];
 }
 
+// *spec_flags: what spec_collect returned (set when the sweep ran to its end)
 template <typename T, typename TIn, class ArenaT>
 inline int ttsvd_spec_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d, const int32_t* rmax, double eps,
                            uint32_t flags, T* cores, int32_t* ranks_host, SweepInfo* info, cudaStream_t st,
-                           SpecOutcome* out) {
-  const int N = d.N;
+                           int* spec_flags) {
   Prof& prof = Prof::get();
   prof.on = !dry && (flags & TNB_FLAG_PROFILE);
   prof.used = 0;
@@ -858,14 +856,11 @@ inline int ttsvd_spec_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDim
   }
   SpecRun<T, TIn, ArenaT> r;
   TNB_TRY(spec_begin(r, ar, dry, data, d, eps, flags, cores, info, st, hb));
-  for (int mu = N - 1, t = 0; mu >= 1; --mu, ++t) {
-    int rc = spec_phase1(r, dry, d, mu, t, prof_on);
-    if (rc == TNB_OK) rc = spec_phase2(r, dry, d, rmax, mu, t, prof_on);
-    if (rc != TNB_OK) {
-      if (!dry) cudaStreamSynchronize(st);  // part of the sweep is enqueued: drain it before the host-driven path
-      prof.on = false;
-      return rc;
-    }
+  const int rc = spec_enqueue(&r, 1, dry, d, rmax, prof_on);
+  if (rc != TNB_OK) {
+    if (!dry) cudaStreamSynchronize(st);  // part of the sweep is enqueued: drain it before the host-driven path
+    prof.on = false;
+    return rc;
   }
   if (dry) {
     ar.off = r.peak;
@@ -873,21 +868,8 @@ inline int ttsvd_spec_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDim
   }
   TNB_TRY(spec_end(r, d));
   TNB_CUDA(cudaStreamSynchronize(st));
-  spec_collect(hb, d, ranks_host, info, out);
-  if (prof_on && info) {
-    const int steps = prof.used / 4;
-    info->nsteps = steps;
-    for (int t = 0; t < steps && t < 8; ++t) {
-      float a = 0, b = 0, c = 0;
-      cudaEventElapsedTime(&a, prof.ev[4 * t], prof.ev[4 * t + 1]);
-      cudaEventElapsedTime(&b, prof.ev[4 * t + 1], prof.ev[4 * t + 2]);
-      cudaEventElapsedTime(&c, prof.ev[4 * t + 2], prof.ev[4 * t + 3]);
-      info->gram_ms[t] = a;
-      info->eig_ms[t] = b;
-      info->factor_ms[t] = c;
-    }
-  }
-  prof.on = false;
+  *spec_flags = spec_collect(hb, d, ranks_host, info);
+  prof.collect(info);
   return TNB_OK;
 }
 
@@ -905,27 +887,26 @@ inline int ttsvd_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d,
       bool all_caps = true;
       for (int mu = 1; mu < d.N; ++mu) all_caps = all_caps && rmax[mu - 1] > 0;
       if (all_caps) {
-        SpecOutcome o;
-        const int rc = ttsvd_spec_impl<T, TIn>(ar, true, data, d, rmax, eps, flags, cores, ranks_host, info, st, &o);
+        const int rc = ttsvd_spec_impl<T, TIn>(ar, true, data, d, rmax, eps, flags, cores, ranks_host, info, st, nullptr);
         if (rc == TNB_OK) need_spec = ar.off - base;
         ar.off = base;
       }
     } else {
-      SpecOutcome o;
+      int sflags = 0;
       SweepInfo saved;
       if (info) saved = *info;
-      const int rc = ttsvd_spec_impl<T, TIn>(ar, false, data, d, rmax, eps, flags, cores, ranks_host, info, st, &o);
-      if (rc == TNB_OK && o.ran && o.flags == 0) {
+      const int rc = ttsvd_spec_impl<T, TIn>(ar, false, data, d, rmax, eps, flags, cores, ranks_host, info, st, &sflags);
+      if (rc == TNB_OK && sflags == 0) {
         if (info) info->speculative = 1;
         return TNB_OK;
       }
       if (rc != TNB_OK && rc != TNB_ERR_UNSUPPORTED && rc != TNB_ERR_NOCONV) return rc;
       // the device disagreed with the speculation (or could not run the sync-free solver): host-driven sweep;
       // bit 0 = the TF32 Gram is too coarse for this spectrum, so the repeat takes exact-product Gram matrices
-      if (info) { *info = saved; info->spec_flags = o.flags; }
+      if (info) { *info = saved; info->spec_flags = sflags; }
       ar.off = base;
       ar.ok = true;
-      return ttsvd_sync_impl<T, TIn>(ar, false, data, d, rmax, eps, flags, cores, ranks_host, info, st, (o.flags & 1) != 0);
+      return ttsvd_sync_impl<T, TIn>(ar, false, data, d, rmax, eps, flags, cores, ranks_host, info, st, (sflags & 1) != 0);
     }
   }
   const int rc = ttsvd_sync_impl<T, TIn>(ar, dry, data, d, rmax, eps, flags, cores, ranks_host, info, st);
@@ -936,8 +917,8 @@ inline int ttsvd_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d,
 // ---------------------------------------------------------------------------------------------
 // A batch of independent dense tensors of one shape (the reference's `batch=True` constructor, tensor.py:401-408 with
 // a leading batch dimension; north_star: "batched decompositions").  Up to `inflight` speculative sweeps are enqueued
-// from ONE host thread, interleaved phase by phase on internal streams, and synchronised once; tensors whose
-// speculation the device rejected are then repeated one by one on the host-driven path.
+// from ONE host thread, interleaved stage by stage on internal streams (spec_enqueue), and synchronised once; tensors
+// whose speculation the device rejected are then repeated one by one on the host-driven path.
 // ---------------------------------------------------------------------------------------------
 constexpr int TNB_BATCH_MAX_INFLIGHT = 8;
 
@@ -952,6 +933,19 @@ struct StreamPool {
     for (int i = 0; i <= TNB_BATCH_MAX_INFLIGHT; ++i) TNB_CUDA(cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming));
     ready = true;
     return TNB_OK;
+  }
+  // the first n internal streams start after whatever the caller enqueued on `caller`
+  int fork(cudaStream_t caller, int n) {
+    TNB_CUDA(cudaEventRecord(ev[TNB_BATCH_MAX_INFLIGHT], caller));
+    for (int i = 0; i < n; ++i) TNB_CUDA(cudaStreamWaitEvent(st[i], ev[TNB_BATCH_MAX_INFLIGHT], 0));
+    return TNB_OK;
+  }
+  // `caller` continues after the first n internal streams; unchecked, as it also runs after a failed enqueue
+  void join(cudaStream_t caller, int n) {
+    for (int i = 0; i < n; ++i) {
+      cudaEventRecord(ev[i], st[i]);
+      cudaStreamWaitEvent(caller, ev[i], 0);
+    }
   }
   static StreamPool& get() {
     static StreamPool pools[TNB_MAX_DEVICES];
@@ -985,9 +979,7 @@ inline int ttsvd_batch_impl(void* workspace, size_t per_tensor_bytes, int inflig
   TNB_TRY(pool.ensure());
   SpecHostBack* hbs = static_cast<SpecHostBack*>(pinned_scratch((size_t)batch * sizeof(SpecHostBack)));
   if (!hbs) return fail(TNB_ERR_CUDA, "pinned scratch allocation failed");
-  // fork: the internal streams start after whatever the caller enqueued on `st`
-  TNB_CUDA(cudaEventRecord(pool.ev[TNB_BATCH_MAX_INFLIGHT], st));
-  for (int s = 0; s < inflight; ++s) TNB_CUDA(cudaStreamWaitEvent(pool.st[s], pool.ev[TNB_BATCH_MAX_INFLIGHT], 0));
+  TNB_TRY(pool.fork(st, inflight));
   const uint32_t bflags = (flags | TNB_FLAG_CONCURRENT) & ~TNB_FLAG_PROFILE;
   std::vector<SweepInfo> infos(batch);
   int rc = TNB_OK;
@@ -1000,57 +992,19 @@ inline int ttsvd_batch_impl(void* workspace, size_t per_tensor_bytes, int inflig
     for (int s = 0; s < g && rc == TNB_OK; ++s)
       rc = spec_begin(runs[s], arenas[s], false, data[g0 + s], d, eps, bflags, cores[g0 + s], &infos[g0 + s], pool.st[s],
                       hbs + g0 + s);
-    // Enqueue order (TNB_BATCH_ORDER):
-    //   "stage" (default): step by step; all Gram kernels of a step, then the eigen stages of all tensors INTERLEAVED
-    //            stage by stage (the resident filter kernels of all streams run one after the other, cheb_filter.cuh:
-    //            this way tensor A's Rayleigh-Ritz step is in flight while tensor B's filter runs), then every
-    //            tensor's rank rule + projection;
-    //   "phase": step by step, each tensor's whole eigen chain enqueued at once (chains then queue behind each other);
-    //   "wave":  a diagonal wavefront — in wave w tensor s is at step w - s.
-    static const char* order_env = getenv("TNB_BATCH_ORDER");
-    const bool order_phase = order_env && !strcmp(order_env, "phase");
-    const bool order_wave = order_env && !strcmp(order_env, "wave");
-    const int steps = N - 1;
-    if (order_wave) {
-      for (int w = 0; w < steps + g - 1 && rc == TNB_OK; ++w) {
-        for (int s = 0; s < g && rc == TNB_OK; ++s) {
-          const int t = w - s;
-          if (t >= 0 && t < steps) rc = spec_phase1(runs[s], false, d, N - 1 - t, t, false);
-        }
-        for (int s = 0; s < g && rc == TNB_OK; ++s) {
-          const int t = w - s;
-          if (t >= 0 && t < steps) rc = spec_phase2(runs[s], false, d, rmax, N - 1 - t, t, false);
-        }
-      }
-    } else {
-      for (int mu = N - 1, t = 0; mu >= 1 && rc == TNB_OK; --mu, ++t) {
-        for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase1(runs[s], false, d, mu, t, false);
-        if (order_phase) {
-          for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase2(runs[s], false, d, rmax, mu, t, false);
-        } else {
-          for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase2a(runs[s], false);
-          for (int stage = 0; stage <= CD_MAX_STAGES && rc == TNB_OK; ++stage)
-            for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase2s(runs[s], false, stage);
-          for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_phase2b(runs[s], false, d, rmax, mu, t, false);
-        }
-      }
-    }
+    if (rc == TNB_OK) rc = spec_enqueue(runs.data(), g, false, d, rmax, false);
     for (int s = 0; s < g && rc == TNB_OK; ++s) rc = spec_end(runs[s], d);
   }
-  // join: the caller's stream continues after every internal stream; then the one host synchronisation
-  for (int s = 0; s < inflight; ++s) {
-    cudaEventRecord(pool.ev[s], pool.st[s]);
-    cudaStreamWaitEvent(st, pool.ev[s], 0);
-  }
+  pool.join(st, inflight);  // then the one host synchronisation
   TNB_CUDA(cudaStreamSynchronize(st));
   if (rc != TNB_OK && rc != TNB_ERR_UNSUPPORTED && rc != TNB_ERR_NOCONV) return rc;
   // read every outcome out of the pinned block first: the host-driven repeats below reuse that scratch
-  std::vector<SpecOutcome> outs(batch);
+  std::vector<int> sflags(batch, 0);
   for (int i = 0; i < batch; ++i)
-    if (rc == TNB_OK) spec_collect(hbs + i, d, ranks_host + (size_t)i * (N + 1), &infos[i], &outs[i]);
+    if (rc == TNB_OK) sflags[i] = spec_collect(hbs + i, d, ranks_host + (size_t)i * (N + 1), &infos[i]);
   for (int i = 0; i < batch; ++i) {
     int32_t* rk = ranks_host + (size_t)i * (N + 1);
-    if (rc == TNB_OK && outs[i].flags == 0) {
+    if (rc == TNB_OK && sflags[i] == 0) {
       if (norms_host) norms_host[i] = infos[i].norm;
       if (spec_host) spec_host[i] = 1;
       continue;
@@ -1059,7 +1013,7 @@ inline int ttsvd_batch_impl(void* workspace, size_t per_tensor_bytes, int inflig
     Arena ar(ws, per_tensor_bytes);
     SweepInfo info;
     TNB_TRY((ttsvd_sync_impl<T, TIn, Arena>(ar, false, data[i], d, rmax, eps, flags & ~TNB_FLAG_PROFILE, cores[i], rk, &info, st,
-                                       (outs[i].flags & 1) != 0)));
+                                       (sflags[i] & 1) != 0)));
     if (norms_host) norms_host[i] = info.norm;
     if (spec_host) spec_host[i] = 0;
   }
