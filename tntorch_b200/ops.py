@@ -294,8 +294,10 @@ def ttsvd_batch(tensors, rmax=None, eps: float = 1e-14, batch_mode: bool = False
 
 
 # --------------------------------------------------------------------------------------
-def tt_round(cores: Sequence[torch.Tensor], eps: float = 1e-14, rmax=None, batch_mode: bool = False):
-    """Tensor.round_tt on device cores (tensor.py:2008-2083). Returns new cores."""
+def tt_round(cores: Sequence[torch.Tensor], eps: float = 1e-14, rmax=None, batch_mode: bool = False,
+             speculate: bool = True):
+    """Tensor.round_tt on device cores (tensor.py:2008-2083). Returns new cores.  speculate=False runs the host-driven
+    sweeps even where the speculative one-synchronisation path is eligible (TNB_FLAG_NO_SPECULATE)."""
     N = len(cores)
     for c in cores:
         _require_cuda(c, "tt_round")
@@ -325,7 +327,7 @@ def tt_round(cores: Sequence[torch.Tensor], eps: float = 1e-14, rmax=None, batch
     out = torch.empty(int(cap), dtype=dt, device=dev)
     ranks = (C.c_int32 * (N + 1))()
     ptrs = (C.c_void_p * N)(*[c.data_ptr() for c in cores])
-    flags = _lib.FLAG_BATCH_MODE if batch_mode else 0
+    flags = (_lib.FLAG_BATCH_MODE if batch_mode else 0) | (0 if speculate else _lib.FLAG_NO_SPECULATE)
     with torch.cuda.device(dev):
         check(L.tnb_tt_round(code, ptrs, N, sh, rinc, rmc, float(eps), flags, _ptr(ws), ws.numel(), _ptr(out), cap, ranks,
                              _stream()))
@@ -337,9 +339,15 @@ def tt_round(cores: Sequence[torch.Tensor], eps: float = 1e-14, rmax=None, batch
 
 
 def tt_round_batch(batch_cores: Sequence[Sequence[torch.Tensor]], eps: float = 1e-14, rmax=None, batch_mode: bool = False,
-                   inflight: int = 8, return_info: bool = False):
+                   inflight: int = 8, return_info: bool = False, speculate: bool = True):
     """Round a batch of TT tensors that share shape and input ranks: ONE library call, several tensors in flight
-    (tnb_tt_round_batch).  batch_cores: per tensor, its list of cores [r, I, r'].  Returns per tensor the new cores."""
+    (tnb_tt_round_batch).  batch_cores: per tensor, its list of cores [r, I, r'].  Returns per tensor the new cores.
+
+    return_info adds dict(speculative=[...]): 1 where a tensor's result came from the speculative sweeps (one
+    synchronisation), 0 where it came from the host-driven sweeps.  With one tensor the call goes through the same
+    dispatcher as tt_round, so this reports which path tt_round takes on that input; with B > 1 and inflight >= 2 it
+    goes through the in-flight driver, which redoes each tensor whose speculation failed on the host-driven path.
+    speculate=False runs the host-driven sweeps for every tensor (TNB_FLAG_NO_SPECULATE)."""
     B = len(batch_cores)
     if B == 0:
         return []
@@ -369,7 +377,7 @@ def tt_round_batch(batch_cores: Sequence[Sequence[torch.Tensor]], eps: float = 1
     spec = (C.c_int32 * B)()
     pin = (C.c_void_p * (B * N))(*[c.data_ptr() for cores in cs for c in cores])
     pout = (C.c_void_p * B)(*[out[i].data_ptr() for i in range(B)])
-    flags = _lib.FLAG_BATCH_MODE if batch_mode else 0
+    flags = (_lib.FLAG_BATCH_MODE if batch_mode else 0) | (0 if speculate else _lib.FLAG_NO_SPECULATE)
     with torch.cuda.device(dev):
         check(L.tnb_tt_round_batch(code, pin, B, N, sh, rinc, rmc, float(eps), flags, _ptr(ws), ws.numel(), pout, cap, ranks, spec,
                                    _stream()))
@@ -420,9 +428,9 @@ def tt_sum(operands, alpha=None):
     return [out[offs[n]: offs[n] + rsum[n] * shape[n] * rsum[n + 1]].view(rsum[n], shape[n], rsum[n + 1]) for n in range(N)]
 
 
-def tt_sum_round(operands, alpha=None, eps: float = 1e-14, rmax=None):
+def tt_sum_round(operands, alpha=None, eps: float = 1e-14, rmax=None, speculate: bool = True):
     """round_tt(sum_k alpha_k T_k) in ONE library call: block cores assembled in the workspace, then the rounding sweeps
-    (the `tn.round(function(a, b))` step of tools.reduce, tools.py:460-512)."""
+    (the `tn.round(function(a, b))` step of tools.reduce, tools.py:460-512).  speculate as for tt_round."""
     ops_c, K, N, shape, ranks, ptrs, dt, dev = _tt_operands(operands)
     L = lib()
     rm = _rmax_list(rmax, max(N - 1, 0))
@@ -439,8 +447,9 @@ def tt_sum_round(operands, alpha=None, eps: float = 1e-14, rmax=None):
     out = torch.empty(int(cap), dtype=dt, device=dev)
     rk = (C.c_int32 * (N + 1))()
     al = None if alpha is None else (C.c_double * K)(*[float(a) for a in alpha])
+    flags = 0 if speculate else _lib.FLAG_NO_SPECULATE
     with torch.cuda.device(dev):
-        check(L.tnb_tt_sum_round(code, ptrs, K, al, N, i64(shape), i32(ranks), rmc, float(eps), 0, _ptr(ws), ws.numel(), _ptr(out),
+        check(L.tnb_tt_sum_round(code, ptrs, K, al, N, i64(shape), i32(ranks), rmc, float(eps), flags, _ptr(ws), ws.numel(), _ptr(out),
                                  cap, rk, _stream()))
     return [out[offs[n]: offs[n] + rk[n] * shape[n] * rk[n + 1]].view(rk[n], shape[n], rk[n + 1]) for n in range(N)]
 
