@@ -36,10 +36,11 @@ extern "C" {
 
 #define TNB_F32 0
 #define TNB_F64 1
-/* bf16 dense input, accepted by tnb_ttsvd, tnb_ttsvd_batch, tnb_ttsvd_host, their *_workspace_bytes queries and
- * tnb_tt_relative_error (bf16 data, fp32 cores).  The cores, their capacity and info_host are fp32 for bf16 input; every
- * other entry point rejects it with TNB_ERR_INVALID. */
+/* bf16 and fp16 dense input, accepted by tnb_ttsvd, tnb_ttsvd_batch, tnb_ttsvd_host, their *_workspace_bytes queries
+ * and tnb_tt_relative_error (16-bit data, fp32 cores).  The cores, their capacity and info_host are fp32 for 16-bit
+ * input; every other entry point rejects both codes with TNB_ERR_INVALID. */
 #define TNB_BF16 2
+#define TNB_F16 3
 
 /* flags for tnb_ttsvd / tnb_tt_round */
 #define TNB_FLAG_NO_TENSORCORE 1u /* force the generic fp32/fp64 CUDA-core kernels (debug / parity A-B) */
@@ -316,11 +317,16 @@ int tnb_gram_tc_kblocked_f32(const float* A, int64_t rows, int64_t n, double* G,
 /* The same Gram of a row-major bf16 A (rows x n, n % 8 == 0; n = 32 / 64 with rows divisible by 128 / n, n = 128 or
  * n >= 256): bf16 wgmma, exact products, fp32 accumulation; workspace: tnb_gram_tc_bf16_workspace_bytes. */
 size_t tnb_gram_tc_bf16_workspace_bytes(int64_t rows, int64_t n);
-/* The noise level ||E|| / ||G|| the TT-SVD's accept rule allows for a tensor-core Gram of TNB_F32 (TF32) or TNB_BF16
- * input, E = G_tc - (1 - c) G after the uniform shrink c; 0 for other codes. */
+/* The noise level ||E|| / ||G|| the TT-SVD's accept rule allows for a tensor-core Gram of TNB_F32 (TF32), TNB_BF16 or
+ * TNB_F16 input, E = G_tc - (1 - c) G after the uniform shrink c; 0 for other codes. */
 double tnb_gram_noise_level(int dtype);
 int tnb_gram_tc_bf16(const void* A, int64_t rows, int64_t n, double* G, void* workspace, size_t workspace_bytes,
                      void* stream);
+/* The same Gram of a row-major fp16 A (same shapes as tnb_gram_tc_bf16): the same kernel with fp16 wgmma, exact
+ * products, fp32 accumulation; workspace: tnb_gram_tc_f16_workspace_bytes. */
+size_t tnb_gram_tc_f16_workspace_bytes(int64_t rows, int64_t n);
+int tnb_gram_tc_f16(const void* A, int64_t rows, int64_t n, double* G, void* workspace, size_t workspace_bytes,
+                    void* stream);
 /* C (m x n) = alpha * A^T B + beta * D on the same tensor-core kernel (A: K x m, B: K x n, row-major fp32, TF32
  * operands, fp32 accumulation; m, n multiples of 4, >= 32).  The Chebyshev-filter products G*Y of
  * tnb_eig_topk's subspace iteration run through this entry (G symmetric => A = G).  D may be NULL. */
@@ -359,6 +365,10 @@ int tnb_project_tc_kblocked_in_f32(const float* A, int64_t rows, int64_t n, cons
  * tnb_project_tc_workspace_bytes. */
 int tnb_project_tc_bf16(const void* A, int64_t rows, int64_t n, const float* V, int32_t r, int64_t inner, float* C,
                         void* workspace, size_t workspace_bytes, void* stream);
+/* The same with A fp16: V is split into two fp16 terms of V scaled per column by a power of two (chosen on the device),
+ * and the scale is divided out of C exactly.  Same shapes, layouts and workspace query as tnb_project_tc_bf16. */
+int tnb_project_tc_f16(const void* A, int64_t rows, int64_t n, const float* V, int32_t r, int64_t inner, float* C,
+                       void* workspace, size_t workspace_bytes, void* stream);
 /* Symmetric eigendecomposition of a PSD matrix G (n x n fp64): all eigenpairs by one-CTA parallel
  * Jacobi (n <= 256), eigenvalues descending in w, eigenvectors in the columns of V (row-major n x n).
  * Replaces: torch.linalg.eigh round.py:114 / the U,S of torch.linalg.svd round.py:96. */

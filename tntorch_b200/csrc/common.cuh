@@ -1,6 +1,7 @@
 // tnb200 — shared helpers for the CUDA translation unit (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
 #include <atomic>

@@ -1,6 +1,6 @@
 // Generic CUDA-core GEMM used for every shape/dtype the tensor-core kernels do not cover:
-// fp64 everywhere, fp32 with fp32 or fp64 accumulation, bf16 operands (dense TT-SVD input), ragged sizes, both storage
-// orders.
+// fp64 everywhere, fp32 with fp32 or fp64 accumulation, bf16 or fp16 operands (dense TT-SVD input), ragged sizes, both
+// storage orders.
 //
 //   C[M,N] = alpha * sum_k A(m,k) * B(k,n)  (+ beta * D + gamma * E)
 //
@@ -15,7 +15,7 @@ namespace tnb {
 
 constexpr int GEMM_BM = 64, GEMM_BN = 64, GEMM_BK = 16, GEMM_THREADS = 256;
 
-// Operand load: the one place an element becomes the accumulation type (bf16 through fp32, exactly).
+// Operand load: the one place an element becomes the accumulation type (bf16 and fp16 through fp32, exactly).
 template <typename TAcc, typename T>
 __device__ __forceinline__ TAcc gemm_ld(const T& v) {
   return (TAcc)v;
@@ -23,6 +23,10 @@ __device__ __forceinline__ TAcc gemm_ld(const T& v) {
 template <typename TAcc>
 __device__ __forceinline__ TAcc gemm_ld(const __nv_bfloat16& v) {
   return (TAcc)__bfloat162float(v);
+}
+template <typename TAcc>
+__device__ __forceinline__ TAcc gemm_ld(const __half& v) {
+  return (TAcc)__half2float(v);
 }
 
 template <typename TA, typename TB, typename TAcc, typename TC>

@@ -33,6 +33,9 @@
 // consumer accumulates TC_BF16_FLUSH stages into a scratch accumulator (the first wgmma of a group overwrites it) and
 // adds that into its running sum with round-to-nearest fp32 adds, which needs the register room of 128-column tiles.
 // Plan (with tn capped at 128), split-K, tile set, fold, partial layout and finalize are those of the fp32 modes.
+// The mode takes its 16-bit element type as a parameter: fp16 input (gram_tc_f16) runs the same kernel with
+// wgmma m64n128k16 .f32.f16.f16 (same MN-major descriptors) on a TMA map of FLOAT16 elements; an fp16 product is exact
+// in fp32 as well (11-bit significands), and nothing else differs.
 //
 // Replaces, for large fp32 unfoldings, the QR of tensor.py:1816 / the Gram of round.py:104-110.
 #pragma once
@@ -412,26 +415,35 @@ __device__ __forceinline__ uint64_t wgmma_desc_mn_sw128(const void* p, uint32_t 
          ((uint64_t)1 << 62);
 }
 
-// D (64 x 128 fp32) = A (64 x 16) * B (16 x 128) + (accumulate ? D : 0), bf16, both operands MN-major through descriptors.
-__device__ __forceinline__ void wgmma_bf16_ss(float (&d)[64], uint64_t desc_a, uint64_t desc_b, int accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {"
-      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"
-      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
-      "}, %64, %65, p, 1, 1, 1, 1;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
-        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
-        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+// D (64 x 128 fp32) = A (64 x 16) * B (16 x 128) + (accumulate ? D : 0), both operands MN-major through descriptors, of
+// the 16-bit type T16 (bf16 or fp16).
+#define TNB_WGMMA_M64N128K16_SS(TY)                                                                              \
+  asm volatile(                                                                                                  \
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                                         \
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " {"                                              \
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"                                    \
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31,"                          \
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47,"                          \
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"                            \
+      "}, %64, %65, p, 1, 1, 1, 1;\n\t}"                                                                        \
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),          \
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),    \
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),  \
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),  \
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),  \
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),  \
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),  \
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])   \
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate))
+template <typename T16>
+__device__ __forceinline__ void wgmma_16_ss(float (&d)[64], uint64_t desc_a, uint64_t desc_b, int accumulate) {
+  static_assert(std::is_same<T16, __half>::value || std::is_same<T16, __nv_bfloat16>::value, "bf16 or fp16 operands");
+  if constexpr (std::is_same<T16, __half>::value)
+    TNB_WGMMA_M64N128K16_SS("f16");
+  else
+    TNB_WGMMA_M64N128K16_SS("bf16");
 }
+#undef TNB_WGMMA_M64N128K16_SS
 
 // The same m64n256k8 with A read from shared memory through `desc_a` as well (K-blocked mode).
 __device__ __forceinline__ void wgmma_tf32_ss(float (&d)[128], uint64_t desc_a, uint64_t desc_b) {
@@ -642,7 +654,8 @@ __device__ __forceinline__ void gram_tc_consumer_blocked(const GramTcParams& p, 
 // Consumer warpgroup cw of the bf16 mode (tn = 128): A (this warpgroup's 64 columns of C, box a_box + cw) and B (the
 // stage's two boxes, TC_BOX_BYTES apart) through MN-major descriptors, two k16 slices per stage, into the scratch
 // accumulator `part`; every TC_BF16_FLUSH stages (and at the end) `part` is added into `acc` with fp32 adds.  A slot is
-// released once the wgmma group that read it has completed, i.e. one stage later.
+// released once the wgmma group that read it has completed, i.e. one stage later.  T16: bf16 or fp16 operands.
+template <typename T16>
 __device__ __forceinline__ void gram_tc_consumer_bf16(const GramTcParams& p, const unsigned char* stage_base,
                                                       uint64_t* full_bar, uint64_t* empty_bar, int64_t iters, int a_box,
                                                       int tile_id, int split, int a_col0, int b_col0) {
@@ -662,7 +675,7 @@ __device__ __forceinline__ void gram_tc_consumer_bf16(const GramTcParams& p, con
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < TC_KC / 16; ++kk)
-      wgmma_bf16_ss(part, wgmma_desc_mn_sw128(sb + (a_box + cw) * TC_BOX_BYTES + kk * 2048, TC_BOX_BYTES),
+      wgmma_16_ss<T16>(part, wgmma_desc_mn_sw128(sb + (a_box + cw) * TC_BOX_BYTES + kk * 2048, TC_BOX_BYTES),
                     wgmma_desc_mn_sw128(sb + kk * 2048, TC_BOX_BYTES), (first && kk == 0) ? 0 : 1);
     wgmma_commit();
     if ((it + 1) % TC_BF16_FLUSH == 0 || it + 1 == iters) {
@@ -716,8 +729,8 @@ __device__ __forceinline__ void gram_tc_epilogue(const GramTcParams& p, const fl
 
 // TC_KBLOCKED: the operands are K-blocked (see the top of the file); tmap / tmap_b are 3-D maps with boxes (64, 16, 4)
 // and (64, 32, 4).  TC_ROWMAJOR: row-major fp32, 2-D maps with boxes of 32 columns x TC_KC rows.  TC_BF16: row-major
-// bf16, 2-D maps with boxes of 64 columns x TC_KC rows.
-template <int MODE>
+// T16 (bf16 or fp16; the other modes ignore it), 2-D maps with boxes of 64 columns x TC_KC rows.
+template <int MODE, typename T16 = __nv_bfloat16>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_b,
                const GramTcParams p) {
@@ -790,7 +803,7 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
   }
   setmaxnreg_inc<TC_CONSUMER_REGS>();
   if constexpr (BF16) {  // tn = 128
-    gram_tc_consumer_bf16(p, stage_base, full_bar, empty_bar, iters, a_box, tile_id, split, a_col0, b_col0);
+    gram_tc_consumer_bf16<T16>(p, stage_base, full_bar, empty_bar, iters, a_box, tile_id, split, a_col0, b_col0);
     return;
   } else if constexpr (BLOCKED) {  // tn == 256; A inside B: its k8 slices are rows of B's (8 KB apart), else 128-row slices in slot 8
     gram_tc_consumer_blocked(p, stage_base, full_bar, empty_bar, iters,
@@ -952,15 +965,24 @@ inline size_t gram_tc_workspace_bytes(int64_t rows, int64_t n, int max_tn = 256)
   return align_up((size_t)p.ksplit * p.num_tiles * 128 * p.tn * sizeof(float));
 }
 
-// boxes of 128 bytes per row: 32 fp32 or 64 bf16 columns
+// TMA element type of the kernels' inputs: fp32, bf16 or fp16
+template <typename T>
+inline CUtensorMapDataType tma_dtype() {
+  static_assert(std::is_same<T, float>::value || std::is_same<T, __nv_bfloat16>::value || std::is_same<T, __half>::value,
+                "fp32, bf16 or fp16 elements");
+  return std::is_same<T, float>::value           ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+         : std::is_same<T, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                                 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+}
+
+// boxes of 128 bytes per row: 32 fp32 or 64 bf16 / fp16 columns
 template <typename T = float>
 inline int encode_rowmajor_f32(CUtensorMap* tmap, const T* ptr, int64_t rows, int64_t cols, int box_rows = TC_KC) {
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t gstride[1] = {(cuuint64_t)cols * sizeof(T)};
   cuuint32_t box[2] = {128 / (cuuint32_t)sizeof(T), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult cr = get_encode_tiled()(tmap, sizeof(T) == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
-                                   2, const_cast<T*>(ptr), gdim, gstride, box,
+  CUresult cr = get_encode_tiled()(tmap, tma_dtype<T>(), 2, const_cast<T*>(ptr), gdim, gstride, box,
                                    estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (cr != CUDA_SUCCESS) return fail(TNB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)cr);
@@ -985,28 +1007,28 @@ inline bool gram_tc_kblocked_shape_ok(int64_t rows, int64_t n) {
   return gram_tc_shape_ok(rows, n) && n >= 256 && n % 8 == 0 && rows % 8 == 0;
 }
 
-// bf16 input: 16-byte rows (n % 8 == 0) and 128-column tiles: a folded n = 32 / 64, n = 128, or n >= 256 (where the
-// upper-triangle tile set of 128 x 128 tiles covers no more than that of the fp32 modes' 128 x 256 tiles).
+// bf16 / fp16 input: 16-byte rows (n % 8 == 0) and 128-column tiles: a folded n = 32 / 64, n = 128, or n >= 256 (where
+// the upper-triangle tile set of 128 x 128 tiles covers no more than that of the fp32 modes' 128 x 256 tiles).
 inline bool gram_tc_bf16_shape_ok(int64_t rows, int64_t n) {
   return gram_tc_shape_ok(rows, n) && n % 8 == 0 && (gram_tc_fold(rows, n) > 1 || n == 128 || n >= 256);
 }
 template <typename T>
 inline size_t gram_tc_input_workspace_bytes(int64_t rows, int64_t n) {
-  return gram_tc_workspace_bytes(rows, n, std::is_same<T, __nv_bfloat16>::value ? 128 : 256);
+  return gram_tc_workspace_bytes(rows, n, sizeof(T) == 2 ? 128 : 256);
 }
 template <typename T>
 inline bool gram_tc_input_ok(int64_t rows, int64_t n) {
   if (std::is_same<T, float>::value) return gram_tc_shape_ok(rows, n);
-  if (std::is_same<T, __nv_bfloat16>::value) return gram_tc_bf16_shape_ok(rows, n);
+  if (std::is_same<T, __nv_bfloat16>::value || std::is_same<T, __half>::value) return gram_tc_bf16_shape_ok(rows, n);
   return false;
 }
 
-// G (n x n fp64) and optionally Gf (fp32 copy) = A^T A, A: rows x n fp32 or bf16 (device), row-major or, with kblocked
-// (fp32 only), stored K-blocked (then n >= 256, n % 8 == 0 and rows % 8 == 0).
+// G (n x n fp64) and optionally Gf (fp32 copy) = A^T A, A: rows x n fp32, bf16 or fp16 (device), row-major or, with
+// kblocked (fp32 only), stored K-blocked (then n >= 256, n % 8 == 0 and rows % 8 == 0).
 template <typename T>
 inline int gram_tc(const T* A, int64_t rows, int64_t n, double* G, float* Gf, void* ws, size_t ws_bytes,
                    cudaStream_t st, bool kblocked = false) {
-  constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
+  constexpr bool BF16 = sizeof(T) == 2;  // the 16-bit mode, bf16 or fp16
   if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "gram_tc: TMA tensor-core path needs an sm_90 device");
   if (!(kblocked ? !BF16 && gram_tc_kblocked_shape_ok(rows, n) : gram_tc_input_ok<T>(rows, n)))
     return fail(TNB_ERR_UNSUPPORTED, "gram_tc: unsupported shape rows=%lld n=%lld", (long long)rows, (long long)n);
@@ -1028,8 +1050,8 @@ inline int gram_tc(const T* A, int64_t rows, int64_t n, double* G, float* Gf, vo
     CUtensorMap tmap;
     TNB_TRY(encode_rowmajor_f32<T>(&tmap, A, rows, n));
     static PerDeviceFlag attr_done;
-    TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel<TC_BF16>, TC_SMEM_BYTES));
-    gram_tc_kernel<TC_BF16><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(tmap, tmap, p);
+    TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel<TC_BF16, T>, TC_SMEM_BYTES));
+    gram_tc_kernel<TC_BF16, T><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(tmap, tmap, p);
   } else if (kblocked) {
     CUtensorMap ta, tb;
     TNB_TRY(encode_kblocked_f32(&ta, A, rows, n, 128));

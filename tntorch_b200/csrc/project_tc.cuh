@@ -26,6 +26,14 @@
 // accumulate in fp32, so C comes out at fp32 accuracy without an fp32 image of A.  A chunk is 64 bf16 columns: the
 // same 128-byte swizzled rows as 32 fp32 columns, so the tiles, the ring, the schedule and both output layouts are
 // shared, and the 32-bit fragment words sit where the tf32 fragments sit.
+//
+// fp16 A takes the same path with mma.sync m16n8k16 .f16 and two terms of V, scaled per column: fp16's smallest normal
+// is 2^-14, and the second term of an orthonormal V's entries (|v| ~ 0.02-0.1, remainder ~|v| 2^-11) would fall below
+// it.  split_v_f16_kernel picks for column j a power of two s_j that puts max_i |V_ij| s_j in [2^14, 2^15) and stores
+// v1 = fp16(v s_j), v2 = fp16(v s_j - v1) (22 significant bits, what V_hi + V_lo carry on the fp32 path) and 1 / s_j;
+// the epilogue multiplies column j by 1 / s_j, which is exact.  The products stay exact in fp32
+// (|A| |v s| <= 65504 * 2^15 < 2^31).  The scale is chosen on the device: the speculative sweep enqueues the projection
+// without a host read.
 #pragma once
 #include <type_traits>
 
@@ -55,6 +63,7 @@ struct ProjTcParams {
   float* C;
   int inner16;      // PT_OUT_KBLOCKED: inner / 16 row blocks per 8 rows of M
   int64_t out_ld;   // PT_OUT_KBLOCKED: n' = inner * r
+  const float* vscale;  // fp16 A: 1 / s_j of the npad columns of V (split_v_f16_kernel), else nullptr
 };
 
 // element (row m, column k) of a 128 x 32 tile of a K-blocked matrix: 16 runs of 32 columns x 8 rows, each four 8 x 8
@@ -72,21 +81,33 @@ struct PtStage {
 };
 
 
-// D += A * B, m16n8k16, bf16 operands (two per 32-bit word, the lower k in the low half), fp32 accumulation.
-__device__ __forceinline__ void mma_bf16(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
-                                         uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
-      "{%0, %1, %2, %3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+// D += A * B, m16n8k16, 16-bit operands of type T16 (bf16 or fp16, two per 32-bit word, the lower k in the low half),
+// fp32 accumulation.
+template <typename T16>
+__device__ __forceinline__ void mma_k16(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0,
+                                        uint32_t b1) {
+  static_assert(std::is_same<T16, __half>::value || std::is_same<T16, __nv_bfloat16>::value, "bf16 or fp16 operands");
+  if constexpr (std::is_same<T16, __half>::value)
+    asm volatile(
+        "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+        "{%0, %1, %2, %3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+  else
+    asm volatile(
+        "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+        "{%0, %1, %2, %3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
 
-// Per A element type: columns per 128-byte chunk row and the number of V terms (fp32: V_hi, V_lo; bf16: v1, v2, v3).
+// Per A element type: columns per 128-byte chunk row and the number of V terms (fp32: V_hi, V_lo; bf16: v1, v2, v3;
+// fp16: the scaled v1, v2).
 template <typename TA>
 struct PtType {
   static constexpr int KC = 128 / (int)sizeof(TA);
-  static constexpr int VTERMS = sizeof(TA) == 4 ? 2 : 3;
+  static constexpr int VTERMS = std::is_same<TA, __nv_bfloat16>::value ? 3 : 2;
+  static constexpr bool SCALED = std::is_same<TA, __half>::value;  // per-column power-of-two scale of V
 };
 
 // element (row m, column k) of a K-major tile of 32 fp32 columns written by TMA with SWIZZLE_128B
@@ -105,6 +126,10 @@ __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const 
   const int vchunk_bytes = PtType<TA>::VTERMS * p.npad * 128;
   const int vlo_off = p.npad * 128;  // between V terms
   if (p.vres && total_items > 0) mbar_wait(v_bar, 0);
+  float vsc[NT][2];  // fp16 A: 1 / s_j of this thread's output columns 8j + 2t, 8j + 2t + 1
+  if constexpr (PtType<TA>::SCALED)
+#pragma unroll
+    for (int j = 0; j < NT; ++j) vsc[j][0] = p.vscale[8 * j + 2 * t], vsc[j][1] = p.vscale[8 * j + 2 * t + 1];
   float out[NT][4];
 #pragma unroll
   for (int j = 0; j < NT; ++j)
@@ -124,7 +149,7 @@ __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const 
 #pragma unroll
       for (int e = 0; e < 4; ++e) acc[j][e] = 0.f;
 #pragma unroll
-    for (int ks = 0; ks < PT_KC; ks += 8) {  // 8 fragment words: 8 fp32 or 16 bf16 columns
+    for (int ks = 0; ks < PT_KC; ks += 8) {  // 8 fragment words: 8 fp32 or 16 bf16 / fp16 columns
       uint32_t a[4], lo[4];
       if constexpr (MODE == PT_IN_KBLOCKED) {
         a[0] = kb_ld(sa, m0 + g, ks + t);
@@ -137,13 +162,14 @@ __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const 
         a[2] = km_ld(sa, m0 + g, ks + t + 4);
         a[3] = km_ld(sa, m0 + g + 8, ks + t + 4);
       }
-      if constexpr (PtType<TA>::VTERMS == 3) {
+      if constexpr (sizeof(TA) == 2) {  // bf16: C v3, C v2, C v1; fp16: C v2, C v1 (scaled terms)
         const unsigned char* v3 = vl + vlo_off;
 #pragma unroll
         for (int j = 0; j < NT; ++j) {
-          mma_bf16(acc[j], a[0], a[1], a[2], a[3], km_ld(v3, 8 * j + g, ks + t), km_ld(v3, 8 * j + g, ks + t + 4));  // C v3
-          mma_bf16(acc[j], a[0], a[1], a[2], a[3], km_ld(vl, 8 * j + g, ks + t), km_ld(vl, 8 * j + g, ks + t + 4));  // C v2
-          mma_bf16(acc[j], a[0], a[1], a[2], a[3], km_ld(vh, 8 * j + g, ks + t), km_ld(vh, 8 * j + g, ks + t + 4));  // C v1
+          if constexpr (PtType<TA>::VTERMS == 3)
+            mma_k16<TA>(acc[j], a[0], a[1], a[2], a[3], km_ld(v3, 8 * j + g, ks + t), km_ld(v3, 8 * j + g, ks + t + 4));
+          mma_k16<TA>(acc[j], a[0], a[1], a[2], a[3], km_ld(vl, 8 * j + g, ks + t), km_ld(vl, 8 * j + g, ks + t + 4));
+          mma_k16<TA>(acc[j], a[0], a[1], a[2], a[3], km_ld(vh, 8 * j + g, ks + t), km_ld(vh, 8 * j + g, ks + t + 4));
         }
       } else {
 #pragma unroll
@@ -169,6 +195,11 @@ __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const 
     if (++kc < p.nk) continue;
     // row block complete: rows m0+g (c0, c1) and m0+g+8 (c2, c3), columns 8j+2t, 8j+2t+1
     kc = 0;
+    if constexpr (PtType<TA>::SCALED)  // undo the column scale of V: a power of two, exact
+#pragma unroll
+      for (int j = 0; j < NT; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) out[j][e] *= vsc[j][e & 1];
     if constexpr (MODE == PT_OUT_KBLOCKED) {  // r == npad
       constexpr int R = 8 * NT, RS = PtStage<R>::RS, SW = PtStage<R>::SW;
       asm volatile("bar.sync 1, %0;" ::"n"(PT_MMA_WARPS * 32) : "memory");  // the last copy-out has read the staging
@@ -327,7 +358,34 @@ __global__ void split_v_bf16_kernel(const float* __restrict__ V, int K, int r, i
   }
 }
 
-// fp32 A: K % 4 == 0 and K >= 32; bf16 A: K % 8 == 0 and K >= 64 (16-byte rows, one full 128-byte chunk).
+// v1, v2 (npad x K fp16 each, K contiguous) and inv_scale[j] = 1 / s_j from V (K x r), one block per column j:
+// s_j = 2^(15 - e) with max_i |V_ij| = f 2^e, f in [0.5, 1), so that max_i |V_ij| s_j lies in [2^14, 2^15) and the
+// second term stays clear of fp16's subnormals.  The exponent is clamped so that s_j and 1 / s_j are normal fp32 values.
+__global__ void __launch_bounds__(256) split_v_f16_kernel(const float* __restrict__ V, int K, int r, __half* __restrict__ V1,
+                                                          __half* __restrict__ V2, float* __restrict__ inv_scale) {
+  __shared__ float red[8];
+  const int j = blockIdx.x;
+  float m = 0.f;
+  if (j < r)
+    for (int k = threadIdx.x; k < K; k += blockDim.x) m = fmaxf(m, fabsf(V[(size_t)k * r + j]));
+  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = m;
+  __syncthreads();
+  m = red[0];
+  for (int w = 1; w < 8; ++w) m = fmaxf(m, red[w]);
+  int e = 0;
+  frexpf(m, &e);
+  const int sh = m > 0.f ? min(max(15 - e, -126), 126) : 0;
+  for (int k = threadIdx.x; k < K; k += blockDim.x) {
+    const float v = j < r ? ldexpf(V[(size_t)k * r + j], sh) : 0.f;  // exact: a power-of-two scale
+    const __half h1 = __float2half_rn(v);
+    V1[(size_t)j * K + k] = h1;
+    V2[(size_t)j * K + k] = __float2half_rn(v - __half2float(h1));
+  }
+  if (threadIdx.x == 0) inv_scale[j] = ldexpf(1.f, -sh);
+}
+
+// fp32 A: K % 4 == 0 and K >= 32; bf16 / fp16 A: K % 8 == 0 and K >= 64 (16-byte rows, one full 128-byte chunk).
 template <typename TA = float>
 inline bool project_tc_shape_ok(int64_t rows, int64_t K, int64_t r, const void* A, const void* C) {
   constexpr int KC = PtType<TA>::KC;
@@ -335,18 +393,15 @@ inline bool project_tc_shape_ok(int64_t rows, int64_t K, int64_t r, const void* 
          rows < ((int64_t)1 << 31) - 256 && (reinterpret_cast<uintptr_t>(A) & 15u) == 0 &&
          (reinterpret_cast<uintptr_t>(C) & 15u) == 0;
 }
+// the V terms, then (fp16 A) the npad inverse column scales
 template <typename TA = float>
 inline size_t project_tc_workspace_bytes(int64_t K, int64_t r) {
   const int64_t npad = (r + 15) / 16 * 16;
-  return PtType<TA>::VTERMS * align_up((size_t)npad * K * sizeof(TA));
+  return PtType<TA>::VTERMS * align_up((size_t)npad * K * sizeof(TA)) +
+         (PtType<TA>::SCALED ? align_up((size_t)npad * sizeof(float)) : 0);
 }
 
-template <typename T>
-inline CUtensorMapDataType tma_dtype() {
-  return sizeof(T) == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-}
-
-// boxes of 128 bytes (32 fp32 or 64 bf16 columns) x box_rows rows
+// boxes of 128 bytes (32 fp32 or 64 bf16 / fp16 columns) x box_rows rows
 template <typename T = float>
 inline int encode_kmajor_f32(CUtensorMap* tmap, const T* ptr, int64_t rows, int64_t cols, int box_rows) {
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
@@ -360,7 +415,8 @@ inline int encode_kmajor_f32(CUtensorMap* tmap, const T* ptr, int64_t rows, int6
   return TNB_OK;
 }
 
-// C (rows x r) = A (rows x K) V (K x r); ws: project_tc_workspace_bytes<TA>(K, r).  TA: float or __nv_bfloat16.
+// C (rows x r) = A (rows x K) V (K x r); ws: project_tc_workspace_bytes<TA>(K, r).  TA: float, __nv_bfloat16 or
+// __half.
 //   layout PT_ROWMAJOR:     A and C row-major;
 //   layout PT_OUT_KBLOCKED: A row-major, C stored as the K-blocked (gram_tc.cuh) (rows / inner) x (inner * r) matrix;
 //                           needs inner % 16 == 0, rows % (8 * inner) == 0, r % 16 == 0, r <= 48;
@@ -368,14 +424,14 @@ inline int encode_kmajor_f32(CUtensorMap* tmap, const T* ptr, int64_t rows, int6
 template <typename TA>
 inline int project_tc(const TA* A, int64_t rows, int64_t K, const float* V, int r, float* C, void* ws, size_t ws_bytes,
                       cudaStream_t st, int layout = PT_ROWMAJOR, int64_t inner = 0) {
-  constexpr bool BF16 = std::is_same<TA, __nv_bfloat16>::value;
+  constexpr bool BF16 = std::is_same<TA, __nv_bfloat16>::value, F16 = std::is_same<TA, __half>::value;
   constexpr int KC = PtType<TA>::KC, VT = PtType<TA>::VTERMS;
   if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "project_tc: needs an sm_90 device");
   if (!project_tc_shape_ok<TA>(rows, K, r, A, C)) return fail(TNB_ERR_UNSUPPORTED, "project_tc: unsupported shape");
   if (layout == PT_OUT_KBLOCKED && !(inner >= 16 && inner % 16 == 0 && rows % (8 * inner) == 0 && r % 16 == 0 && r <= 48))
     return fail(TNB_ERR_UNSUPPORTED,
                 "project_tc: K-blocked output needs inner %% 16 == 0, rows %% (8 inner) == 0, r %% 16 == 0, r <= 48");
-  if (layout == PT_IN_KBLOCKED && (BF16 || rows % 8 != 0 || K % 8 != 0))
+  if (layout == PT_IN_KBLOCKED && (sizeof(TA) != 4 || rows % 8 != 0 || K % 8 != 0))
     return fail(TNB_ERR_UNSUPPORTED, "project_tc: K-blocked input needs fp32, rows %% 8 == 0 and K %% 8 == 0");
   if (ws_bytes < project_tc_workspace_bytes<TA>(K, r)) return fail(TNB_ERR_WORKSPACE, "project_tc: workspace too small");
   ProjTcParams p;
@@ -393,9 +449,14 @@ inline int project_tc(const TA* A, int64_t rows, int64_t K, const float* V, int 
   const size_t term_bytes = align_up((size_t)p.npad * K * sizeof(TA));
   TA* Vt[3];
   for (int q = 0; q < 3; ++q) Vt[q] = reinterpret_cast<TA*>(static_cast<char*>(ws) + (q < VT ? q : 0) * term_bytes);
-  if constexpr (BF16)
+  p.vscale = nullptr;
+  if constexpr (BF16) {
     split_v_bf16_kernel<<<grid_for((int64_t)p.npad * K), 256, 0, st>>>(V, (int)K, r, p.npad, Vt[0], Vt[1], Vt[2]);
-  else
+  } else if constexpr (F16) {
+    float* inv_scale = reinterpret_cast<float*>(static_cast<char*>(ws) + VT * term_bytes);
+    split_v_f16_kernel<<<p.npad, 256, 0, st>>>(V, (int)K, r, Vt[0], Vt[1], inv_scale);
+    p.vscale = inv_scale;
+  } else
     split_v_kernel<<<grid_for((int64_t)p.npad * K), 256, 0, st>>>(V, (int)K, r, p.npad, Vt[0], Vt[1]);
   TNB_LAUNCH_CHECK();
   CUtensorMap ta, th, tl, t3;
@@ -429,7 +490,7 @@ inline int project_tc(const TA* A, int64_t rows, int64_t K, const float* V, int 
     TNB_CUDA(ensure_dyn_smem(attr_done, project_tc_kernel<PT_OUT_KBLOCKED, TA>, PT_SMEM_BYTES));
     project_tc_kernel<PT_OUT_KBLOCKED, TA><<<(unsigned)grid, PT_THREADS, PT_SMEM_BYTES, st>>>(ta, th, tl, t3, p);
   } else if (layout == PT_IN_KBLOCKED) {
-    if constexpr (!BF16) {
+    if constexpr (sizeof(TA) == 4) {
       static PerDeviceFlag attr_done;
       TNB_CUDA(ensure_dyn_smem(attr_done, project_tc_kernel<PT_IN_KBLOCKED, TA>, PT_SMEM_BYTES));
       project_tc_kernel<PT_IN_KBLOCKED, TA><<<(unsigned)grid, PT_THREADS, PT_SMEM_BYTES, st>>>(ta, th, tl, t3, p);

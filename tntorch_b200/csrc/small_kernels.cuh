@@ -28,12 +28,18 @@ struct SweepScalars {
 // (half the 1e-5 parity bar), with the tail taken at the low end of what the noisy values resolve.  A flat spectrum
 // (random data: lambda_0 << trace, tail ~ trace) passes on the first bound; signal + noise with a clear gap passes on the
 // second; a tensor whose discarded tail is below ~1e-4 of its norm does not, and takes the exact Gram.
-// `noise` is the measured ||E|| / ||G|| of the kernel that produced G (TF32_GRAM_NOISE, BF16_GRAM_NOISE).  The bf16
+// `noise` is the measured ||E|| / ||G|| of the kernel that produced G (TF32_GRAM_NOISE, BF16_GRAM_NOISE,
+// FP16_GRAM_NOISE).  The bf16
 // Gram has exact products and adds its 512-row partial sums with round-to-nearest (gram_tc.cuh): on bf16-rounded
 // randn(2^24, 64), randn(262144, 2048) and a rank-6 signal plus 1e-3 noise of 2^24 x 64, ||G_bf16 - (1 - c) G_fp64||_2 /
 // ||G_fp64||_2 measured 7.3e-9, 9.2e-8 and 6.3e-8, with shrinks c of 9.3e-7, 9.2e-7 and 5.9e-7 (H100 80GB HBM3, 700 W).
+// The fp16 Gram is the same kernel with fp16 operands (exact products as well, the same 512-row round-to-nearest
+// flushes).  Its products carry 22 significant bits against bf16's 16, so more of the fp32 adds round: on the same three
+// inputs rounded to fp16 the noise measured 9.2e-9, 2.2e-7 and 2.9e-7, with shrinks of 2.0e-6, 2.0e-6 and 1.4e-6
+// (scripts/bench_fp16.py --noise-only, H100 80GB HBM3, 700 W).
 constexpr double TF32_GRAM_NOISE = 2e-6;
 constexpr double BF16_GRAM_NOISE = 1e-7;
+constexpr double FP16_GRAM_NOISE = 3e-7;
 __device__ inline int tf32_gram_rejected(const double* w, int nvals, int L, int rank, double trace, double noise) {
   if (rank >= L) return 0;  // nothing discarded
   const double lam0 = w[0] > 0.0 ? w[0] : 0.0;
@@ -141,7 +147,7 @@ __global__ void spec_check_kernel(const SweepScalars* sc, int expect, int32_t* r
   if (f) atomicOr(flags, f);
 }
 
-// out[i] = in[i] in the output type (a bf16 input's single core, N = 1)
+// out[i] = in[i] in the output type (a bf16 or fp16 input's single core, N = 1)
 template <typename TOut, typename TIn>
 __global__ void convert_kernel(const TIn* __restrict__ in, int64_t n, TOut* __restrict__ out) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)

@@ -25,13 +25,14 @@
 
 namespace tnb {
 
-// The input of the dense TT-SVD may be bf16 (TIn); only step 0 reads it, every carry and core is T (fp32 for bf16 input).
+// The input of the dense TT-SVD may be bf16 or fp16 (TIn); only step 0 reads it, every carry and core is T (fp32 for
+// 16-bit input).
 template <typename TIn>
 constexpr bool tc_input() {
-  return std::is_same<TIn, float>::value || std::is_same<TIn, __nv_bfloat16>::value;
+  return std::is_same<TIn, float>::value || std::is_same<TIn, __nv_bfloat16>::value || std::is_same<TIn, __half>::value;
 }
 
-// C (rows x r) = A (rows x n) * V (n x r) in the data precision (fp32 for bf16 A): tensor-core kernel, streaming FFMA
+// C (rows x r) = A (rows x n) * V (n x r) in the data precision (fp32 for 16-bit A): tensor-core kernel, streaming FFMA
 // kernel for fp32 when the shape allows, generic tiled GEMM otherwise.
 constexpr int64_t PROJ_TC_MIN_ROWS = 16384;
 template <typename TIn = float>
@@ -102,7 +103,8 @@ inline int make_dims(int ndim, const int64_t* shape, const int32_t* rmax, SweepD
 // step mu takes the tensor-core Gram unfolded (n' >= 256) and the tensor-core projection, and step mu + 1 projects on the
 // tensor cores with an epilogue that can write it (rcap[mu+1] % 16 == 0 and <= 48, shape[mu] % 16 == 0).  Its Gram then loads
 // K-major operands directly instead of transposing every slab in shared memory.  The writer's own input must be
-// row-major (fp32, or the bf16 input when the writer is step 0), and the last carry (step mu = 0's core) stays row-major.
+// row-major (fp32, or the bf16 / fp16 input when the writer is step 0), and the last carry (step mu = 0's core) stays
+// row-major.
 template <typename T, typename TIn = T>
 inline bool carry_kblocked(const SweepDims& d, int mu, bool allow_tc) {
   if (!std::is_same<T, float>::value || !allow_tc || mu < 1 || mu + 1 > d.N - 1) return false;
@@ -142,7 +144,7 @@ inline void gram_carve(ArenaT& ar, int64_t rows, int64_t n, bool allow_tc, GramW
   }
 }
 
-// *used_tc: 0 exact-product Gram, 1 TF32 tensor-core Gram, 2 bf16 tensor-core Gram (gram_noise)
+// *used_tc: 0 exact-product Gram, 1 TF32 tensor-core Gram, 2 bf16 tensor-core Gram, 3 fp16 tensor-core Gram (gram_noise)
 template <typename T>
 inline int gram_small_side(const T* C, int64_t rows, int64_t n, double* G, float* Gf, GramWork& w, bool use_tc,
                            int* used_tc, cudaStream_t st) {
@@ -151,7 +153,7 @@ inline int gram_small_side(const T* C, int64_t rows, int64_t n, double* G, float
   if (tall) {
     if constexpr (tc_input<T>())
       if (use_tc && w.tc_ws) {
-        if (used_tc) *used_tc = std::is_same<T, __nv_bfloat16>::value ? 2 : 1;
+        if (used_tc) *used_tc = std::is_same<T, __nv_bfloat16>::value ? 2 : std::is_same<T, __half>::value ? 3 : 1;
         return gram_tc<T>(C, rows, n, G, Gf, w.tc_ws, w.tc_bytes, st);
       }
     GemmPlan pl = plan_gemm(n, n, rows, true);
@@ -166,7 +168,7 @@ inline int gram_small_side(const T* C, int64_t rows, int64_t n, double* G, float
 // The accept rule's noise level for a Gram made as gram_small_side's *used_tc says (0: exact, nothing to guard), and,
 // when its eigenpairs come from an fp32 solve, at least the TF32 level that covers the solve (spec_step_eig_begin).
 inline double gram_noise(int used_tc, bool fp32_solve = false) {
-  const double g = used_tc == 2 ? BF16_GRAM_NOISE : used_tc ? TF32_GRAM_NOISE : 0.0;
+  const double g = used_tc == 3 ? FP16_GRAM_NOISE : used_tc == 2 ? BF16_GRAM_NOISE : used_tc ? TF32_GRAM_NOISE : 0.0;
   return fp32_solve ? std::max(g, TF32_GRAM_NOISE) : g;
 }
 
@@ -640,7 +642,7 @@ inline void carve_carries(ArenaT& ar, const SweepDims& d, T* carry[2]) {
   carry[1] = ar.template take<T>(elems[1]);
 }
 
-// T: carries and cores; TIn: the dense input (T, or bf16 with T = float), read by step 0 only.
+// T: carries and cores; TIn: the dense input (T, or bf16 / fp16 with T = float), read by step 0 only.
 template <typename T, typename TIn, class ArenaT>
 inline int ttsvd_sync_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d, const int32_t* rmax, double eps,
                            uint32_t flags, T* cores, int32_t* ranks_host, SweepInfo* info, cudaStream_t st,
