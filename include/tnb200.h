@@ -36,11 +36,14 @@ extern "C" {
 
 #define TNB_F32 0
 #define TNB_F64 1
-/* bf16 and fp16 dense input, accepted by tnb_ttsvd, tnb_ttsvd_batch, tnb_ttsvd_host, their *_workspace_bytes queries
- * and tnb_tt_relative_error (16-bit data, fp32 cores).  The cores, their capacity and info_host are fp32 for 16-bit
- * input; every other entry point rejects both codes with TNB_ERR_INVALID. */
+/* bf16, fp16 and fp8 (e4m3 and e5m2, the OCP formats without unsigned zero) dense input, accepted by tnb_ttsvd,
+ * tnb_ttsvd_batch, tnb_ttsvd_host, their *_workspace_bytes queries and tnb_tt_relative_error (16-bit or 8-bit data, fp32
+ * cores).  The cores, their capacity and info_host are fp32 for such input; every other entry point rejects these codes
+ * with TNB_ERR_INVALID. */
 #define TNB_BF16 2
 #define TNB_F16 3
+#define TNB_F8E4M3 4
+#define TNB_F8E5M2 5
 
 /* flags for tnb_ttsvd / tnb_tt_round */
 #define TNB_FLAG_NO_TENSORCORE 1u /* force the generic fp32/fp64 CUDA-core kernels (debug / parity A-B) */
@@ -317,8 +320,8 @@ int tnb_gram_tc_kblocked_f32(const float* A, int64_t rows, int64_t n, double* G,
 /* The same Gram of a row-major bf16 A (rows x n, n % 8 == 0; n = 32 / 64 with rows divisible by 128 / n, n = 128 or
  * n >= 256): bf16 wgmma, exact products, fp32 accumulation; workspace: tnb_gram_tc_bf16_workspace_bytes. */
 size_t tnb_gram_tc_bf16_workspace_bytes(int64_t rows, int64_t n);
-/* The noise level ||E|| / ||G|| the TT-SVD's accept rule allows for a tensor-core Gram of TNB_F32 (TF32), TNB_BF16 or
- * TNB_F16 input, E = G_tc - (1 - c) G after the uniform shrink c; 0 for other codes. */
+/* The noise level ||E|| / ||G|| the TT-SVD's accept rule allows for a tensor-core Gram of TNB_F32 (TF32), TNB_BF16,
+ * TNB_F16, TNB_F8E4M3 or TNB_F8E5M2 input, E = G_tc - (1 - c) G after the uniform shrink c; 0 for other codes. */
 double tnb_gram_noise_level(int dtype);
 int tnb_gram_tc_bf16(const void* A, int64_t rows, int64_t n, double* G, void* workspace, size_t workspace_bytes,
                      void* stream);
@@ -327,6 +330,12 @@ int tnb_gram_tc_bf16(const void* A, int64_t rows, int64_t n, double* G, void* wo
 size_t tnb_gram_tc_f16_workspace_bytes(int64_t rows, int64_t n);
 int tnb_gram_tc_f16(const void* A, int64_t rows, int64_t n, double* G, void* workspace, size_t workspace_bytes,
                     void* stream);
+/* The same Gram of a row-major fp8 A, dtype TNB_F8E4M3 or TNB_F8E5M2 (shapes of tnb_gram_tc_bf16 with n % 16 == 0): the
+ * fp16 kernel on the values widened to fp16 in shared memory (exact), so exact products and fp32 accumulation;
+ * workspace: tnb_gram_tc_f8_workspace_bytes. */
+size_t tnb_gram_tc_f8_workspace_bytes(int64_t rows, int64_t n);
+int tnb_gram_tc_f8(int dtype, const void* A, int64_t rows, int64_t n, double* G, void* workspace, size_t workspace_bytes,
+                   void* stream);
 /* C (m x n) = alpha * A^T B + beta * D on the same tensor-core kernel (A: K x m, B: K x n, row-major fp32, TF32
  * operands, fp32 accumulation; m, n multiples of 4, >= 32).  The Chebyshev-filter products G*Y of
  * tnb_eig_topk's subspace iteration run through this entry (G symmetric => A = G).  D may be NULL. */
@@ -369,6 +378,10 @@ int tnb_project_tc_bf16(const void* A, int64_t rows, int64_t n, const float* V, 
  * and the scale is divided out of C exactly.  Same shapes, layouts and workspace query as tnb_project_tc_bf16. */
 int tnb_project_tc_f16(const void* A, int64_t rows, int64_t n, const float* V, int32_t r, int64_t inner, float* C,
                        void* workspace, size_t workspace_bytes, void* stream);
+/* The same with A fp8, dtype TNB_F8E4M3 or TNB_F8E5M2: the two scaled fp16 terms of V of tnb_project_tc_f16, A widened to
+ * fp16 in registers (exact); n % 16 == 0, n >= 64, rows >= 128.  Same layouts and workspace query. */
+int tnb_project_tc_f8(int dtype, const void* A, int64_t rows, int64_t n, const float* V, int32_t r, int64_t inner,
+                      float* C, void* workspace, size_t workspace_bytes, void* stream);
 /* Symmetric eigendecomposition of a PSD matrix G (n x n fp64): all eigenpairs by one-CTA parallel
  * Jacobi (n <= 256), eigenvalues descending in w, eigenvectors in the columns of V (row-major n x n).
  * Replaces: torch.linalg.eigh round.py:114 / the U,S of torch.linalg.svd round.py:96. */

@@ -12,7 +12,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libtnb200.so")
 
-TNB_F32, TNB_F64, TNB_BF16, TNB_F16 = 0, 1, 2, 3
+TNB_F32, TNB_F64, TNB_BF16, TNB_F16, TNB_F8E4M3, TNB_F8E5M2 = 0, 1, 2, 3, 4, 5
 FLAG_NO_TENSORCORE = 1
 FLAG_BATCH_MODE = 2
 FLAG_PROFILE = 4
@@ -100,6 +100,10 @@ SIGNATURES = {
     "tnb_gram_tc_f16_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
     "tnb_gram_tc_f16": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, _vp, C.c_size_t, _vp]),
     "tnb_project_tc_f16": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, C.c_int32, C.c_int64, _vp, _vp, C.c_size_t, _vp]),
+    "tnb_gram_tc_f8_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64]),
+    "tnb_gram_tc_f8": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, _vp, C.c_size_t, _vp]),
+    "tnb_project_tc_f8": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, _vp, C.c_int32, C.c_int64, _vp, _vp, C.c_size_t,
+                                    _vp]),
     "tnb_atb_tc_workspace_bytes": (C.c_size_t, [C.c_int64, C.c_int64, C.c_int64]),
     "tnb_atb_tc_f32": (C.c_int, [_vp, C.c_int64, C.c_int64, _vp, C.c_int64, _vp, C.c_float, _vp, C.c_float, _vp,
                                  C.c_size_t, _vp]),

@@ -37,6 +37,13 @@
 // wgmma m64n128k16 .f32.f16.f16 (same MN-major descriptors) on a TMA map of FLOAT16 elements; an fp16 product is exact
 // in fp32 as well (11-bit significands), and nothing else differs.
 //
+// fp8 input (gram_tc_f8, e4m3 or e5m2) runs the fp16 form of that mode.  TMA has no fp8 element type and fp8 wgmma takes
+// K-major operands only, so TMA lands boxes of 128 fp8 columns (UINT8 elements, the same 128-byte swizzled rows) in two
+// raw slots of the stage, and producer warps 1-3 widen each landed stage into the fp16 boxes the consumers read
+// (gram_tc_convert_f8); on a folded tile each consumer warpgroup widens its own 64 columns and runs m64n64k16 on the
+// diagonal block the Gram needs (gram_tc_consumer_bf16).  Every e4m3 and e5m2 value is exact in fp16, so the products, the accumulation order and the
+// result are those of the fp16 mode on the same values.
+//
 // Replaces, for large fp32 unfoldings, the QR of tensor.py:1816 / the Gram of round.py:104-110.
 #pragma once
 #include <cuda.h>
@@ -66,6 +73,7 @@ static_assert(TC_BLK_STAGES * TC_STAGE_BYTES <= TC_RING_BYTES, "K-blocked ring m
 constexpr int TC_BF16_STAGE_BYTES = 6 * TC_BOX_BYTES;  // bf16 mode: 4 B boxes (256 columns) + 2 A boxes, TC_KC rows each
 constexpr int TC_BF16_STAGES = 8;
 constexpr int TC_BF16_FLUSH = 16;               // stages (512 rows) per scratch accumulation of the bf16 mode
+constexpr int TC_F8_RAW_SLOT = 2;               // fp8 input: raw B box in slot 2, raw A box in slot 3 (free in that mode)
 static_assert(TC_BF16_STAGES * TC_BF16_STAGE_BYTES <= TC_RING_BYTES, "bf16 ring must fit the row-major mode's buffers");
 constexpr int TC_MAX_RING = 8;                  // mbarriers per ring
 constexpr int TC_ROWMAJOR = 0, TC_KBLOCKED = 1, TC_BF16 = 2;  // gram_tc_kernel modes
@@ -445,6 +453,37 @@ __device__ __forceinline__ void wgmma_16_ss(float (&d)[64], uint64_t desc_a, uin
 }
 #undef TNB_WGMMA_M64N128K16_SS
 
+// D (64 x 64 fp32) = A (64 x 16) * B (16 x 64) + (accumulate ? D : 0), fp16, both operands MN-major through descriptors
+// (the folded Gram of fp8 input: only the diagonal 64-column block of each warpgroup's rows is needed).
+__device__ __forceinline__ void wgmma_f16_n64_ss(float (&d)[32], uint64_t desc_a, uint64_t desc_b, int accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15,"
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+      "}, %32, %33, p, 1, 1, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate));
+}
+
+// Four fp8 values of type T8 (e4m3 or e5m2) packed in w, the first in the low byte, as two f16x2 words: lo holds the
+// first two, hi the last two.  Exact: every e4m3 and e5m2 value is an fp16 value.
+template <typename T8>
+__device__ __forceinline__ void f8x4_to_f16x2(uint32_t w, uint32_t& lo, uint32_t& hi) {
+  static_assert(std::is_same<T8, __nv_fp8_e4m3>::value || std::is_same<T8, __nv_fp8_e5m2>::value, "e4m3 or e5m2");
+  if constexpr (std::is_same<T8, __nv_fp8_e4m3>::value)
+    asm("{\n\t.reg .b16 l, h;\n\tmov.b32 {l, h}, %2;\n\tcvt.rn.f16x2.e4m3x2 %0, l;\n\tcvt.rn.f16x2.e4m3x2 %1, h;\n\t}"
+        : "=r"(lo), "=r"(hi)
+        : "r"(w));
+  else
+    asm("{\n\t.reg .b16 l, h;\n\tmov.b32 {l, h}, %2;\n\tcvt.rn.f16x2.e5m2x2 %0, l;\n\tcvt.rn.f16x2.e5m2x2 %1, h;\n\t}"
+        : "=r"(lo), "=r"(hi)
+        : "r"(w));
+}
+
 // The same m64n256k8 with A read from shared memory through `desc_a` as well (K-blocked mode).
 __device__ __forceinline__ void wgmma_tf32_ss(float (&d)[128], uint64_t desc_a, uint64_t desc_b) {
   asm volatile(
@@ -493,12 +532,15 @@ static_assert(TcRing<TC_BF16>::STAGES <= TC_MAX_RING && TcRing<TC_KBLOCKED>::STA
 // Loads of pipeline iteration `it` (rows it_begin + it) into its ring slot, once the transposers and the consumers have
 // released it.  B first (slots 0..nbox_b), then A (slots A_SLOT..).  Row-major: boxes of 32 columns.  bf16: boxes of 64
 // columns.  K-blocked: one box of (64, tn / 8 column groups, 4 row groups) for B and one of (64, 16, 4) for A, i.e.
-// four k8 slices of tn (128) columns x 32 bytes.
-template <int MODE>
+// four k8 slices of tn (128) columns x 32 bytes.  F8 (bf16 mode, fp8 input): boxes of 128 fp8 columns into the raw
+// slots TC_F8_RAW_SLOT (B) and TC_F8_RAW_SLOT + 1 (A), completing on `full_bar` = the converters' raw barriers.
+template <int MODE, bool F8 = false>
 __device__ __forceinline__ void gram_tc_produce(const CUtensorMap* tmap, const CUtensorMap* tmap_b, unsigned char* stage_base,
                                                 uint64_t* full_bar, uint64_t* empty_bar, int64_t it, int64_t it_begin,
                                                 int nbox_a, int nbox_b, int a_col0, int b_col0) {
   using R = TcRing<MODE>;
+  constexpr int BOX_COLS = F8 ? 128 : R::BOX_COLS, B_SLOT = F8 ? TC_F8_RAW_SLOT : 0;
+  constexpr int A_SLOT = F8 ? TC_F8_RAW_SLOT + 1 : R::A_SLOT;
   const int stage = (int)(it % R::STAGES);
   const uint32_t phase = (uint32_t)(it / R::STAGES) & 1u;
   mbar_wait_quiet(&empty_bar[stage], phase ^ 1u);
@@ -510,9 +552,55 @@ __device__ __forceinline__ void gram_tc_produce(const CUtensorMap* tmap, const C
     if (nbox_a) tma_load_3d(sb + 8 * TC_BOX_BYTES, tmap, &full_bar[stage], 0, a_col0 / 8, row0 / 8);
   } else {
     for (int j = 0; j < nbox_b; ++j)
-      tma_load_2d(sb + j * TC_BOX_BYTES, tmap_b, &full_bar[stage], b_col0 + R::BOX_COLS * j, row0);
+      tma_load_2d(sb + (B_SLOT + j) * TC_BOX_BYTES, tmap_b, &full_bar[stage], b_col0 + BOX_COLS * j, row0);
     for (int j = 0; j < nbox_a; ++j)
-      tma_load_2d(sb + (R::A_SLOT + j) * TC_BOX_BYTES, tmap, &full_bar[stage], a_col0 + R::BOX_COLS * j, row0);
+      tma_load_2d(sb + (A_SLOT + j) * TC_BOX_BYTES, tmap, &full_bar[stage], a_col0 + BOX_COLS * j, row0);
+  }
+}
+
+// fp8 input, producer warps 1-3: widen every landed stage (raw_bar) from its raw boxes of 128 fp8 columns (B, and A when
+// `raw_a`) into the fp16 boxes of 64 columns the consumers read (B: slots 0-1; A: slots A_SLOT, A_SLOT + 1), then
+// arrive on the stage's full barrier, which counts these 96 threads.  Both layouts are 128-byte swizzled rows: the
+// 16-byte chunk c of raw row k (fp8 columns 16c .. 16c + 15, at chunk c ^ k%8) becomes chunks 2(c%4) and 2(c%4) + 1 of
+// fp16 box c / 4 (at chunk ^ k%8).  Eight lanes take the eight chunks of one row, so the loads and the stores of a warp
+// touch every bank equally.  The stage's previous fp16 contents were released by the consumers before TMA refilled it.
+// Each thread loads two chunks before it widens either, so their shared-memory latencies overlap.
+__device__ __forceinline__ uint4 f8_raw_ld(const unsigned char* sb, int u) {
+  const int box = u / (TC_KC * 8), k = (u >> 3) % TC_KC, c = u & 7;
+  return *reinterpret_cast<const uint4*>(sb + (TC_F8_RAW_SLOT + box) * TC_BOX_BYTES + k * 128 + ((c ^ (k & 7)) << 4));
+}
+template <typename T8>
+__device__ __forceinline__ void f8_widen_st(unsigned char* sb, int u, const uint4& v) {
+  const int box = u / (TC_KC * 8), k = (u >> 3) % TC_KC, c = u & 7, sw = k & 7;
+  uint4 lo, hi;
+  f8x4_to_f16x2<T8>(v.x, lo.x, lo.y);
+  f8x4_to_f16x2<T8>(v.y, lo.z, lo.w);
+  f8x4_to_f16x2<T8>(v.z, hi.x, hi.y);
+  f8x4_to_f16x2<T8>(v.w, hi.z, hi.w);
+  unsigned char* row = sb + ((box ? TcRing<TC_BF16>::A_SLOT : 0) + (c >> 2)) * TC_BOX_BYTES + k * 128;
+  const int c0 = (c & 3) << 1;
+  *reinterpret_cast<uint4*>(row + ((c0 ^ sw) << 4)) = lo;
+  *reinterpret_cast<uint4*>(row + (((c0 + 1) ^ sw) << 4)) = hi;
+}
+template <typename T8>
+__device__ __forceinline__ void gram_tc_convert_f8(unsigned char* stage_base, uint64_t* raw_bar, uint64_t* full_bar,
+                                                   int64_t iters, bool raw_a) {
+  using R = TcRing<TC_BF16>;
+  const int tid = threadIdx.x - 32, units = (raw_a ? 2 : 1) * TC_KC * 8;
+  for (int64_t it = 0; it < iters; ++it) {
+    const int s = (int)(it % R::STAGES);
+    mbar_wait_quiet(&raw_bar[s], (uint32_t)(it / R::STAGES) & 1u);
+    unsigned char* sb = stage_base + s * R::STAGE_BYTES;
+    for (int u = tid; u < units; u += 2 * TC_TRANSPOSE_THREADS) {
+      const int u1 = u + TC_TRANSPOSE_THREADS;
+      const uint4 v0 = f8_raw_ld(sb, u);
+      uint4 v1 = v0;
+      if (u1 < units) v1 = f8_raw_ld(sb, u1);
+      f8_widen_st<T8>(sb, u, v0);
+      if (u1 < units) f8_widen_st<T8>(sb, u1, v1);
+    }
+    fence_proxy_async_smem();  // the stores are read by wgmma (async proxy)
+    mbar_arrive(&full_bar[s]);
   }
 }
 
@@ -655,34 +743,56 @@ __device__ __forceinline__ void gram_tc_consumer_blocked(const GramTcParams& p, 
 // stage's two boxes, TC_BOX_BYTES apart) through MN-major descriptors, two k16 slices per stage, into the scratch
 // accumulator `part`; every TC_BF16_FLUSH stages (and at the end) `part` is added into `acc` with fp32 adds.  A slot is
 // released once the wgmma group that read it has completed, i.e. one stage later.  T16: bf16 or fp16 operands.
-template <typename T16>
+// T8 (e4m3 or e5m2; a folded tile of fp8 input): the Gram is the sum of the diagonal n x n blocks (n = 32 or 64), all
+// inside the 64 x 64 block of columns 64 cw .. 64 cw + 63 of the warpgroup's rows.  So the warpgroup needs only fp16 box
+// cw, as both A and B, and widens it itself: `full_bar` is then the TMA (raw) barrier, each of its 128 threads widens
+// one 16-byte chunk of the raw box (row t / 4, chunk 4 cw + t % 4), and a warpgroup barrier orders the stores before the
+// wgmma, which overlaps the previous stage's.  The wgmma is m64n64k16: half the tensor-core work of the full 128 x 128
+// tile, the same sum for every element the finalize reads (the other half of the partial tile is never written nor
+// read).  Widening in the three producer warps instead kept that Gram at 0.87 ms on the 64^5 step 0, against 0.53 ms
+// with the widening removed (H100 80GB HBM3, 700 W).
+template <typename T16, typename T8 = void>
 __device__ __forceinline__ void gram_tc_consumer_bf16(const GramTcParams& p, const unsigned char* stage_base,
                                                       uint64_t* full_bar, uint64_t* empty_bar, int64_t iters, int a_box,
                                                       int tile_id, int split, int a_col0, int b_col0) {
   using R = TcRing<TC_BF16>;
+  constexpr bool DIAG64 = !std::is_void<T8>::value;
+  constexpr int NACC = DIAG64 ? 32 : 64;
   const int ct = threadIdx.x - 128;
   const int lane = ct & 31, w = (ct >> 5) & 3, cw = ct >> 7;
   const int cm = 64 * cw + 16 * w;
-  float acc[64], part[64];
+  float acc[NACC], part[NACC];
 #pragma unroll
-  for (int i = 0; i < 64; ++i) acc[i] = 0.f, part[i] = 0.f;
+  for (int i = 0; i < NACC; ++i) acc[i] = 0.f, part[i] = 0.f;
   wgmma_fence_operand(part);
   for (int64_t it = 0; it < iters; ++it) {
     const int s = (int)(it % R::STAGES);
     mbar_wait_spin(&full_bar[s], (uint32_t)(it / R::STAGES) & 1u);
     const unsigned char* sb = stage_base + s * R::STAGE_BYTES;
     const int first = it % TC_BF16_FLUSH == 0;
+    if constexpr (DIAG64) {
+      const int u = ((ct & 127) >> 2) * 8 + 4 * cw + (ct & 3);  // raw B box (slot TC_F8_RAW_SLOT), row u / 8, chunk u % 8
+      unsigned char* sbw = const_cast<unsigned char*>(sb);
+      f8_widen_st<T8>(sbw, u, f8_raw_ld(sb, u));
+      fence_proxy_async_smem();  // the stores are read by wgmma (async proxy)
+      asm volatile("bar.sync %0, 128;" ::"r"(2 + cw) : "memory");
+    }
     wgmma_fence();
 #pragma unroll
-    for (int kk = 0; kk < TC_KC / 16; ++kk)
-      wgmma_16_ss<T16>(part, wgmma_desc_mn_sw128(sb + (a_box + cw) * TC_BOX_BYTES + kk * 2048, TC_BOX_BYTES),
-                    wgmma_desc_mn_sw128(sb + kk * 2048, TC_BOX_BYTES), (first && kk == 0) ? 0 : 1);
+    for (int kk = 0; kk < TC_KC / 16; ++kk) {
+      if constexpr (DIAG64)
+        wgmma_f16_n64_ss(part, wgmma_desc_mn_sw128(sb + (a_box + cw) * TC_BOX_BYTES + kk * 2048, TC_BOX_BYTES),
+                         wgmma_desc_mn_sw128(sb + cw * TC_BOX_BYTES + kk * 2048, TC_BOX_BYTES), (first && kk == 0) ? 0 : 1);
+      else
+        wgmma_16_ss<T16>(part, wgmma_desc_mn_sw128(sb + (a_box + cw) * TC_BOX_BYTES + kk * 2048, TC_BOX_BYTES),
+                         wgmma_desc_mn_sw128(sb + kk * 2048, TC_BOX_BYTES), (first && kk == 0) ? 0 : 1);
+    }
     wgmma_commit();
     if ((it + 1) % TC_BF16_FLUSH == 0 || it + 1 == iters) {
       wgmma_wait<0>();
       wgmma_fence_operand(part);
 #pragma unroll
-      for (int i = 0; i < 64; ++i) acc[i] += part[i];
+      for (int i = 0; i < NACC; ++i) acc[i] += part[i];
       wgmma_fence_operand(part);
     } else {
       wgmma_wait<1>();
@@ -690,7 +800,18 @@ __device__ __forceinline__ void gram_tc_consumer_bf16(const GramTcParams& p, con
     __syncwarp();
     if (it > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % R::STAGES]);
   }
-  gram_tc_epilogue<4>(p, acc, cm, lane, tile_id, split, a_col0, b_col0);
+  if constexpr (DIAG64) {  // columns 64 cw .. 64 cw + 63 of the partial tile (a folded Gram is never direct)
+    const int g = lane >> 2, t = lane & 3;
+    float* out = p.partial + ((size_t)split * p.num_tiles + tile_id) * 128 * (size_t)p.tn + 64 * cw + 2 * t;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        *reinterpret_cast<float2*>(out + (size_t)(cm + g + 8 * h) * p.tn + 8 * j) =
+            make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+  } else {
+    gram_tc_epilogue<4>(p, acc, cm, lane, tile_id, split, a_col0, b_col0);
+  }
 }
 
 // Output of one consumer warp: acc[4j + 2h + e] is (row cm + g + 8h, column 8j + 2t + e) of the 128 x tn tile.
@@ -729,11 +850,13 @@ __device__ __forceinline__ void gram_tc_epilogue(const GramTcParams& p, const fl
 
 // TC_KBLOCKED: the operands are K-blocked (see the top of the file); tmap / tmap_b are 3-D maps with boxes (64, 16, 4)
 // and (64, 32, 4).  TC_ROWMAJOR: row-major fp32, 2-D maps with boxes of 32 columns x TC_KC rows.  TC_BF16: row-major
-// T16 (bf16 or fp16; the other modes ignore it), 2-D maps with boxes of 64 columns x TC_KC rows.
+// T16 (bf16 or fp16; the other modes ignore it), 2-D maps with boxes of 64 columns x TC_KC rows; T16 fp8 (e4m3 or
+// e5m2): UINT8 maps with boxes of 128 columns x TC_KC rows, widened to fp16 in shared memory.
 template <int MODE, typename T16 = __nv_bfloat16>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__ CUtensorMap tmap_b,
                const GramTcParams p) {
+  constexpr bool F8 = sizeof(T16) == 1;
   extern __shared__ unsigned char tc_smem_raw[];
   // 1024-byte aligned stage buffers (SWIZZLE_128B atoms are 1024 B)
   const uint32_t raw_addr = smem_u32(tc_smem_raw);
@@ -746,6 +869,8 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
   uint64_t* tb_full = empty_bar + TC_MAX_RING;
   uint64_t* tb_empty = tb_full + TC_TB_STAGES;
   int* tile_smem = reinterpret_cast<int*>(tb_empty + TC_TB_STAGES);  // bm, bn
+  uint64_t* raw_bar = reinterpret_cast<uint64_t*>(tile_smem + 2);     // fp8 input: TMA -> converters
+  static_assert((2 * TC_MAX_RING + 2 * TC_TB_STAGES + 1 + TC_MAX_RING) * 8 <= 256, "barriers must fit their 256 bytes");
 
   const int tile_id = blockIdx.x, split = blockIdx.y;
 
@@ -766,7 +891,8 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
     tile_smem[0] = fbm;
     tile_smem[1] = fbn;
     for (int s = 0; s < TcRing<MODE>::STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
+      mbar_init(&full_bar[s], F8 ? TC_TRANSPOSE_THREADS : 1);  // fp8: the converters, per thread
+      if constexpr (F8) mbar_init(&raw_bar[s], 1);
       // per warp: transposers and consumers (K-blocked, bf16: consumers only)
       mbar_init(&empty_bar[s], (MODE == TC_ROWMAJOR ? TC_TRANSPOSE_THREADS / 32 : 0) + 8);
     }
@@ -792,7 +918,15 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
 
   if (threadIdx.x < 128) {  // producer warpgroup
     setmaxnreg_dec<TC_PRODUCER_REGS>();
-    if (threadIdx.x == 0) {
+    if constexpr (F8) {  // one raw box of 128 fp8 columns per 128-column operand
+      if (threadIdx.x == 0) {
+        for (int64_t it = 0; it < iters; ++it)
+          gram_tc_produce<MODE, true>(&tmap, &tmap_b, stage_base, raw_bar, empty_bar, it, it_begin, nbox_a / 2,
+                                      nbox_b / 2, a_col0, b_col0);
+      } else if (threadIdx.x >= 32 && p.fold == 1) {  // a folded tile is widened by its consumers
+        gram_tc_convert_f8<T16>(stage_base, raw_bar, full_bar, iters, nbox_a > 0);
+      }
+    } else if (threadIdx.x == 0) {
       for (int64_t it = 0; it < iters; ++it)
         gram_tc_produce<MODE>(&tmap, &tmap_b, stage_base, full_bar, empty_bar, it, it_begin, nbox_a, nbox_b, a_col0,
                               b_col0);
@@ -803,7 +937,15 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
   }
   setmaxnreg_inc<TC_CONSUMER_REGS>();
   if constexpr (BF16) {  // tn = 128
-    gram_tc_consumer_bf16<T16>(p, stage_base, full_bar, empty_bar, iters, a_box, tile_id, split, a_col0, b_col0);
+    if constexpr (F8) {
+      if (p.fold > 1)
+        gram_tc_consumer_bf16<__half, T16>(p, stage_base, raw_bar, empty_bar, iters, a_box, tile_id, split, a_col0,
+                                           b_col0);
+      else
+        gram_tc_consumer_bf16<__half>(p, stage_base, full_bar, empty_bar, iters, a_box, tile_id, split, a_col0, b_col0);
+    } else {
+      gram_tc_consumer_bf16<T16>(p, stage_base, full_bar, empty_bar, iters, a_box, tile_id, split, a_col0, b_col0);
+    }
     return;
   } else if constexpr (BLOCKED) {  // tn == 256; A inside B: its k8 slices are rows of B's (8 KB apart), else 128-row slices in slot 8
     gram_tc_consumer_blocked(p, stage_base, full_bar, empty_bar, iters,
@@ -965,17 +1107,24 @@ inline size_t gram_tc_workspace_bytes(int64_t rows, int64_t n, int max_tn = 256)
   return align_up((size_t)p.ksplit * p.num_tiles * 128 * p.tn * sizeof(float));
 }
 
-// TMA element type of the kernels' inputs: fp32, bf16 or fp16
 template <typename T>
-inline CUtensorMapDataType tma_dtype() {
-  static_assert(std::is_same<T, float>::value || std::is_same<T, __nv_bfloat16>::value || std::is_same<T, __half>::value,
-                "fp32, bf16 or fp16 elements");
-  return std::is_same<T, float>::value           ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
-         : std::is_same<T, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
-                                                 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+constexpr bool is_fp8() {
+  return std::is_same<T, __nv_fp8_e4m3>::value || std::is_same<T, __nv_fp8_e5m2>::value;
 }
 
-// boxes of 128 bytes per row: 32 fp32 or 64 bf16 / fp16 columns
+// TMA element type of the kernels' inputs: fp32, bf16, fp16, or bytes for fp8 (TMA has no fp8 type)
+template <typename T>
+inline CUtensorMapDataType tma_dtype() {
+  static_assert(std::is_same<T, float>::value || std::is_same<T, __nv_bfloat16>::value || std::is_same<T, __half>::value ||
+                    is_fp8<T>(),
+                "fp32, bf16, fp16 or fp8 elements");
+  return std::is_same<T, float>::value           ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+         : std::is_same<T, __nv_bfloat16>::value ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+         : std::is_same<T, __half>::value        ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                                 : CU_TENSOR_MAP_DATA_TYPE_UINT8;
+}
+
+// boxes of 128 bytes per row: 32 fp32, 64 bf16 / fp16 or 128 fp8 columns
 template <typename T = float>
 inline int encode_rowmajor_f32(CUtensorMap* tmap, const T* ptr, int64_t rows, int64_t cols, int box_rows = TC_KC) {
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
@@ -1012,23 +1161,26 @@ inline bool gram_tc_kblocked_shape_ok(int64_t rows, int64_t n) {
 inline bool gram_tc_bf16_shape_ok(int64_t rows, int64_t n) {
   return gram_tc_shape_ok(rows, n) && n % 8 == 0 && (gram_tc_fold(rows, n) > 1 || n == 128 || n >= 256);
 }
+// fp8 input: the same tiles, and 16-byte rows of fp8 (n % 16 == 0).
+inline bool gram_tc_f8_shape_ok(int64_t rows, int64_t n) { return gram_tc_bf16_shape_ok(rows, n) && n % 16 == 0; }
 template <typename T>
 inline size_t gram_tc_input_workspace_bytes(int64_t rows, int64_t n) {
-  return gram_tc_workspace_bytes(rows, n, sizeof(T) == 2 ? 128 : 256);
+  return gram_tc_workspace_bytes(rows, n, sizeof(T) <= 2 ? 128 : 256);
 }
 template <typename T>
 inline bool gram_tc_input_ok(int64_t rows, int64_t n) {
   if (std::is_same<T, float>::value) return gram_tc_shape_ok(rows, n);
   if (std::is_same<T, __nv_bfloat16>::value || std::is_same<T, __half>::value) return gram_tc_bf16_shape_ok(rows, n);
+  if (is_fp8<T>()) return gram_tc_f8_shape_ok(rows, n);
   return false;
 }
 
-// G (n x n fp64) and optionally Gf (fp32 copy) = A^T A, A: rows x n fp32, bf16 or fp16 (device), row-major or, with
+// G (n x n fp64) and optionally Gf (fp32 copy) = A^T A, A: rows x n fp32, bf16, fp16 or fp8 (device), row-major or, with
 // kblocked (fp32 only), stored K-blocked (then n >= 256, n % 8 == 0 and rows % 8 == 0).
 template <typename T>
 inline int gram_tc(const T* A, int64_t rows, int64_t n, double* G, float* Gf, void* ws, size_t ws_bytes,
                    cudaStream_t st, bool kblocked = false) {
-  constexpr bool BF16 = sizeof(T) == 2;  // the 16-bit mode, bf16 or fp16
+  constexpr bool BF16 = sizeof(T) <= 2;  // the 16-bit mode: bf16, fp16, or fp8 widened to fp16
   if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "gram_tc: TMA tensor-core path needs an sm_90 device");
   if (!(kblocked ? !BF16 && gram_tc_kblocked_shape_ok(rows, n) : gram_tc_input_ok<T>(rows, n)))
     return fail(TNB_ERR_UNSUPPORTED, "gram_tc: unsupported shape rows=%lld n=%lld", (long long)rows, (long long)n);

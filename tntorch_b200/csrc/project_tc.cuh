@@ -34,6 +34,15 @@
 // the epilogue multiplies column j by 1 / s_j, which is exact.  The products stay exact in fp32
 // (|A| |v s| <= 65504 * 2^15 < 2^31).  The scale is chosen on the device: the speculative sweep enqueues the projection
 // without a host read.
+//
+// fp8 A (e4m3 or e5m2) uses those two scaled fp16 terms of V as they are.  A chunk is 128 fp8 columns (TMA boxes of
+// UINT8, the same 128-byte swizzled rows, so A's tiles and ring are the fp32 path's), and each V term of a chunk is two
+// 64-column fp16 boxes.  A fragment word (km_ld, the tf32 access pattern) holds four consecutive k; it is widened to two
+// f16x2 words in registers (exact) and feeds two mma.sync m16n8k16 .f16 whose k order is permuted the same way for A and
+// V: word w of the row pairs with the 8-byte V load of k 4w .. 4w + 3.  An fp8 value times an fp16 term has at most
+// 4 + 11 significant bits, so the products stay exact in fp32 (|A| |v s| <= 57344 * 2^15).  K need only be a multiple of
+// 16 and >= 64: the A box reads zeros past K, the V boxes past K are not loaded, and the 32-wide k-steps past K are
+// skipped (K = 64, the 64^5 step-0 shape, fills half an A box and one V box per term).
 #pragma once
 #include <type_traits>
 
@@ -102,17 +111,38 @@ __device__ __forceinline__ void mma_k16(float (&d)[4], uint32_t a0, uint32_t a1,
 }
 
 // Per A element type: columns per 128-byte chunk row and the number of V terms (fp32: V_hi, V_lo; bf16: v1, v2, v3;
-// fp16: the scaled v1, v2).
+// fp16 and fp8: the scaled fp16 v1, v2), their element type TV and the 128-byte V boxes per term and chunk.
 template <typename TA>
 struct PtType {
   static constexpr int KC = 128 / (int)sizeof(TA);
   static constexpr int VTERMS = std::is_same<TA, __nv_bfloat16>::value ? 3 : 2;
-  static constexpr bool SCALED = std::is_same<TA, __half>::value;  // per-column power-of-two scale of V
+  static constexpr bool SCALED = sizeof(TA) <= 2 && !std::is_same<TA, __nv_bfloat16>::value;  // per-column 2^e scale of V
+  using TV = std::conditional_t<sizeof(TA) == 1, __half, TA>;
+  static constexpr int VSUB = sizeof(TA) == 1 ? 2 : 1;
 };
+
+// fp8 A: V boxes of chunk kc that start inside K (the second 64 columns of the last chunk may lie past it)
+__device__ __forceinline__ int pt_f8_vsub(const ProjTcParams& p, int kc) { return kc * 128 + 64 < p.K ? 2 : 1; }
 
 // element (row m, column k) of a K-major tile of 32 fp32 columns written by TMA with SWIZZLE_128B
 __device__ __forceinline__ uint32_t km_ld(const unsigned char* base, int m, int k) {
   return *reinterpret_cast<const uint32_t*>(base + m * 128 + ((((k >> 2) ^ (m & 7))) << 4) + ((k & 3) << 2));
+}
+
+// fp8 A: the fp16 values of one V term at column `col`, k 4w .. 4w + 3 of the chunk (two f16x2 words), from the term's
+// two boxes of 64 columns (box w / 16: npad rows of 128 bytes, 128-byte swizzle)
+__device__ __forceinline__ uint2 pt_f8_vld(const unsigned char* v, int npad, int col, int w) {
+  return *reinterpret_cast<const uint2*>(v + (w >> 4) * npad * 128 + col * 128 + ((((w & 15) >> 1) ^ (col & 7)) << 4) +
+                                         ((w & 1) << 3));
+}
+
+// fp8 A: TMA loads of V chunk kc, both terms and the boxes pt_f8_vsub keeps, into dst as [term][box][npad rows][128 B]
+__device__ __forceinline__ void pt_f8_load_v(unsigned char* dst, const CUtensorMap* th, const CUtensorMap* tl,
+                                             uint64_t* bar, const ProjTcParams& p, int kc) {
+  for (int h = 0; h < pt_f8_vsub(p, kc); ++h) {
+    tma_load_2d(dst + h * p.npad * 128, th, bar, kc * 128 + 64 * h, 0);
+    tma_load_2d(dst + (2 + h) * p.npad * 128, tl, bar, kc * 128 + 64 * h, 0);
+  }
 }
 
 // NT = npad / 8 n8 tiles
@@ -123,8 +153,8 @@ __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const 
   const int w = (threadIdx.x >> 5) - 1, lane = threadIdx.x & 31;
   const int g = lane >> 2, t = lane & 3;
   const int m0 = 16 * w;
-  const int vchunk_bytes = PtType<TA>::VTERMS * p.npad * 128;
-  const int vlo_off = p.npad * 128;  // between V terms
+  const int vchunk_bytes = PtType<TA>::VTERMS * PtType<TA>::VSUB * p.npad * 128;
+  const int vlo_off = PtType<TA>::VSUB * p.npad * 128;  // between V terms
   if (p.vres && total_items > 0) mbar_wait(v_bar, 0);
   float vsc[NT][2];  // fp16 A: 1 / s_j of this thread's output columns 8j + 2t, 8j + 2t + 1
   if constexpr (PtType<TA>::SCALED)
@@ -149,7 +179,9 @@ __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const 
 #pragma unroll
       for (int e = 0; e < 4; ++e) acc[j][e] = 0.f;
 #pragma unroll
-    for (int ks = 0; ks < PT_KC; ks += 8) {  // 8 fragment words: 8 fp32 or 16 bf16 / fp16 columns
+    for (int ks = 0; ks < PT_KC; ks += 8) {  // 8 fragment words: 8 fp32, 16 bf16 / fp16 or 32 fp8 columns
+      if constexpr (sizeof(TA) == 1)
+        if (kc * 128 + 4 * ks >= p.K) break;  // past K: A and V are zero there
       uint32_t a[4], lo[4];
       if constexpr (MODE == PT_IN_KBLOCKED) {
         a[0] = kb_ld(sa, m0 + g, ks + t);
@@ -162,7 +194,21 @@ __device__ __forceinline__ void project_tc_consume(const ProjTcParams& p, const 
         a[2] = km_ld(sa, m0 + g, ks + t + 4);
         a[3] = km_ld(sa, m0 + g + 8, ks + t + 4);
       }
-      if constexpr (sizeof(TA) == 2) {  // bf16: C v3, C v2, C v1; fp16: C v2, C v1 (scaled terms)
+      if constexpr (sizeof(TA) == 1) {  // fp8: C v2, C v1 (scaled fp16 terms), k 4w, 4w + 1 in x, 4w + 2, 4w + 3 in y
+        uint32_t x[4], y[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) f8x4_to_f16x2<TA>(a[i], x[i], y[i]);
+#pragma unroll
+        for (int j = 0; j < NT; ++j) {
+          const int col = 8 * j + g;
+          const uint2 l0 = pt_f8_vld(vl, p.npad, col, ks + t), l1 = pt_f8_vld(vl, p.npad, col, ks + t + 4);
+          const uint2 h0 = pt_f8_vld(vh, p.npad, col, ks + t), h1 = pt_f8_vld(vh, p.npad, col, ks + t + 4);
+          mma_k16<__half>(acc[j], x[0], x[1], x[2], x[3], l0.x, l1.x);
+          mma_k16<__half>(acc[j], y[0], y[1], y[2], y[3], l0.y, l1.y);
+          mma_k16<__half>(acc[j], x[0], x[1], x[2], x[3], h0.x, h1.x);
+          mma_k16<__half>(acc[j], y[0], y[1], y[2], y[3], h0.y, h1.y);
+        }
+      } else if constexpr (sizeof(TA) == 2) {  // bf16: C v3, C v2, C v1; fp16: C v2, C v1 (scaled terms)
         const unsigned char* v3 = vl + vlo_off;
 #pragma unroll
         for (int j = 0; j < NT; ++j) {
@@ -262,7 +308,8 @@ project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(stage_base + PT_RING_BYTES + PT_STG_MAX_BYTES);
   uint64_t* empty_bar = full_bar + PT_MAX_STAGES;
   uint64_t* v_bar = empty_bar + PT_MAX_STAGES;
-  const int vchunk_bytes = VT * p.npad * 128;
+  constexpr bool F8 = sizeof(TA) == 1;
+  const int vchunk_bytes = VT * PtType<TA>::VSUB * p.npad * 128;
 
   const int warp_idx = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
@@ -281,7 +328,14 @@ project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   if (warp_idx == 0) {
     // ================= TMA producer =================
     if (lane == 0) {
-      if (p.vres && total_items > 0) {
+      if constexpr (F8) {
+        if (p.vres && total_items > 0) {
+          uint32_t bytes = 0;
+          for (int kc = 0; kc < p.nk; ++kc) bytes += (uint32_t)(VT * pt_f8_vsub(p, kc) * p.npad * 128);
+          mbar_expect_tx(v_bar, bytes);
+          for (int kc = 0; kc < p.nk; ++kc) pt_f8_load_v(v_res + (size_t)kc * vchunk_bytes, &tmap_vhi, &tmap_vlo, v_bar, p, kc);
+        }
+      } else if (p.vres && total_items > 0) {
         mbar_expect_tx(v_bar, (uint32_t)(p.nk * vchunk_bytes));
         for (int kc = 0; kc < p.nk; ++kc) {
           tma_load_2d(v_res + (size_t)kc * vchunk_bytes, &tmap_vhi, v_bar, kc * PtType<TA>::KC, 0);
@@ -297,7 +351,11 @@ project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       for (int64_t item = 0; item < total_items; ++item) {
         mbar_wait(&empty_bar[stage], phase ^ 1u);
         unsigned char* sb = stage_base + (size_t)stage * p.stage_bytes;
-        mbar_expect_tx(&full_bar[stage], tx_bytes);
+        if constexpr (F8)
+          mbar_expect_tx(&full_bar[stage],
+                         (uint32_t)PT_A_BYTES + (p.vres ? 0u : (uint32_t)(VT * pt_f8_vsub(p, kc) * p.npad * 128)));
+        else
+          mbar_expect_tx(&full_bar[stage], tx_bytes);
         constexpr int KC = PtType<TA>::KC;
         if (MODE == PT_OUT_KBLOCKED)
           tma_load_3d(sb, &tmap_a, &full_bar[stage], kc * KC, (rb % p.inner16) * 16, (rb / p.inner16) * 8);
@@ -305,7 +363,9 @@ project_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
           tma_load_2d(sb, &tmap_a, &full_bar[stage], kc * KC * 8, rb * (PT_BM / 8));
         else
           tma_load_2d(sb, &tmap_a, &full_bar[stage], kc * KC, rb * PT_BM);
-        if (!p.vres) {
+        if constexpr (F8) {
+          if (!p.vres) pt_f8_load_v(sb + PT_A_BYTES, &tmap_vhi, &tmap_vlo, &full_bar[stage], p, kc);
+        } else if (!p.vres) {
           tma_load_2d(sb + PT_A_BYTES, &tmap_vhi, &full_bar[stage], kc * KC, 0);
           tma_load_2d(sb + PT_A_BYTES + p.npad * 128, &tmap_vlo, &full_bar[stage], kc * KC, 0);  // rows npad..2npad-1
           if (VT == 3) tma_load_2d(sb + PT_A_BYTES + 2 * p.npad * 128, &tmap_v3, &full_bar[stage], kc * KC, 0);
@@ -385,23 +445,24 @@ __global__ void __launch_bounds__(256) split_v_f16_kernel(const float* __restric
   if (threadIdx.x == 0) inv_scale[j] = ldexpf(1.f, -sh);
 }
 
-// fp32 A: K % 4 == 0 and K >= 32; bf16 / fp16 A: K % 8 == 0 and K >= 64 (16-byte rows, one full 128-byte chunk).
+// fp32 A: K % 4 == 0 and K >= 32; bf16 / fp16 A: K % 8 == 0 and K >= 64 (16-byte rows, one full 128-byte chunk); fp8 A:
+// K % 16 == 0 and K >= 64 (16-byte rows, one full V box).
 template <typename TA = float>
 inline bool project_tc_shape_ok(int64_t rows, int64_t K, int64_t r, const void* A, const void* C) {
-  constexpr int KC = PtType<TA>::KC;
-  return r >= 1 && r <= PT_MAX_N && K % (16 / (int)sizeof(TA)) == 0 && K >= KC && K <= (1 << 24) && rows >= 128 &&
+  constexpr int KMIN = sizeof(TA) == 1 ? 64 : PtType<TA>::KC;
+  return r >= 1 && r <= PT_MAX_N && K % (16 / (int)sizeof(TA)) == 0 && K >= KMIN && K <= (1 << 24) && rows >= 128 &&
          rows < ((int64_t)1 << 31) - 256 && (reinterpret_cast<uintptr_t>(A) & 15u) == 0 &&
          (reinterpret_cast<uintptr_t>(C) & 15u) == 0;
 }
-// the V terms, then (fp16 A) the npad inverse column scales
+// the V terms, then (fp16 / fp8 A) the npad inverse column scales
 template <typename TA = float>
 inline size_t project_tc_workspace_bytes(int64_t K, int64_t r) {
   const int64_t npad = (r + 15) / 16 * 16;
-  return PtType<TA>::VTERMS * align_up((size_t)npad * K * sizeof(TA)) +
+  return PtType<TA>::VTERMS * align_up((size_t)npad * K * sizeof(typename PtType<TA>::TV)) +
          (PtType<TA>::SCALED ? align_up((size_t)npad * sizeof(float)) : 0);
 }
 
-// boxes of 128 bytes (32 fp32 or 64 bf16 / fp16 columns) x box_rows rows
+// boxes of 128 bytes (32 fp32, 64 bf16 / fp16 or 128 fp8 columns) x box_rows rows
 template <typename T = float>
 inline int encode_kmajor_f32(CUtensorMap* tmap, const T* ptr, int64_t rows, int64_t cols, int box_rows) {
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
@@ -415,8 +476,8 @@ inline int encode_kmajor_f32(CUtensorMap* tmap, const T* ptr, int64_t rows, int6
   return TNB_OK;
 }
 
-// C (rows x r) = A (rows x K) V (K x r); ws: project_tc_workspace_bytes<TA>(K, r).  TA: float, __nv_bfloat16 or
-// __half.
+// C (rows x r) = A (rows x K) V (K x r); ws: project_tc_workspace_bytes<TA>(K, r).  TA: float, __nv_bfloat16, __half,
+// __nv_fp8_e4m3 or __nv_fp8_e5m2.
 //   layout PT_ROWMAJOR:     A and C row-major;
 //   layout PT_OUT_KBLOCKED: A row-major, C stored as the K-blocked (gram_tc.cuh) (rows / inner) x (inner * r) matrix;
 //                           needs inner % 16 == 0, rows % (8 * inner) == 0, r % 16 == 0, r <= 48;
@@ -425,7 +486,9 @@ template <typename TA>
 inline int project_tc(const TA* A, int64_t rows, int64_t K, const float* V, int r, float* C, void* ws, size_t ws_bytes,
                       cudaStream_t st, int layout = PT_ROWMAJOR, int64_t inner = 0) {
   constexpr bool BF16 = std::is_same<TA, __nv_bfloat16>::value, F16 = std::is_same<TA, __half>::value;
+  constexpr bool F8 = sizeof(TA) == 1;
   constexpr int KC = PtType<TA>::KC, VT = PtType<TA>::VTERMS;
+  using TV = typename PtType<TA>::TV;
   if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "project_tc: needs an sm_90 device");
   if (!project_tc_shape_ok<TA>(rows, K, r, A, C)) return fail(TNB_ERR_UNSUPPORTED, "project_tc: unsupported shape");
   if (layout == PT_OUT_KBLOCKED && !(inner >= 16 && inner % 16 == 0 && rows % (8 * inner) == 0 && r % 16 == 0 && r <= 48))
@@ -441,18 +504,18 @@ inline int project_tc(const TA* A, int64_t rows, int64_t K, const float* V, int 
   p.C = C;
   p.inner16 = layout == PT_OUT_KBLOCKED ? (int)(inner / 16) : 1;
   p.out_ld = layout == PT_OUT_KBLOCKED ? inner * r : 0;
-  const int vchunk = VT * p.npad * 128;
+  const int vchunk = VT * PtType<TA>::VSUB * p.npad * 128;
   p.vres = ((int64_t)p.nk * vchunk <= PT_VRES_MAX_BYTES) ? 1 : 0;
   p.stage_bytes = PT_A_BYTES + (p.vres ? 0 : vchunk);
   p.nstages = (PT_RING_BYTES - (p.vres ? p.nk * vchunk : 0)) / p.stage_bytes;
   if (p.nstages > PT_MAX_STAGES) p.nstages = PT_MAX_STAGES;
-  const size_t term_bytes = align_up((size_t)p.npad * K * sizeof(TA));
-  TA* Vt[3];
-  for (int q = 0; q < 3; ++q) Vt[q] = reinterpret_cast<TA*>(static_cast<char*>(ws) + (q < VT ? q : 0) * term_bytes);
+  const size_t term_bytes = align_up((size_t)p.npad * K * sizeof(TV));
+  TV* Vt[3];
+  for (int q = 0; q < 3; ++q) Vt[q] = reinterpret_cast<TV*>(static_cast<char*>(ws) + (q < VT ? q : 0) * term_bytes);
   p.vscale = nullptr;
   if constexpr (BF16) {
     split_v_bf16_kernel<<<grid_for((int64_t)p.npad * K), 256, 0, st>>>(V, (int)K, r, p.npad, Vt[0], Vt[1], Vt[2]);
-  } else if constexpr (F16) {
+  } else if constexpr (F16 || F8) {
     float* inv_scale = reinterpret_cast<float*>(static_cast<char*>(ws) + VT * term_bytes);
     split_v_f16_kernel<<<p.npad, 256, 0, st>>>(V, (int)K, r, Vt[0], Vt[1], inv_scale);
     p.vscale = inv_scale;
@@ -479,10 +542,10 @@ inline int project_tc(const TA* A, int64_t rows, int64_t K, const float* V, int 
     TNB_TRY(encode_kmajor_f32<TA>(&ta, A, rows, K, PT_BM));
   }
   if (cr != CUDA_SUCCESS) return fail(TNB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d)", (int)cr);
-  TNB_TRY(encode_kmajor_f32<TA>(&th, Vt[0], p.npad, K, p.npad));
-  TNB_TRY(encode_kmajor_f32<TA>(&tl, Vt[1], p.npad, K, p.npad));
+  TNB_TRY(encode_kmajor_f32<TV>(&th, Vt[0], p.npad, K, p.npad));
+  TNB_TRY(encode_kmajor_f32<TV>(&tl, Vt[1], p.npad, K, p.npad));
   t3 = th;
-  if (VT == 3) TNB_TRY(encode_kmajor_f32<TA>(&t3, Vt[2], p.npad, K, p.npad));
+  if (VT == 3) TNB_TRY(encode_kmajor_f32<TV>(&t3, Vt[2], p.npad, K, p.npad));
   const int sms = usable_sms();
   const int64_t grid = p.num_row_blocks < sms ? p.num_row_blocks : sms;
   if (layout == PT_OUT_KBLOCKED) {

@@ -653,7 +653,7 @@ __global__ void __launch_bounds__(256) recon_diff_kernel(const T* __restrict__ F
   }
 }
 
-// TD: the data's element type (T, or bf16 / fp16 with fp32 cores)
+// TD: the data's element type (T, or bf16 / fp16 / fp8 with fp32 cores)
 template <typename T, typename TD, class ArenaT>
 inline int tt_relative_error_impl(ArenaT& ar, bool dry, const TD* data, const T* const* cores, int N,
                                   const int64_t* shape, const int32_t* ranks, double* result_host, cudaStream_t st) {

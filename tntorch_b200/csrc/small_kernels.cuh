@@ -29,7 +29,7 @@ struct SweepScalars {
 // (random data: lambda_0 << trace, tail ~ trace) passes on the first bound; signal + noise with a clear gap passes on the
 // second; a tensor whose discarded tail is below ~1e-4 of its norm does not, and takes the exact Gram.
 // `noise` is the measured ||E|| / ||G|| of the kernel that produced G (TF32_GRAM_NOISE, BF16_GRAM_NOISE,
-// FP16_GRAM_NOISE).  The bf16
+// FP16_GRAM_NOISE, FP8_GRAM_NOISE).  The bf16
 // Gram has exact products and adds its 512-row partial sums with round-to-nearest (gram_tc.cuh): on bf16-rounded
 // randn(2^24, 64), randn(262144, 2048) and a rank-6 signal plus 1e-3 noise of 2^24 x 64, ||G_bf16 - (1 - c) G_fp64||_2 /
 // ||G_fp64||_2 measured 7.3e-9, 9.2e-8 and 6.3e-8, with shrinks c of 9.3e-7, 9.2e-7 and 5.9e-7 (H100 80GB HBM3, 700 W).
@@ -37,9 +37,15 @@ struct SweepScalars {
 // flushes).  Its products carry 22 significant bits against bf16's 16, so more of the fp32 adds round: on the same three
 // inputs rounded to fp16 the noise measured 9.2e-9, 2.2e-7 and 2.9e-7, with shrinks of 2.0e-6, 2.0e-6 and 1.4e-6
 // (scripts/bench_fp16.py --noise-only, H100 80GB HBM3, 700 W).
+// The fp8 Gram is the fp16 kernel on the values widened to fp16 (FP8_GRAM_NOISE, both formats).  A product of two e4m3
+// (e5m2) values has at most 8 (6) significant bits, so fewer of the fp32 adds round than for fp16: on the same three
+// inputs rounded to e4m3 the noise measured 6.6e-9, 5.5e-8 and 3.7e-8 (shrinks 1.8e-7, 1.8e-7, 6.5e-8), rounded to e5m2
+// 6.0e-9, 5.0e-8 and 2.2e-8 (shrinks 1.3e-7, 1.3e-7, 4.1e-8) (scripts/bench_fp8.py --noise-only and
+// tests/test_gpu_fp8.py, H100 80GB HBM3, 700 W).  Both maxima fall under one level.
 constexpr double TF32_GRAM_NOISE = 2e-6;
 constexpr double BF16_GRAM_NOISE = 1e-7;
 constexpr double FP16_GRAM_NOISE = 3e-7;
+constexpr double FP8_GRAM_NOISE = 6e-8;
 __device__ inline int tf32_gram_rejected(const double* w, int nvals, int L, int rank, double trace, double noise) {
   if (rank >= L) return 0;  // nothing discarded
   const double lam0 = w[0] > 0.0 ? w[0] : 0.0;
@@ -147,7 +153,7 @@ __global__ void spec_check_kernel(const SweepScalars* sc, int expect, int32_t* r
   if (f) atomicOr(flags, f);
 }
 
-// out[i] = in[i] in the output type (a bf16 or fp16 input's single core, N = 1)
+// out[i] = in[i] in the output type (a bf16, fp16 or fp8 input's single core, N = 1)
 template <typename TOut, typename TIn>
 __global__ void convert_kernel(const TIn* __restrict__ in, int64_t n, TOut* __restrict__ out) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)

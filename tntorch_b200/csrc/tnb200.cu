@@ -22,13 +22,18 @@ inline int check_dtype(int dtype) {
   if (dtype != TNB_F32 && dtype != TNB_F64) return fail(TNB_ERR_INVALID, "dtype must be TNB_F32 or TNB_F64, got %d", dtype);
   return TNB_OK;
 }
-// The dense TT-SVD entry points also take bf16 and fp16 input (fp32 cores).
+// The dense TT-SVD entry points also take bf16, fp16 and fp8 (e4m3, e5m2) input (fp32 cores).
 inline int check_ttsvd_dtype(int dtype) {
-  if (dtype != TNB_F32 && dtype != TNB_F64 && dtype != TNB_BF16 && dtype != TNB_F16)
-    return fail(TNB_ERR_INVALID, "dtype must be TNB_F32, TNB_F64, TNB_BF16 or TNB_F16, got %d", dtype);
+  if (dtype != TNB_F32 && dtype != TNB_F64 && dtype != TNB_BF16 && dtype != TNB_F16 && dtype != TNB_F8E4M3 &&
+      dtype != TNB_F8E5M2)
+    return fail(TNB_ERR_INVALID, "dtype must be TNB_F32, TNB_F64, TNB_BF16, TNB_F16, TNB_F8E4M3 or TNB_F8E5M2, got %d",
+                dtype);
   return TNB_OK;
 }
-inline size_t dtype_bytes(int dtype) { return dtype == TNB_F64 ? 8 : dtype == TNB_F32 ? 4 : 2; }
+inline bool is_f8_code(int dtype) { return dtype == TNB_F8E4M3 || dtype == TNB_F8E5M2; }
+inline size_t dtype_bytes(int dtype) {
+  return dtype == TNB_F64 ? 8 : dtype == TNB_F32 ? 4 : is_f8_code(dtype) ? 1 : 2;
+}
 inline int require_device() {
   int dev = -1;
   if (cudaGetDevice(&dev) != cudaSuccess || !device_info().valid) {
@@ -70,6 +75,12 @@ size_t tnb_ttsvd_workspace_bytes(int dtype, int ndim, const int64_t* shape, cons
                                           nullptr, 0);
   else if (dtype == TNB_F16)
     rc = ttsvd_impl<float, __half>(ar, true, (const __half*)nullptr, d, rmax, 0.0, flags, nullptr, nullptr, nullptr, 0);
+  else if (dtype == TNB_F8E4M3)
+    rc = ttsvd_impl<float, __nv_fp8_e4m3>(ar, true, (const __nv_fp8_e4m3*)nullptr, d, rmax, 0.0, flags, nullptr, nullptr,
+                                          nullptr, 0);
+  else if (dtype == TNB_F8E5M2)
+    rc = ttsvd_impl<float, __nv_fp8_e5m2>(ar, true, (const __nv_fp8_e5m2*)nullptr, d, rmax, 0.0, flags, nullptr, nullptr,
+                                          nullptr, 0);
   else
     rc = ttsvd_impl<double, double>(ar, true, (const double*)nullptr, d, rmax, 0.0, flags, nullptr, nullptr, nullptr, 0);
   if (rc != TNB_OK) return 0;
@@ -102,6 +113,12 @@ int tnb_ttsvd(int dtype, const void* data, int ndim, const int64_t* shape, const
   else if (dtype == TNB_F16)
     rc = ttsvd_impl<float, __half>(ar, false, static_cast<const __half*>(data), d, rmax, eps, flags,
                                    static_cast<float*>(cores), ranks_host, &info, as_stream(stream));
+  else if (dtype == TNB_F8E4M3)
+    rc = ttsvd_impl<float, __nv_fp8_e4m3>(ar, false, static_cast<const __nv_fp8_e4m3*>(data), d, rmax, eps, flags,
+                                          static_cast<float*>(cores), ranks_host, &info, as_stream(stream));
+  else if (dtype == TNB_F8E5M2)
+    rc = ttsvd_impl<float, __nv_fp8_e5m2>(ar, false, static_cast<const __nv_fp8_e5m2*>(data), d, rmax, eps, flags,
+                                          static_cast<float*>(cores), ranks_host, &info, as_stream(stream));
   else
     rc = ttsvd_impl<double, double>(ar, false, static_cast<const double*>(data), d, rmax, eps, flags,
                                     static_cast<double*>(cores), ranks_host, &info, as_stream(stream));
@@ -173,6 +190,14 @@ int tnb_ttsvd_batch(int dtype, const void* const* data, int batch, int ndim, con
     return ttsvd_batch_impl<float, __half>(workspace, one, inflight, reinterpret_cast<const __half* const*>(data), batch, d,
                                            rmax, eps, flags, reinterpret_cast<float* const*>(cores), ranks_host, norms_host,
                                            speculative_host, as_stream(stream));
+  if (dtype == TNB_F8E4M3)
+    return ttsvd_batch_impl<float, __nv_fp8_e4m3>(workspace, one, inflight, reinterpret_cast<const __nv_fp8_e4m3* const*>(data),
+                                                  batch, d, rmax, eps, flags, reinterpret_cast<float* const*>(cores), ranks_host,
+                                                  norms_host, speculative_host, as_stream(stream));
+  if (dtype == TNB_F8E5M2)
+    return ttsvd_batch_impl<float, __nv_fp8_e5m2>(workspace, one, inflight, reinterpret_cast<const __nv_fp8_e5m2* const*>(data),
+                                                  batch, d, rmax, eps, flags, reinterpret_cast<float* const*>(cores), ranks_host,
+                                                  norms_host, speculative_host, as_stream(stream));
   return ttsvd_batch_impl<double, double>(workspace, one, inflight, reinterpret_cast<const double* const*>(data), batch, d, rmax, eps,
                                   flags, reinterpret_cast<double* const*>(cores), ranks_host, norms_host, speculative_host,
                                   as_stream(stream));
@@ -187,7 +212,7 @@ int tnb_ttsvd_host(int dtype, const void* data_host, int ndim, const int64_t* sh
   SweepDims d;
   TNB_TRY(make_dims(ndim, shape, rmax, d));
   const size_t total = (size_t)d.rows[ndim] * dtype_bytes(dtype);
-  const size_t core_esz = dtype == TNB_F64 ? 8 : 4;  // bf16 / fp16 input: fp32 cores
+  const size_t core_esz = dtype == TNB_F64 ? 8 : 4;  // bf16 / fp16 / fp8 input: fp32 cores
   cudaStream_t st = as_stream(stream);
   // chunked so that a pageable source still overlaps its staging copies with the DMA
   const size_t chunk = (size_t)256 << 20;
@@ -646,6 +671,7 @@ double tnb_gram_noise_level(int dtype) {
   return dtype == TNB_F32    ? TF32_GRAM_NOISE
          : dtype == TNB_BF16 ? BF16_GRAM_NOISE
          : dtype == TNB_F16  ? FP16_GRAM_NOISE
+         : is_f8_code(dtype) ? FP8_GRAM_NOISE
                              : 0.0;
 }
 
@@ -666,6 +692,21 @@ int tnb_gram_tc_f16(const void* A, int64_t rows, int64_t n, double* G, void* wor
   TNB_TRY(require_device());
   if (!A || !G || !workspace) return fail(TNB_ERR_INVALID, "tnb_gram_tc_f16: null argument");
   return gram_tc(static_cast<const __half*>(A), rows, n, G, nullptr, workspace, workspace_bytes, as_stream(stream));
+}
+
+size_t tnb_gram_tc_f8_workspace_bytes(int64_t rows, int64_t n) {
+  if (!gram_tc_f8_shape_ok(rows, n)) return 0;
+  return gram_tc_input_workspace_bytes<__nv_fp8_e4m3>(rows, n) + 256;
+}
+
+int tnb_gram_tc_f8(int dtype, const void* A, int64_t rows, int64_t n, double* G, void* workspace, size_t workspace_bytes,
+                   void* stream) {
+  if (!is_f8_code(dtype)) return fail(TNB_ERR_INVALID, "tnb_gram_tc_f8: dtype must be TNB_F8E4M3 or TNB_F8E5M2");
+  TNB_TRY(require_device());
+  if (!A || !G || !workspace) return fail(TNB_ERR_INVALID, "tnb_gram_tc_f8: null argument");
+  if (dtype == TNB_F8E4M3)
+    return gram_tc(static_cast<const __nv_fp8_e4m3*>(A), rows, n, G, nullptr, workspace, workspace_bytes, as_stream(stream));
+  return gram_tc(static_cast<const __nv_fp8_e5m2*>(A), rows, n, G, nullptr, workspace, workspace_bytes, as_stream(stream));
 }
 
 size_t tnb_atb_tc_workspace_bytes(int64_t K, int64_t m, int64_t n) {
@@ -752,6 +793,19 @@ int tnb_project_tc_f16(const void* A, int64_t rows, int64_t n, const float* V, i
                     inner > 0 ? PT_OUT_KBLOCKED : PT_ROWMAJOR, inner);
 }
 
+int tnb_project_tc_f8(int dtype, const void* A, int64_t rows, int64_t n, const float* V, int32_t r, int64_t inner,
+                      float* C, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!is_f8_code(dtype)) return fail(TNB_ERR_INVALID, "tnb_project_tc_f8: dtype must be TNB_F8E4M3 or TNB_F8E5M2");
+  TNB_TRY(require_device());
+  if (!A || !V || !C || !workspace) return fail(TNB_ERR_INVALID, "tnb_project_tc_f8: null argument");
+  const int layout = inner > 0 ? PT_OUT_KBLOCKED : PT_ROWMAJOR;
+  if (dtype == TNB_F8E4M3)
+    return project_tc(static_cast<const __nv_fp8_e4m3*>(A), rows, n, V, r, C, workspace, workspace_bytes, as_stream(stream),
+                      layout, inner);
+  return project_tc(static_cast<const __nv_fp8_e5m2*>(A), rows, n, V, r, C, workspace, workspace_bytes, as_stream(stream),
+                    layout, inner);
+}
+
 size_t tnb_eigh_workspace_bytes(int32_t n) {
   if (n < 1 || n > JACOBI_MAX_N) return 0;
   return align_up(jacobi_scratch_doubles(n) * sizeof(double)) + 256;
@@ -812,7 +866,7 @@ size_t tnb_tt_relative_error_workspace_bytes(int dtype, int ndim, const int64_t*
   int rc;
   if (dtype == TNB_F64)
     rc = tt_relative_error_impl<double, double>(ar, true, nullptr, nullptr, ndim, shape, ranks, nullptr, 0);
-  else  // fp32 cores for fp32, bf16 and fp16 data
+  else  // fp32 cores for fp32, bf16, fp16 and fp8 data
     rc = tt_relative_error_impl<float, float>(ar, true, nullptr, nullptr, ndim, shape, ranks, nullptr, 0);
   return rc == TNB_OK ? ar.off + 4096 : 0;
 }
@@ -837,6 +891,14 @@ int tnb_tt_relative_error(int dtype, const void* data, const void* const* cores,
     return tt_relative_error_impl<float, __half>(ar, false, static_cast<const __half*>(data),
                                                  reinterpret_cast<const float* const*>(cores), ndim, shape, ranks,
                                                  result_host, as_stream(stream));
+  if (dtype == TNB_F8E4M3)
+    return tt_relative_error_impl<float, __nv_fp8_e4m3>(ar, false, static_cast<const __nv_fp8_e4m3*>(data),
+                                                        reinterpret_cast<const float* const*>(cores), ndim, shape, ranks,
+                                                        result_host, as_stream(stream));
+  if (dtype == TNB_F8E5M2)
+    return tt_relative_error_impl<float, __nv_fp8_e5m2>(ar, false, static_cast<const __nv_fp8_e5m2*>(data),
+                                                        reinterpret_cast<const float* const*>(cores), ndim, shape, ranks,
+                                                        result_host, as_stream(stream));
   return tt_relative_error_impl<double, double>(ar, false, static_cast<const double*>(data),
                                         reinterpret_cast<const double* const*>(cores), ndim, shape, ranks, result_host,
                                         as_stream(stream));

@@ -22,20 +22,22 @@ def _dtype_code(t: torch.Tensor) -> int:
     return _DT[t.dtype]
 
 
-# The dense TT-SVD (ttsvd, ttsvd_batch, their plans, tt_relative_error) also reads bfloat16 and float16 data; its cores
-# are float32.
-_DT_DENSE = {**_DT, torch.bfloat16: _lib.TNB_BF16, torch.float16: _lib.TNB_F16}
-_DT_16 = (torch.bfloat16, torch.float16)
+# The dense TT-SVD (ttsvd, ttsvd_batch, their plans, tt_relative_error) also reads bfloat16, float16 and float8 (e4m3fn,
+# e5m2) data; its cores are float32.
+_DT_F8 = {torch.float8_e4m3fn: _lib.TNB_F8E4M3, torch.float8_e5m2: _lib.TNB_F8E5M2}
+_DT_DENSE = {**_DT, torch.bfloat16: _lib.TNB_BF16, torch.float16: _lib.TNB_F16, **_DT_F8}
+_DT_LOW = (torch.bfloat16, torch.float16, *_DT_F8)  # read as they are, float32 cores
 
 
 def _dense_code(dtype: torch.dtype) -> int:
     if dtype not in _DT_DENSE:
-        raise ValueError(f"the dense TT-SVD supports float32/float64/bfloat16/float16 tensors, got {dtype}")
+        raise ValueError("the dense TT-SVD supports float32/float64/bfloat16/float16/float8_e4m3fn/float8_e5m2 tensors, "
+                         f"got {dtype}")
     return _DT_DENSE[dtype]
 
 
 def _core_dtype(dtype: torch.dtype) -> torch.dtype:
-    return torch.float32 if dtype in _DT_16 else dtype
+    return torch.float32 if dtype in _DT_LOW else dtype
 
 
 def _require_cuda(t: torch.Tensor, what: str):
@@ -776,9 +778,27 @@ def gram_f16(A: torch.Tensor) -> torch.Tensor:
     return G
 
 
+def gram_f8(A: torch.Tensor) -> torch.Tensor:
+    """fp64 A^T A of a row-major float8 (e4m3fn or e5m2, rows x n) matrix on the tensor-core Gram kernel, the values
+    widened to fp16 in shared memory (exact products, fp32 accumulation); the shapes of gram_bf16 with n % 16 == 0."""
+    _require_cuda(A, "gram_f8")
+    assert A.dtype in _DT_F8
+    A = A.contiguous()
+    rows, n = A.shape
+    G = torch.empty(n, n, dtype=torch.float64, device=A.device)
+    L = lib()
+    wsb = L.tnb_gram_tc_f8_workspace_bytes(rows, n)
+    if wsb == 0:
+        check(_lib.ERR_UNSUPPORTED)
+    ws = _ws(wsb, A.device)
+    with torch.cuda.device(A.device):
+        check(L.tnb_gram_tc_f8(_DT_F8[A.dtype], _ptr(A), rows, n, _ptr(G), _ptr(ws), ws.numel(), _stream()))
+    return G
+
+
 def gram_noise_level(dtype: torch.dtype) -> float:
     """||G_tc - (1 - c) G|| / ||G|| the TT-SVD's accept rule allows for the tensor-core Gram of float32 (TF32),
-    bfloat16 or float16 input."""
+    bfloat16, float16 or float8 (e4m3fn, e5m2) input."""
     return float(lib().tnb_gram_noise_level(_dense_code(dtype)))
 
 
@@ -818,6 +838,27 @@ def project_f16(A: torch.Tensor, V: torch.Tensor, inner: int = 0) -> torch.Tenso
     ws = _ws(wsb, A.device)
     with torch.cuda.device(A.device):
         check(L.tnb_project_tc_f16(_ptr(A), rows, n, _ptr(V), r, int(inner), _ptr(out), _ptr(ws), ws.numel(), _stream()))
+    return out
+
+
+def project_f8(A: torch.Tensor, V: torch.Tensor, inner: int = 0) -> torch.Tensor:
+    """A (rows x n, float8 e4m3fn or e5m2) @ V (n x r, float32) at fp32 accuracy on the tensor cores (A widened to fp16
+    in registers, the two scaled fp16 terms of V of project_f16), float32 result.  inner > 0 writes it K-blocked like
+    project_kblocked_out (returned flat)."""
+    _require_cuda(A, "project_f8")
+    assert A.dtype in _DT_F8 and V.dtype == torch.float32
+    A, V = A.contiguous(), V.contiguous()
+    rows, n = A.shape
+    r = V.shape[1]
+    out = torch.empty(rows * r if inner > 0 else (rows, r), dtype=torch.float32, device=A.device)
+    L = lib()
+    wsb = L.tnb_project_tc_workspace_bytes(n, r)
+    if wsb == 0:
+        check(_lib.ERR_UNSUPPORTED)
+    ws = _ws(wsb, A.device)
+    with torch.cuda.device(A.device):
+        check(L.tnb_project_tc_f8(_DT_F8[A.dtype], _ptr(A), rows, n, _ptr(V), r, int(inner), _ptr(out), _ptr(ws),
+                                  ws.numel(), _stream()))
     return out
 
 
@@ -952,14 +993,14 @@ def eig_topk(G: torch.Tensor, k: int, b: int = 0, tol: float = 1e-6):
 
 
 def tt_relative_error(data: torch.Tensor, cores: Sequence[torch.Tensor]) -> float:
-    """‖data − TT(cores)‖_F / ‖data‖_F, fp64 accumulation on the device (metrics.py:135-151).  bfloat16 and float16
-    data take float32 cores (what ttsvd returns for them)."""
+    """‖data − TT(cores)‖_F / ‖data‖_F, fp64 accumulation on the device (metrics.py:135-151).  bfloat16, float16 and
+    float8 data take float32 cores (what ttsvd returns for them)."""
     _require_cuda(data, "tt_relative_error")
     data = data.contiguous()
     cores = [c.contiguous() for c in cores]
     N = data.dim()
     code = _dense_code(data.dtype)
-    if data.dtype in _DT_16 and any(c.dtype != torch.float32 for c in cores):
+    if data.dtype in _DT_LOW and any(c.dtype != torch.float32 for c in cores):
         raise ValueError(f"tt_relative_error: {str(data.dtype).replace('torch.', '')} data needs float32 cores")
     ranks = [cores[0].shape[0]] + [c.shape[2] for c in cores]
     L = lib()

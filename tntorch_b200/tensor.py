@@ -71,7 +71,10 @@ class Tensor(object):
             dev = _default_device(device if device is not None else (data.device if data.is_cuda else None))
             data = data.to(dev)
             if data.dim() == 0:
-                data = data * torch.ones(1, device=dev, dtype=data.dtype)
+                if data.dtype in (torch.float8_e4m3fn, torch.float8_e5m2):  # torch has no arithmetic on float8
+                    data = data.reshape(1).clone()
+                else:
+                    data = data * torch.ones(1, device=dev, dtype=data.dtype)
             if eps is not None and ranks_tt is not None:
                 raise ValueError("Specify eps or ranks, but not both")  # tensor.py:436-438
             N = data.dim() - 1 if batch else data.dim()
