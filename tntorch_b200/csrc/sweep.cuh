@@ -32,6 +32,8 @@ constexpr bool tc_input() {
   return std::is_same<TIn, float>::value || std::is_same<TIn, __nv_bfloat16>::value || std::is_same<TIn, __half>::value ||
          is_fp8<TIn>();
 }
+// The TMA tensor-core kernels need 16-byte aligned operands; the dense input is the caller's pointer and may not be.
+inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // C (rows x r) = A (rows x n) * V (n x r) in the data precision (fp32 for 16-bit A): tensor-core kernel, streaming FFMA
 // kernel for fp32 when the shape allows, generic tiled GEMM otherwise.
@@ -105,9 +107,9 @@ inline int make_dims(int ndim, const int64_t* shape, const int32_t* rmax, SweepD
 // tensor cores with an epilogue that can write it (rcap[mu+1] % 16 == 0 and <= 48, shape[mu] % 16 == 0).  Its Gram then loads
 // K-major operands directly instead of transposing every slab in shared memory.  The writer's own input must be
 // row-major (fp32, or the bf16 / fp16 / fp8 input when the writer is step 0), and the last carry (step mu = 0's core) stays
-// row-major.
+// row-major, and 16-byte aligned when it is the caller's input (`data`; nullptr when only sizing).
 template <typename T, typename TIn = T>
-inline bool carry_kblocked(const SweepDims& d, int mu, bool allow_tc) {
+inline bool carry_kblocked(const SweepDims& d, int mu, bool allow_tc, const void* data = nullptr) {
   if (!std::is_same<T, float>::value || !allow_tc || mu < 1 || mu + 1 > d.N - 1) return false;
   const int64_t rows = d.rows[mu], n = d.shape[mu] * d.rcap[mu + 1], k = std::min<int64_t>(d.rcap[mu], n);
   const bool reader = rows >= n && rows >= std::max(TC_MIN_ROWS, PROJ_TC_MIN_ROWS) && gram_tc_kblocked_shape_ok(rows, n) &&
@@ -115,8 +117,9 @@ inline bool carry_kblocked(const SweepDims& d, int mu, bool allow_tc) {
   const int64_t wrows = d.rows[mu + 1], wn = d.shape[mu + 1] * d.rcap[mu + 2], r = d.rcap[mu + 1];
   const bool wtc = mu + 1 == d.N - 1 ? project_use_tc<TIn>(wrows, wn, r, nullptr, nullptr)
                                      : project_use_tc<T>(wrows, wn, r, nullptr, nullptr);
-  const bool writer = wrows >= wn && wn >= 32 && wtc && r % 16 == 0 && r <= 48 && d.shape[mu] % 16 == 0;
-  return reader && writer && !carry_kblocked<T, TIn>(d, mu + 1, allow_tc);
+  const bool writer = wrows >= wn && wn >= 32 && wtc && r % 16 == 0 && r <= 48 && d.shape[mu] % 16 == 0 &&
+                      (mu + 1 != d.N - 1 || data == nullptr || aligned16(data));
+  return reader && writer && !carry_kblocked<T, TIn>(d, mu + 1, allow_tc, data);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -154,7 +157,7 @@ inline int gram_small_side(const T* C, int64_t rows, int64_t n, double* G, float
   if (used_tc) *used_tc = 0;
   if (tall) {
     if constexpr (tc_input<T>())
-      if (use_tc && w.tc_ws) {
+      if (use_tc && w.tc_ws && aligned16(C)) {  // a misaligned input takes the generic Gram, whose partials are always carved
         if (used_tc)
           *used_tc = std::is_same<T, __nv_bfloat16>::value   ? 2
                      : std::is_same<T, __half>::value        ? 3
@@ -269,7 +272,9 @@ inline int eig_solve_and_rank(const double* G, const TBk* Gb, int64_t L, EigWork
   }
   for (;;) {
     ChfsiStats cs;
-    TNB_TRY(eig_run<TBk>(G, Gb, L, ew, &sc->trace, &cs, st, allow_tc, shared_gpu, k_try, tol));
+    // the eps-only solve must resolve the tail energy to 0.05 delta^2; TF32 filter products do not (on a 512 x 512 fp32
+    // Gram with eps = 1e-2 they left ~3e-6 of the energy uncaptured and moved the relative error by 3 %): CUDA cores
+    TNB_TRY(eig_run<TBk>(G, Gb, L, ew, &sc->trace, &cs, st, allow_tc && !adaptive, shared_gpu, k_try, tol));
     if (total)
       total->products += cs.products, total->fused_filters += cs.fused_filters, total->outer += cs.outer,
           total->rr_sweeps += cs.rr_sweeps;
@@ -383,15 +388,142 @@ inline StepCtx make_step_ctx(ArenaT& ar, int N, double eps, uint32_t flags, bool
   return cx;
 }
 
+// A wide step's factor (step_factors) in fp64 scratch: F = U_r diag(1/d) (rows x kcap), the split-K partials of the
+// kcap x kcap Gram of the core's rows (~4 sms kcap^2 / tiles doubles, at most n kcap^2 / 64), that Gram, the Cholesky-QR factors T and R,
+// the factorisation's scratch, and a control block (tnb_skip words: word 1 set = the rows are already orthonormal).
+// O(rows * kcap + kcap^2): nothing of the core's length n.
+struct WideWork {
+  double *F = nullptr, *partial = nullptr, *S = nullptr, *Tm = nullptr, *Rm = nullptr, *scratch = nullptr;
+  int* ctrl = nullptr;
+  int splits = 1;
+};
+template <class ArenaT>
+inline void wide_carve(ArenaT& ar, int64_t rows, int64_t n, int64_t kcap, WideWork& ww) {
+  // the Gram has a few output tiles and a long K: split it over ~4 CTAs per SM (plan_gemm stops at 64 splits, which left
+  // a 64 x 64 Gram over 2^21 columns on half the SMs), at most n / 64 of them
+  const int64_t tm = ceil_div<int64_t>(kcap, GEMM_BM), tiles = tm * (tm + 1) / 2;
+  const int sms = device_info().valid ? device_info().sm_count : 132;
+  const int64_t want = std::min<int64_t>(std::max<int64_t>(ceil_div<int64_t>(4 * (int64_t)sms, tiles), 1),
+                                         std::max<int64_t>(n / 64, 1));
+  const GemmPlan pl = plan_gemm(kcap, kcap, n, true, (int)std::min<int64_t>(want, 1024));
+  ww.splits = pl.splits;
+  ww.F = ar.template take<double>((size_t)rows * kcap);
+  ww.partial = ar.template take<double>(pl.partial_elems);
+  ww.S = ar.template take<double>((size_t)kcap * kcap);
+  ww.Tm = ar.template take<double>((size_t)kcap * kcap);
+  ww.Rm = ar.template take<double>((size_t)kcap * kcap);
+  ww.scratch = ar.template take<double>((size_t)2 * kcap * (kcap | 1));
+  ww.ctrl = ar.template take<int>(4);
+}
+
+// F[a][j] = U[a][j] / d_j and Cn[a][j] = U[a][j] d_j, d_j = max(s_j, 1e-8 s_0): F^T C has rows near unit length (at the
+// Gram's noise floor, where s_j carries no information, shorter) and Cn (F^T C) = U_r U_r^T C exactly.
+template <typename T>
+__global__ void wide_prep_kernel(const double* __restrict__ V, int ldv, int64_t rows, int rank, const double* __restrict__ w,
+                                 double* __restrict__ F, T* __restrict__ Cn) {
+  const double s0 = sqrt(w[0] > 0.0 ? w[0] : 0.0);
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < rows * rank; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t a = idx / rank;
+    const int j = (int)(idx % rank);
+    const double d = fmax(sqrt(w[j] > 0.0 ? w[j] : 0.0), 1e-8 * s0);
+    const double u = V[(size_t)a * ldv + j];
+    F[idx] = d > 0.0 ? u / d : 0.0;
+    Cn[idx] = (T)(u * d);
+  }
+}
+
+// Are the core's rows orthonormal already (S = core core^T within tol of I)?  Then every later stage of the step is
+// skipped (ctrl word 1, read by tnb_skip); otherwise they run.  One warp.
+__global__ void wide_check_kernel(const double* __restrict__ S, int rank, double tol, int* ctrl) {
+  double dev = 0.0;
+  for (int idx = threadIdx.x; idx < rank * rank; idx += blockDim.x) {
+    const int i = idx / rank, j = idx % rank;
+    dev = fmax(dev, fabs(S[idx] - (i == j ? 1.0 : 0.0)));
+  }
+  for (int o = 16; o > 0; o >>= 1) dev = fmax(dev, __shfl_xor_sync(0xffffffffu, dev, o));
+  if (threadIdx.x == 0) {
+    ctrl[0] = 0;
+    ctrl[1] = dev <= tol ? 1 : 0;
+    ctrl[2] = 0;
+  }
+}
+
+template <typename TB>
+__global__ void __launch_bounds__(1024) wide_chol_kernel(const double* __restrict__ S, int b, double* scratch, TB* __restrict__ T,
+                                                         int use_smem, TB* __restrict__ Rout, int* ctrl) {
+  extern __shared__ __align__(16) unsigned char wide_chol_smem[];
+  if (tnb_skip(ctrl, 0)) return;
+  chol_orth_device<TB>(S, b, scratch, T, ctrl + 3, use_smem, Rout, wide_chol_smem);
+}
+
+// One Cholesky-QR step in place, from the factors of chol_orth_kernel for A = core^T (A T has orthonormal columns,
+// A = (A T) R; T and R upper triangular with positive diagonals): core <- T^T core and Cn <- Cn R^T.  Each block takes
+// 32 vectors (columns of core, or rows of Cn) into shared memory, then writes the products over them.  With `fill`, a
+// core row that was exactly zero (S_jj <= 1e-30 max S: U_r's direction meets a null row space of C, or the tensor is
+// zero) has no direction to keep: it becomes a fixed pseudo-random row and its Cn column zero, which leaves Cn core as it
+// was; the next step orthonormalises it against the others.
+template <typename T, bool CORE>
+__global__ void __launch_bounds__(256) wide_apply_kernel(const double* __restrict__ M, const double* __restrict__ S, int rank,
+                                                         int64_t nvec, T* __restrict__ X, int fill, const int* ctrl) {
+  extern __shared__ __align__(16) unsigned char wide_apply_smem[];
+  if (tnb_skip(ctrl, 0)) return;
+  double* x = reinterpret_cast<double*>(wide_apply_smem);  // [rank][32]
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  double smax = 0.0;
+  if (fill)
+    for (int k = 0; k < rank; ++k) smax = fmax(smax, S[(size_t)k * rank + k]);
+  for (int64_t v0 = (int64_t)blockIdx.x * 32; v0 < nvec; v0 += (int64_t)gridDim.x * 32) {
+    __syncthreads();
+    for (int idx = threadIdx.x; idx < rank * 32; idx += blockDim.x) {
+      const int k = idx / 32, v = idx % 32;
+      const int64_t g = v0 + v;
+      x[idx] = g < nvec ? (double)(CORE ? X[(size_t)k * nvec + g] : X[(size_t)g * rank + k]) : 0.0;
+    }
+    __syncthreads();
+    const int64_t g = v0 + lane;
+    if (g < nvec)
+      for (int j = warp; j < rank; j += 8) {
+        double acc = 0.0;
+        if (CORE)
+          for (int k = 0; k <= j; ++k) acc = fma(M[(size_t)k * rank + j], x[k * 32 + lane], acc);
+        else
+          for (int k = j; k < rank; ++k) acc = fma(M[(size_t)j * rank + k], x[k * 32 + lane], acc);
+        if (fill && (S[(size_t)j * rank + j] <= 1e-30 * smax || !(smax > 0.0))) {
+          if (CORE) {
+            const uint64_t e = (uint64_t)j * nvec + g;
+            const uint32_t h = hash_u32((uint32_t)e * 2654435761U + 0x5bd1e995U) ^ hash_u32((uint32_t)(e >> 32) + 0x9e3779b9U);
+            acc = ((double)(h >> 8) + 0.5) * (2.0 / 16777216.0) - 1.0;
+          } else {
+            acc = 0.0;
+          }
+        }
+        if (CORE) X[(size_t)j * nvec + g] = (T)acc;
+        else X[(size_t)g * rank + j] = (T)acc;
+      }
+  }
+}
+
+// Rows of a wide step's core that are orthonormal to this level skip the Cholesky-QR steps (fp64 accumulation of
+// diag(1/d) U_r^T C leaves them within ~eps_64 lambda_0 / lambda_{r-1} of it, plus the storage rounding).
+template <typename T>
+constexpr double wide_orth_tol() { return std::is_same<T, double>::value ? 1e-13 : 1e-6; }
+
 // The end of a truncation step at rank `rank`, from the step's eigenpairs (w descending, V with leading dimension ldv):
 //   tall (rows >= n): core = V_r^T (rank x n);  Cn = C V_r;
-//   wide:             core = diag(1/s) U_r^T C (rank x n);  Cn = U_r diag(s).
-// fac (L x rank) is scratch; ptc_ws the tensor-core projection's workspace (project_tc_carve_bytes).  `layout` is
-// PT_ROWMAJOR unless the speculative sweep reads (PT_IN_KBLOCKED) or writes (PT_OUT_KBLOCKED, out_inner) a K-blocked carry.
+//   wide:             core = diag(1/d) U_r^T C (accumulated in fp64), Cn = U_r diag(d), d_j = max(s_j, 1e-8 s_0), then
+//                     the fp64 Gram of core's rows (split-K GEMM).  When it is within wide_orth_tol of I (a spectrum
+//                     well above the Gram's noise floor) the step ends there, decided on the device; otherwise two
+//                     Cholesky-QR steps follow (one-CTA Cholesky of the rank x rank Gram, in-place triangular updates of
+//                     core and Cn on the whole GPU, a second Gram), which make the rows orthonormal when s_r nears the
+//                     noise floor or the unfolding's rank is below the cap, where diag(1/s) U_r^T C alone is not.
+//                     Positive diagonals keep the basis; Cn core = U_r U_r^T C throughout.
+// fac (n x rank, tall steps) and ww (wide steps) are scratch; ptc_ws the tensor-core projection's workspace
+// (project_tc_carve_bytes).  `layout` is PT_ROWMAJOR unless the speculative sweep reads (PT_IN_KBLOCKED) or writes
+// (PT_OUT_KBLOCKED, out_inner) a K-blocked carry.
 template <typename T, typename TIn>
 inline int step_factors(const StepCtx& cx, const TIn* C, int64_t rows, int64_t n, int64_t rank, const double* w,
-                        const double* V, int ldv, T* fac, void* ptc_ws, size_t ptc_bytes, T* core, T* Cn,
-                        int layout = PT_ROWMAJOR, int64_t out_inner = 0) {
+                        const double* V, int ldv, T* fac, const WideWork& ww, void* ptc_ws, size_t ptc_bytes, T* core,
+                        T* Cn, int layout = PT_ROWMAJOR, int64_t out_inner = 0) {
   cudaStream_t st = cx.st;
   if (rows >= n) {
     scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(V, ldv, (int)n, (int)rank, w, core, 0, 1);
@@ -405,12 +537,35 @@ inline int step_factors(const StepCtx& cx, const TIn* C, int64_t rows, int64_t n
                                ptc_ws, ptc_bytes, st, layout, out_inner);
     return project_any<T, TIn>(C, rows, n, fac, rank, Cn, st, ptc_ws, ptc_bytes);
   }
-  scale_extract_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(V, ldv, (int)rows, (int)rank, w, fac, 1, 0);
+  wide_prep_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(V, ldv, rows, (int)rank, w, ww.F, Cn);
   TNB_LAUNCH_CHECK();
-  TNB_TRY((gemm_direct<T, TIn, T, T>(rank, n, rows, fac, rank, false, C, n, false, core, n, (T)1, nullptr, 0, (T)0,
-                                     nullptr, 0, (T)0, st)));
-  scale_extract_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(V, ldv, (int)rows, (int)rank, w, Cn, 2, 0);
-  TNB_LAUNCH_CHECK();
+  TNB_TRY((gemm_direct<double, TIn, double, T>(rank, n, rows, ww.F, rank, false, C, n, false, core, n, 1.0, nullptr, 0, 0.0,
+                                               nullptr, 0, 0.0, st)));
+  const GemmPlan pl = plan_gemm(rank, rank, n, true, ww.splits);
+  const size_t csm = (size_t)2 * rank * (rank | 1) * sizeof(double), asm_bytes = (size_t)rank * 32 * sizeof(double);
+  const bool fits = csm <= 180 * 1024;
+  static PerDeviceFlag attr_chol, attr_core, attr_cn;
+  TNB_CUDA(ensure_dyn_smem(attr_chol, wide_chol_kernel<double>, 180 * 1024));
+  TNB_CUDA(ensure_dyn_smem(attr_core, wide_apply_kernel<T, true>, 64 * 1024));
+  TNB_CUDA(ensure_dyn_smem(attr_cn, wide_apply_kernel<T, false>, 64 * 1024));
+  const int grid_core = (int)std::min<int64_t>(ceil_div<int64_t>(n, 32), 8 * usable_sms());
+  const int grid_cn = (int)std::min<int64_t>(ceil_div<int64_t>(rows, 32), 8 * usable_sms());
+  // two Cholesky-QR steps, all of them skipped on the device when the first Gram finds the rows orthonormal
+  for (int pass = 0; pass < 2; ++pass) {
+    TNB_TRY((gemm_splitk<T, T, double, double, float>(pl, rank, rank, n, core, n, true, core, n, true, ww.partial, ww.S, rank,
+                                                      1.0, nullptr, 0, 0.0, nullptr, 0, 0.0, true, (float*)nullptr, 0, st,
+                                                      pass ? ww.ctrl : nullptr, 0)));
+    if (pass == 0) {
+      wide_check_kernel<<<1, 32, 0, st>>>(ww.S, (int)rank, wide_orth_tol<T>(), ww.ctrl);
+      TNB_LAUNCH_CHECK();
+    }
+    wide_chol_kernel<double><<<1, 1024, fits ? csm : 0, st>>>(ww.S, (int)rank, ww.scratch, ww.Tm, fits ? 1 : 0, ww.Rm, ww.ctrl);
+    TNB_LAUNCH_CHECK();
+    wide_apply_kernel<T, true><<<grid_core, 256, asm_bytes, st>>>(ww.Tm, ww.S, (int)rank, n, core, pass == 0, ww.ctrl);
+    TNB_LAUNCH_CHECK();
+    wide_apply_kernel<T, false><<<grid_cn, 256, asm_bytes, st>>>(ww.Rm, ww.S, (int)rank, rows, Cn, pass == 0, ww.ctrl);
+    TNB_LAUNCH_CHECK();
+  }
   return TNB_OK;
 }
 
@@ -436,7 +591,9 @@ inline int truncate_step(ArenaT& ar, bool dry, const StepCtx& cx, const TIn* C, 
   const int64_t kcap = std::min<int64_t>(rank_cap, L);
   TNB_TRY(eig_carve<TBk>(ar, L, kcap, have_rmax, ew));
   if (ew.chfsi && std::is_same<TBk, float>::value) Gf = reinterpret_cast<float*>(ew.Gb);
-  T* fac = ar.template take<T>((size_t)L * (size_t)kcap);  // V_r or U_r/s
+  T* fac = tall ? ar.template take<T>((size_t)L * (size_t)kcap) : nullptr;  // V_r
+  WideWork ww;
+  if (!tall) wide_carve(ar, rows, n, kcap, ww);
   const size_t ptc_bytes = project_tc_carve_bytes<TIn>(cx.allow_tc, rows, n, kcap);
   void* ptc_ws = ptc_bytes ? ar.template take<char>(ptc_bytes) : nullptr;
   if (dry) return TNB_OK;
@@ -482,7 +639,7 @@ inline int truncate_step(ArenaT& ar, bool dry, const StepCtx& cx, const TIn* C, 
     fill_kernel<T><<<grid_for(rows), 256, 0, st>>>(Cn, rows, (T)0);
     TNB_LAUNCH_CHECK();
   } else {
-    TNB_TRY((step_factors<T, TIn>(cx, C, rows, n, rank, ew.w, ew.V, ew.ldv, fac, ptc_ws, ptc_bytes, core, Cn)));
+    TNB_TRY((step_factors<T, TIn>(cx, C, rows, n, rank, ew.w, ew.V, ew.ldv, fac, ww, ptc_ws, ptc_bytes, core, Cn)));
   }
   prof.mark(st);
   *rank_out = rank;
@@ -518,7 +675,8 @@ struct SpecStep {
   int* jinfo = nullptr;
   float* Gf = nullptr;
   CdWork<float> cw;
-  T* fac = nullptr;
+  T* fac = nullptr;   // tall step: V_r
+  WideWork ww;        // wide step
   void* ptc_ws = nullptr;
   size_t ptc_bytes = 0;
   int ldv = 0, b = 0, used_tc = 0;
@@ -556,7 +714,8 @@ inline void spec_step_carve(ArenaT& ar, const StepCtx& cx, int64_t rows, int64_t
     s.Gf = ar.template take<float>((size_t)L * L);
     chfsi_dev_carve<float>(ar, (int)L, s.b, s.cw);
   }
-  s.fac = ar.template take<T>((size_t)L * (size_t)s.kcap);
+  s.fac = tall ? ar.template take<T>((size_t)L * (size_t)s.kcap) : nullptr;
+  if (!tall) wide_carve(ar, rows, n, s.kcap, s.ww);
   s.ptc_bytes = project_tc_carve_bytes<TIn>(cx.allow_tc, rows, n, s.kcap);
   s.ptc_ws = s.ptc_bytes ? ar.template take<char>(s.ptc_bytes) : nullptr;
 }
@@ -632,8 +791,8 @@ inline int spec_step_rest(const StepCtx& cx, const TIn* C, int64_t rows, int64_t
   TNB_LAUNCH_CHECK();
   if (prof_on) prof.mark(st);
   const int layout = s.in_kblocked ? PT_IN_KBLOCKED : s.out_inner > 0 ? PT_OUT_KBLOCKED : PT_ROWMAJOR;
-  TNB_TRY((step_factors<T, TIn>(cx, C, rows, n, s.kcap, s.w, s.V, s.ldv, s.fac, s.ptc_ws, s.ptc_bytes, core, Cn, layout,
-                                s.out_inner)));
+  TNB_TRY((step_factors<T, TIn>(cx, C, rows, n, s.kcap, s.w, s.V, s.ldv, s.fac, s.ww, s.ptc_ws, s.ptc_bytes, core, Cn,
+                                layout, s.out_inner)));
   if (prof_on) prof.mark(st);
   return TNB_OK;
 }
@@ -782,8 +941,8 @@ inline int spec_phase1(SpecRun<T, TIn, ArenaT>& r, bool dry, const SweepDims& d,
     spec_step_carve<T, TIn>(ar, r.cx, rows, n, d.rcap[mu], r.step);
   else
     spec_step_carve<T, T>(ar, r.cx, rows, n, d.rcap[mu], r.step);
-  r.step.in_kblocked = carry_kblocked<T, TIn>(d, mu, r.cx.allow_tc);
-  r.step.out_inner = carry_kblocked<T, TIn>(d, mu - 1, r.cx.allow_tc) ? d.shape[mu - 1] : 0;
+  r.step.in_kblocked = carry_kblocked<T, TIn>(d, mu, r.cx.allow_tc, r.data);
+  r.step.out_inner = carry_kblocked<T, TIn>(d, mu - 1, r.cx.allow_tc, r.data) ? d.shape[mu - 1] : 0;
   if (ar.off > r.peak) r.peak = ar.off;
   if (dry) return TNB_OK;
   if (!ar.ok) return fail(TNB_ERR_WORKSPACE, "workspace too small (need > %zu bytes)", ar.off);
