@@ -400,6 +400,20 @@ int tnb_tt_relative_error(int dtype, const void* data, const void* const* cores,
                           const int32_t* ranks, void* workspace, size_t workspace_bytes, double* result_host,
                           void* stream);
 
+/* TT -> dense: expands the cores of one tensor train (core j: ranks[j] x shape[j] x ranks[j+1], row-major) into the
+ * caller's row-major buffer `out` of prod(shape) elements.  Stream-ordered, no host synchronisation, no allocation.
+ * core_dtype TNB_F32 or TNB_F64; out_dtype the same, or TNB_BF16 / TNB_F16 with fp32 cores (the fp32 result rounded once,
+ * to nearest even, at the store).  Any other pair returns TNB_ERR_UNSUPPORTED and sizes to 0.  ranks has ndim + 1
+ * entries with ranks[0] == ranks[ndim] == 1; 1 <= ndim <= 62.  The two half-chains meet at the bond that minimises their
+ * sizes and one product writes the result: on the tensor cores at fp32 accuracy when it has fp32 cores, 8 <= r_k <= 256,
+ * a column count that is a multiple of 8, at least 2^20 elements and a 16-byte aligned `out`, on the generic tiles
+ * otherwise.  The workspace holds the chains, their two ends and the TF32 images of those, never an image of the result.
+ * Replaces: Tensor.torch() tensor.py:1639-1687 followed by .to(dtype). */
+size_t tnb_tt_decompress_workspace_bytes(int core_dtype, int out_dtype, int ndim, const int64_t* shape,
+                                         const int32_t* ranks);
+int tnb_tt_decompress(int core_dtype, int out_dtype, const void* const* cores, int ndim, const int64_t* shape,
+                      const int32_t* ranks, void* out, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -137,11 +137,12 @@ class TTMatrix:
         self.ranks = tt.ranks_tt[1:-1]
         self.cores = [c.reshape(*c.shape[: off + 1], input_dims[k], output_dims[k], c.shape[-1]) for k, c in enumerate(tt.cores)]
 
-    def torch(self):
-        """Back to the dense 2-D (or batched 3-D) matrix (matrix.py:120-160)."""
+    def torch(self, dtype=None):
+        """Back to the dense 2-D (or batched 3-D) matrix (matrix.py:120-160); with `dtype=` the TT part is one library
+        call that writes that dtype (Tensor.torch(dtype=))."""
         d, off = self.d, 1 if self.batch else 0
         cores = [c.reshape(*c.shape[: off + 1], -1, c.shape[-1]) for c in self.cores]
-        X = Tensor(cores, batch=self.batch).torch()
+        X = Tensor(cores, batch=self.batch).torch(dtype=dtype)
         idims, odims = self.input_dims.tolist(), self.output_dims.tolist()
         lead = [X.shape[0]] if self.batch else []
         X = X.reshape(lead + [s for k in range(d) for s in (idims[k], odims[k])])

@@ -13,6 +13,7 @@
 #include "qr.cuh"
 #include "cross_kernels.cuh"
 #include "peak_tf32.cuh"
+#include "expand_tc.cuh"
 
 using namespace tnb;
 
@@ -902,6 +903,32 @@ int tnb_tt_relative_error(int dtype, const void* data, const void* const* cores,
   return tt_relative_error_impl<double, double>(ar, false, static_cast<const double*>(data),
                                         reinterpret_cast<const double* const*>(cores), ndim, shape, ranks, result_host,
                                         as_stream(stream));
+}
+
+// ------------------------------------------------------------------ TT -> dense
+size_t tnb_tt_decompress_workspace_bytes(int core_dtype, int out_dtype, int ndim, const int64_t* shape,
+                                         const int32_t* ranks) {
+  if (!decompress_pair_ok(core_dtype, out_dtype) || !shape || !ranks || decompress_check_dims(ndim, shape, ranks) != TNB_OK)
+    return 0;
+  ArenaSizer ar;
+  if (tt_decompress_dispatch(ar, true, core_dtype, out_dtype, nullptr, ndim, shape, ranks, nullptr, 0) != TNB_OK) return 0;
+  return ar.off > 256 ? ar.off : 256;  // never 0 for a supported call: 0 is the refusal
+}
+
+int tnb_tt_decompress(int core_dtype, int out_dtype, const void* const* cores, int ndim, const int64_t* shape,
+                      const int32_t* ranks, void* out, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!decompress_pair_ok(core_dtype, out_dtype))
+    return fail(TNB_ERR_UNSUPPORTED, "tnb_tt_decompress: cores %d -> output %d is not built (fp32 -> fp32 / bf16 / fp16, fp64 -> fp64)",
+                core_dtype, out_dtype);
+  if (!cores || !shape || !ranks || !out || !workspace) return fail(TNB_ERR_INVALID, "tnb_tt_decompress: null argument");
+  TNB_TRY(decompress_check_dims(ndim, shape, ranks));
+  for (int j = 0; j < ndim; ++j)
+    if (!cores[j]) return fail(TNB_ERR_INVALID, "tnb_tt_decompress: core %d is null", j);
+  TNB_TRY(require_device());
+  if (workspace_bytes < tnb_tt_decompress_workspace_bytes(core_dtype, out_dtype, ndim, shape, ranks))
+    return fail(TNB_ERR_WORKSPACE, "tnb_tt_decompress: workspace too small");
+  Arena ar(workspace, workspace_bytes);
+  return tt_decompress_dispatch(ar, false, core_dtype, out_dtype, cores, ndim, shape, ranks, out, as_stream(stream));
 }
 
 }  // extern "C"

@@ -1014,3 +1014,45 @@ def tt_relative_error(data: torch.Tensor, cores: Sequence[torch.Tensor]) -> floa
     with torch.cuda.device(data.device):
         check(L.tnb_tt_relative_error(code, _ptr(data), ptrs, N, sh, rk, _ptr(ws), ws.numel(), res, _stream()))
     return float(res[0])
+
+
+_DT_OUT = {torch.float32: _lib.TNB_F32, torch.float64: _lib.TNB_F64, torch.bfloat16: _lib.TNB_BF16, torch.float16: _lib.TNB_F16}
+
+
+def tt_decompress(cores: Sequence[torch.Tensor], dtype: Optional[torch.dtype] = None,
+                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The dense tensor of TT cores [r, I, r'] (one dtype, one CUDA device, boundary ranks 1) in one library call
+    (tnb_tt_decompress): stream-ordered, no host synchronisation.  `dtype` defaults to the cores' dtype; float32 cores
+    also decompress to bfloat16 or float16 (the float32 result rounded once).  `out`: a preallocated contiguous tensor of
+    the result's shape and dtype."""
+    cores = list(cores)
+    if not cores or any(c.dim() != 3 for c in cores):
+        raise ValueError("tt_decompress: cores must be 3-D tensors [r, I, r']")
+    c0 = cores[0]
+    _require_cuda(c0, "tt_decompress")
+    if any(c.dtype != c0.dtype or c.device != c0.device for c in cores):
+        raise ValueError("tt_decompress: cores must share one dtype and one device")
+    if any(c.requires_grad for c in cores):
+        raise ValueError("tt_decompress: cores that require grad are not supported (use Tensor.torch() without arguments)")
+    ranks = [c0.shape[0]] + [c.shape[2] for c in cores]
+    if ranks[0] != 1 or ranks[-1] != 1:
+        raise ValueError(f"tt_decompress: boundary ranks must be 1, got {ranks[0]} and {ranks[-1]}")
+    if any(a.shape[2] != b.shape[0] for a, b in zip(cores[:-1], cores[1:])):
+        raise ValueError("tt_decompress: core ranks do not match")
+    dtype = c0.dtype if dtype is None else dtype
+    shape = [c.shape[1] for c in cores]
+    if out is None:
+        out = torch.empty(shape, dtype=dtype, device=c0.device)
+    elif list(out.shape) != shape or out.dtype != dtype or out.device != c0.device or not out.is_contiguous():
+        raise ValueError(f"tt_decompress: out must be a contiguous {dtype} tensor of shape {shape} on {c0.device}")
+    code, ocode = _dtype_code(c0), _DT_OUT.get(dtype, -1)
+    cores = [c.contiguous() for c in cores]
+    N = len(cores)
+    L = lib()
+    sh, rk = i64(shape), i32(ranks)
+    wsb = L.tnb_tt_decompress_workspace_bytes(code, ocode, N, sh, rk)
+    ws = _ws(wsb, c0.device)
+    ptrs = (C.c_void_p * N)(*[c.data_ptr() for c in cores])
+    with torch.cuda.device(c0.device):
+        check(L.tnb_tt_decompress(code, ocode, ptrs, N, sh, rk, _ptr(out), _ptr(ws), wsb, _stream()))
+    return out

@@ -239,7 +239,11 @@ class Tensor(object):
         raise NotImplementedError("tensor / tensor needs cross-approximation (tn.cross)")
 
     # ------------------------------------------------------------------ decompression (tensor.py:1639-1687)
-    def torch(self):
+    def torch(self, dtype=None, out=None):
+        """The dense tensor.  With `dtype=` and/or `out=` it is written by one library call (ops.tt_decompress): float32
+        cores to float32, bfloat16 or float16, float64 cores to float64, into `out` when given."""
+        if dtype is not None or out is not None:
+            return self._decompress(dtype, out)
         if self.batch:
             return torch.stack([Tensor([c[b] for c in self.cores]).torch() for b in range(self.cores[0].shape[0])])
         if any(U is not None for U in self.Us):
@@ -261,6 +265,24 @@ class Tensor(object):
             f = f.reshape(-1, f.shape[-1])
         f = f.sum(dim=-1) if f.shape[-1] > 1 else f[..., 0]
         return f.reshape(list(self.shape))
+
+    def _decompress(self, dtype, out):
+        """torch(dtype=, out=): plain TT cores through ops.tt_decompress; Tucker factors are absorbed first, a batch is
+        one call per sample into the slices of the result."""
+        if any(U is not None for U in self.Us):
+            return self.decompress_tucker_factors()._decompress(dtype, out)
+        if any(c.dim() != (4 if self.batch else 3) for c in self.cores):
+            raise ValueError("torch(dtype=, out=) needs TT cores; CP factors decompress through torch() without arguments")
+        if self.batch:
+            B, c0 = self.cores[0].shape[0], self.cores[0]
+            if out is None:
+                out = torch.empty([B] + list(self.shape), dtype=c0.dtype if dtype is None else dtype, device=c0.device)
+            elif out.shape[0] != B or not out.is_contiguous():
+                raise ValueError(f"torch(out=): out must be contiguous with a leading batch dimension of {B}")
+            for b in range(B):
+                ops.tt_decompress([c[b] for c in self.cores], dtype=dtype, out=out[b])
+            return out
+        return ops.tt_decompress(self.cores, dtype=dtype, out=out)
 
     def numpy(self):
         return self.torch().detach().cpu().numpy()
