@@ -37,8 +37,8 @@ extern "C" {
 #define TNB_F32 0
 #define TNB_F64 1
 /* bf16, fp16 and fp8 (e4m3 and e5m2, the OCP formats without unsigned zero) dense input, accepted by tnb_ttsvd,
- * tnb_ttsvd_batch, tnb_ttsvd_host, their *_workspace_bytes queries and tnb_tt_relative_error (16-bit or 8-bit data, fp32
- * cores).  The cores, their capacity and info_host are fp32 for such input; every other entry point rejects these codes
+ * tnb_ttsvd_batch, tnb_ttsvd_host, tnb_ttsvd_stream, their *_workspace_bytes queries and tnb_tt_relative_error
+ * (16-bit or 8-bit data, fp32 cores).  The cores, their capacity and info_host are fp32 for such input; every other entry point rejects these codes
  * with TNB_ERR_INVALID. */
 #define TNB_BF16 2
 #define TNB_F16 3
@@ -127,6 +127,25 @@ int tnb_ttsvd_batch(int dtype, const void* const* data, int batch, int ndim, con
 int tnb_ttsvd_host(int dtype, const void* data_host, int ndim, const int64_t* shape, const int32_t* rmax, double eps,
                    uint32_t flags, void* device_buffer, void* workspace, size_t workspace_bytes, void* cores_dev,
                    int64_t cores_capacity, void* cores_host, int32_t* ranks_host, double* info_host, void* stream);
+
+/* A dense tensor in HOST memory (pinned or pageable, any tnb_ttsvd input code) -> its TT cores on the device, without
+ * the device ever holding the whole tensor: for tensors larger than free device memory.  Step 0 of the sweep streams the
+ * input through a ring of two device chunks of about `chunk_bytes` (0: 256 MiB), twice (the chunk Grams summed in fp64
+ * in chunk order, then the projection of each chunk into the device-resident step-0 carry); chunk c + 1 is copied while
+ * chunk c is computed.  A pageable source is staged through pinned 64 MiB pieces by the calling thread.  The later steps
+ * run exactly as in tnb_ttsvd on that carry.  `cores`, `ranks_host` and `info_host` are those of tnb_ttsvd
+ * (info_host[0] = ||T||_F: the exact step-0 Gram's trace, or, when that Gram is a tensor-core one, the sum of squares
+ * accumulated in fp64 over the chunks of the first pass), except that TNB_FLAG_PROFILE is ignored and info_host[24] =
+ * passes over the host tensor (2, or 3 when the tensor-core step-0 Gram was rejected for the exact one; 1 for a zero
+ * tensor), info_host[25] = chunks per pass.  The call returns after a stream synchronisation.
+ * Refused: ndim < 2 or a wide step 0 (prod(shape[:-1]) < shape[-1]) with TNB_ERR_UNSUPPORTED; a step-0 carry as large as
+ * the input (rank cap of the last bond >= shape[-1]) with TNB_ERR_WORKSPACE.  The sizing query returns 0 in those cases
+ * and for invalid codes; tnb_last_error() says why. */
+size_t tnb_ttsvd_stream_workspace_bytes(int dtype, int ndim, const int64_t* shape, const int32_t* rmax,
+                                        size_t chunk_bytes, uint32_t flags);
+int tnb_ttsvd_stream(int dtype, const void* data_host, int ndim, const int64_t* shape, const int32_t* rmax, double eps,
+                     uint32_t flags, size_t chunk_bytes, void* workspace, size_t workspace_bytes, void* cores,
+                     int64_t cores_capacity, int32_t* ranks_host, double* info_host, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * TT rounding of an existing tensor train.

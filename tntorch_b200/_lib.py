@@ -49,6 +49,9 @@ SIGNATURES = {
                                   C.c_size_t, C.POINTER(_vp), C.c_int64, _i32p, _f64p, _i32p, _vp]),
     "tnb_ttsvd_host": (C.c_int, [C.c_int, _vp, C.c_int, _i64p, _i32p, C.c_double, C.c_uint32, _vp, _vp, C.c_size_t,
                                  _vp, C.c_int64, _vp, _i32p, _f64p, _vp]),
+    "tnb_ttsvd_stream_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, _i64p, _i32p, C.c_size_t, C.c_uint32]),
+    "tnb_ttsvd_stream": (C.c_int, [C.c_int, _vp, C.c_int, _i64p, _i32p, C.c_double, C.c_uint32, C.c_size_t, _vp,
+                                   C.c_size_t, _vp, C.c_int64, _i32p, _f64p, _vp]),
     "tnb_tt_round_cores_capacity": (C.c_int64, [C.c_int, _i64p, _i32p, _i32p, _i64p]),
     "tnb_tt_round_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, _i64p, _i32p, _i32p]),
     "tnb_tt_round": (C.c_int, [C.c_int, C.POINTER(_vp), C.c_int, _i64p, _i32p, _i32p, C.c_double, C.c_uint32, _vp,

@@ -239,8 +239,8 @@ inline int eig_carve(ArenaT& ar, int64_t L, int64_t rcap, bool have_rmax, EigWor
 template <typename TBk>
 inline int eig_run(const double* G, const TBk* Gb_in, int64_t L, EigWork<TBk>& e, const double* d_trace,
                    ChfsiStats* stats, cudaStream_t st, bool allow_tc = false, bool shared_gpu = false, int k_try = 0,
-                   double tol = 1e-6) {
-  if (!e.chfsi) return jacobi2_eigh(G, (int)L, (int)L, e.w, e.V, e.jscratch, e.jinfo, st);
+                   double tol = 1e-6, bool fp32_solve = false) {
+  if (!e.chfsi) return jacobi2_eigh(G, (int)L, (int)L, e.w, e.V, e.jscratch, e.jinfo, st, fp32_solve, fp32_solve ? 2e-7 : 0.0);
   e.cw.use_tc = allow_tc;
   e.cw.shared_gpu = shared_gpu;
   e.cw.narrow = shared_gpu && getenv("TNB_NARROW") != nullptr;
@@ -256,10 +256,12 @@ inline int eig_run(const double* G, const TBk* Gb_in, int64_t L, EigWork<TBk>& e
 // Eigen stage + rank rule + host read-back of the step scalars (one sync, which the caller needs anyway for the rank).
 // eps-only truncation of a large Gram matrix (EigWork::adaptive) repeats the subspace solve with k = 32, 64, 128, 240
 // leading values until the tail-energy rule is decided, with a stopping rule fine enough to resolve delta^2.
+// fp32_solve: a small Gram's eigenpairs from fp32 rotations, as the speculative sweep takes them (spec_step_eig_begin).
 template <typename TBk>
 inline int eig_solve_and_rank(const double* G, const TBk* Gb, int64_t L, EigWork<TBk>& ew, SweepScalars* sc, int* h_sc,
                               int32_t rm, int batch_mode, ChfsiStats* total, int* solves, cudaStream_t st, bool allow_tc,
-                              bool shared_gpu, int used_tc = 0) {
+                              bool shared_gpu, int used_tc = 0, bool fp32_solve = false) {
+  fp32_solve = fp32_solve && !ew.chfsi;
   const SweepScalars* hs = reinterpret_cast<const SweepScalars*>(h_sc);
   const bool adaptive = ew.chfsi && ew.adaptive;
   int k_try = adaptive ? 32 : 0;
@@ -274,13 +276,13 @@ inline int eig_solve_and_rank(const double* G, const TBk* Gb, int64_t L, EigWork
     ChfsiStats cs;
     // the eps-only solve must resolve the tail energy to 0.05 delta^2; TF32 filter products do not (on a 512 x 512 fp32
     // Gram with eps = 1e-2 they left ~3e-6 of the energy uncaptured and moved the relative error by 3 %): CUDA cores
-    TNB_TRY(eig_run<TBk>(G, Gb, L, ew, &sc->trace, &cs, st, allow_tc && !adaptive, shared_gpu, k_try, tol));
+    TNB_TRY(eig_run<TBk>(G, Gb, L, ew, &sc->trace, &cs, st, allow_tc && !adaptive, shared_gpu, k_try, tol, fp32_solve));
     if (total)
       total->products += cs.products, total->fused_filters += cs.fused_filters, total->outer += cs.outer,
           total->rr_sweeps += cs.rr_sweeps;
     if (solves) *solves += 1;
     rank_rule_kernel<<<1, 32, 0, st>>>(ew.w, (int)L, ew.chfsi ? ew.k_run : (int)L, rm, ew.chfsi ? 1 : 0, batch_mode, sc,
-                                       gram_noise(used_tc), ew.chfsi ? ew.b_run : (int)L);
+                                       gram_noise(used_tc, fp32_solve), ew.chfsi ? ew.b_run : (int)L);
     TNB_LAUNCH_CHECK();
     TNB_CUDA(cudaMemcpyAsync(h_sc, sc, sizeof(SweepScalars), cudaMemcpyDeviceToHost, st));
     TNB_CUDA(cudaStreamSynchronize(st));
@@ -309,6 +311,7 @@ struct SweepInfo {
   int kblocked_steps = 0;  // steps whose Gram and projection read a K-blocked carry (carry_kblocked)
   int speculative = 0;  // 1: the sync-free sweep was accepted (one host synchronisation in total)
   int spec_flags = 0;   // why a speculative sweep was repeated on the host-driven path (spec_check_kernel bits)
+  int stream_passes = 0, stream_chunks = 0;  // tnb_ttsvd_stream: passes over the host tensor, chunks per pass
   // TNB_FLAG_PROFILE: CUDA-event timings (ms) on the launching stream, per step (t = 0 is the first Gram)
   int nsteps = 0;
   double gram_ms[8] = {0}, eig_ms[8] = {0}, factor_ms[8] = {0};
@@ -800,11 +803,24 @@ inline int spec_step_rest(const StepCtx& cx, const TIn* C, int64_t rows, int64_t
 // ---------------------------------------------------------------------------------------------
 // Dense TT-SVD
 // ---------------------------------------------------------------------------------------------
-// The two ping-pong carries, sized by the rank caps: step t writes carry[t & 1] (rows[mu] x rcap[mu]).
+// The carry step 0 wrote when it ran outside the sweep (the streamed step 0 of tnb_ttsvd_stream): C holds
+// rows[N-1] x rank elements, K-blocked for step 1 (carry_kblocked(d, N - 2)) or row-major, in memory of its own (never one
+// of the ping-pong pair, so that a host-driven repeat of the sweep can start from it again); sc: step 0's device scalars
+// (norm2, delta2), copied into the sweep's own.
+template <typename T>
+struct Carry0 {
+  T* C = nullptr;
+  int64_t rank = 0;
+  bool kblocked = false;
+  const SweepScalars* sc = nullptr;
+};
+
+// The two ping-pong carries, sized by the rank caps: step t writes carry[t & 1] (rows[mu] x rcap[mu]); steps before t0
+// write elsewhere.
 template <typename T, class ArenaT>
-inline void carve_carries(ArenaT& ar, const SweepDims& d, T* carry[2]) {
+inline void carve_carries(ArenaT& ar, const SweepDims& d, T* carry[2], int t0 = 0) {
   size_t elems[2] = {0, 0};
-  for (int mu = d.N - 1, t = 0; mu >= 1; --mu, ++t) {
+  for (int mu = d.N - 1 - t0, t = t0; mu >= 1; --mu, ++t) {
     const size_t e = (size_t)d.rows[mu] * (size_t)d.rcap[mu];
     if (e > elems[t & 1]) elems[t & 1] = e;
   }
@@ -812,15 +828,47 @@ inline void carve_carries(ArenaT& ar, const SweepDims& d, T* carry[2]) {
   carry[1] = ar.template take<T>(elems[1]);
 }
 
-// T: carries and cores; TIn: the dense input (T, or bf16 / fp16 / fp8 with T = float), read by step 0 only.
+// A K-blocked carry (rows' x n', gram_tc.cuh) rewritten row-major in place, one group of 8 rows (8 n' contiguous elements)
+// per block through shared memory: what the host-driven sweep reads when it repeats a speculative one from a step-0 carry
+// that was written K-blocked.
+constexpr int UNBLOCK_MAX_SMEM = 192 * 1024;
+__global__ void __launch_bounds__(256) unblock_carry_kernel(float* __restrict__ M, int64_t groups, int64_t n) {
+  extern __shared__ __align__(16) float unblock_smem[];
+  for (int64_t g = blockIdx.x; g < groups; g += gridDim.x) {
+    float* p = M + (size_t)g * 8 * n;
+    __syncthreads();
+    for (int64_t i = threadIdx.x; i < 8 * n; i += blockDim.x) unblock_smem[i] = p[i];
+    __syncthreads();
+    for (int64_t i = threadIdx.x; i < 8 * n; i += blockDim.x) {
+      const int64_t k = i / n, c = i % n;
+      p[i] = unblock_smem[((c / 8 * 2 + k / 4) * 8 + c % 8) * 4 + k % 4];
+    }
+  }
+}
+
+// T: carries and cores; TIn: the dense input (T, or bf16 / fp16 / fp8 with T = float), read by step 0 only.  With c0 the
+// sweep starts at step 1 from that step-0 carry (data unused).
 template <typename T, typename TIn, class ArenaT>
 inline int ttsvd_sync_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d, const int32_t* rmax, double eps,
                            uint32_t flags, T* cores, int32_t* ranks_host, SweepInfo* info, cudaStream_t st,
-                           bool exact_gram = false) {
+                           bool exact_gram = false, const Carry0<T>* c0 = nullptr) {
   const int N = d.N;
   StepCtx cx = make_step_ctx(ar, N, eps, flags, !(flags & TNB_FLAG_NO_TENSORCORE) && (dry || tc_path_available()), info,
                              st, false);
   cx.exact_gram = exact_gram;
+  if (c0 && !dry) {
+    TNB_CUDA(cudaMemcpyAsync(cx.sc, c0->sc, sizeof(SweepScalars), cudaMemcpyDeviceToDevice, st));
+    if (c0->kblocked) {  // this path reads row-major carries
+      if constexpr (std::is_same<T, float>::value) {
+        const int64_t n = d.shape[N - 2] * c0->rank, groups = d.rows[N - 1] / d.shape[N - 2] / 8;
+        static PerDeviceFlag attr;
+        TNB_CUDA(ensure_dyn_smem(attr, unblock_carry_kernel, UNBLOCK_MAX_SMEM));
+        unblock_carry_kernel<<<(unsigned)std::min<int64_t>(groups, 8 * usable_sms()), 256, 8 * n * sizeof(float), st>>>(
+            c0->C, groups, n);
+        TNB_LAUNCH_CHECK();
+      }
+    }
+  }
   Prof& prof = Prof::get();
   prof.on = !dry && (flags & TNB_FLAG_PROFILE);
   prof.used = 0;
@@ -843,12 +891,13 @@ inline int ttsvd_sync_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDim
     }
     return TNB_OK;
   }
+  const int t0 = c0 ? 1 : 0;
   T* carry[2];
-  carve_carries(ar, d, carry);
-  const T* C = nullptr;  // the carry step t > 0 reads; step 0 reads data
-  int64_t r_next = 1;
+  carve_carries(ar, d, carry, t0);
+  const T* C = c0 ? c0->C : nullptr;  // the carry step t > 0 reads; step 0 reads data
+  int64_t r_next = c0 ? c0->rank : 1;
   size_t peak = ar.off;
-  for (int mu = N - 1, t = 0; mu >= 1; --mu, ++t) {
+  for (int mu = N - 1 - t0, t = t0; mu >= 1; --mu, ++t) {
     const int64_t rows = d.rows[mu];
     const int64_t n = dry ? d.shape[mu] * d.rcap[mu + 1] : d.shape[mu] * r_next;
     const bool have_rmax = rmax && rmax[mu - 1] > 0;
@@ -916,17 +965,19 @@ struct SpecRun {
 
 template <typename T, typename TIn, class ArenaT>
 inline int spec_begin(SpecRun<T, TIn, ArenaT>& r, ArenaT& ar, bool dry, const TIn* data, const SweepDims& d, double eps,
-                      uint32_t flags, T* cores, SweepInfo* info, cudaStream_t st, SpecHostBack* hb) {
+                      uint32_t flags, T* cores, SweepInfo* info, cudaStream_t st, SpecHostBack* hb,
+                      const Carry0<T>* c0 = nullptr) {
   r.ar = &ar;
   r.cx = make_step_ctx(ar, d.N, eps, flags, !(flags & TNB_FLAG_NO_TENSORCORE) && (dry || tc_path_available()), info, st,
                        true);
-  carve_carries(ar, d, r.carry);
+  carve_carries(ar, d, r.carry, c0 ? 1 : 0);
   r.data = data;
-  r.C = nullptr;
+  r.C = c0 ? c0->C : nullptr;
   r.cores = cores;
   r.peak = ar.off;
   r.hb = hb;
   if (!dry) TNB_CUDA(cudaMemsetAsync(r.cx.d_flags, 0, 4 * sizeof(int), st));
+  if (!dry && c0) TNB_CUDA(cudaMemcpyAsync(r.cx.sc, c0->sc, sizeof(SweepScalars), cudaMemcpyDeviceToDevice, st));
   return TNB_OK;
 }
 
@@ -970,11 +1021,11 @@ inline int spec_phase2b(SpecRun<T, TIn, ArenaT>& r, bool dry, const SweepDims& d
 // run's eigen start (phase 2a), then the subspace-solver stages interleaved run by run, then every run's rank rule and
 // projection (phase 2b).  Interleaving the stages makes the resident filter kernels of the streams run one after the
 // other (cheb_filter.cuh), so one run's Rayleigh-Ritz step is in flight while another run's filter runs.  With dry it
-// only sizes the step scratch.
+// only sizes the step scratch.  t0 = 1: step 0 ran already (Carry0).
 template <typename T, typename TIn, class ArenaT>
 inline int spec_enqueue(SpecRun<T, TIn, ArenaT>* runs, int g, bool dry, const SweepDims& d, const int32_t* rmax,
-                        bool prof_on) {
-  for (int mu = d.N - 1, t = 0; mu >= 1; --mu, ++t) {
+                        bool prof_on, int t0 = 0) {
+  for (int mu = d.N - 1 - t0, t = t0; mu >= 1; --mu, ++t) {
     for (int s = 0; s < g; ++s) TNB_TRY(spec_phase1(runs[s], dry, d, mu, t, prof_on));
     if (!dry) {
       for (int s = 0; s < g; ++s) TNB_TRY(spec_step_eig_begin<T>(runs[s].cx, runs[s].step));
@@ -1016,7 +1067,7 @@ inline int spec_collect(const SpecHostBack* hb, const SweepDims& d, int32_t* ran
 template <typename T, typename TIn, class ArenaT>
 inline int ttsvd_spec_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d, const int32_t* rmax, double eps,
                            uint32_t flags, T* cores, int32_t* ranks_host, SweepInfo* info, cudaStream_t st,
-                           int* spec_flags) {
+                           int* spec_flags, const Carry0<T>* c0 = nullptr) {
   Prof& prof = Prof::get();
   prof.on = !dry && (flags & TNB_FLAG_PROFILE);
   prof.used = 0;
@@ -1027,8 +1078,8 @@ inline int ttsvd_spec_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDim
     if (!hb) return fail(TNB_ERR_CUDA, "pinned scratch allocation failed");
   }
   SpecRun<T, TIn, ArenaT> r;
-  TNB_TRY(spec_begin(r, ar, dry, data, d, eps, flags, cores, info, st, hb));
-  const int rc = spec_enqueue(&r, 1, dry, d, rmax, prof_on);
+  TNB_TRY(spec_begin(r, ar, dry, data, d, eps, flags, cores, info, st, hb, c0));
+  const int rc = spec_enqueue(&r, 1, dry, d, rmax, prof_on, c0 ? 1 : 0);
   if (rc != TNB_OK) {
     if (!dry) cudaStreamSynchronize(st);  // part of the sweep is enqueued: drain it before the host-driven path
     prof.on = false;
@@ -1046,12 +1097,15 @@ inline int ttsvd_spec_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDim
 }
 
 // Dispatcher: speculative sweep when a rank cap decides every bond, host-driven sweep otherwise and as the fallback.
+// With c0 the sweep starts at step 1 from that step-0 carry; it is speculative only if step 0 kept its rank cap.
 template <typename T, typename TIn, class ArenaT>
 inline int ttsvd_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d, const int32_t* rmax, double eps,
-                      uint32_t flags, T* cores, int32_t* ranks_host, SweepInfo* info, cudaStream_t st) {
+                      uint32_t flags, T* cores, int32_t* ranks_host, SweepInfo* info, cudaStream_t st,
+                      const Carry0<T>* c0 = nullptr) {
   const bool allow_tc = !(flags & TNB_FLAG_NO_TENSORCORE) && (dry || tc_path_available());
   // the sizing pass cannot ask the device what it supports: size for both paths
-  const bool spec = dry ? (d.N >= 2 && rmax != nullptr) : spec_eligible<T>(d, rmax, eps, flags, allow_tc);
+  const bool spec = dry ? (d.N >= 2 && rmax != nullptr)
+                        : spec_eligible<T>(d, rmax, eps, flags, allow_tc) && (!c0 || c0->rank == d.rcap[d.N - 1]);
   const size_t base = ar.off;
   size_t need_spec = 0;
   if (spec) {
@@ -1059,7 +1113,7 @@ inline int ttsvd_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d,
       bool all_caps = true;
       for (int mu = 1; mu < d.N; ++mu) all_caps = all_caps && rmax[mu - 1] > 0;
       if (all_caps) {
-        const int rc = ttsvd_spec_impl<T, TIn>(ar, true, data, d, rmax, eps, flags, cores, ranks_host, info, st, nullptr);
+        const int rc = ttsvd_spec_impl<T, TIn>(ar, true, data, d, rmax, eps, flags, cores, ranks_host, info, st, nullptr, c0);
         if (rc == TNB_OK) need_spec = ar.off - base;
         ar.off = base;
       }
@@ -1067,7 +1121,7 @@ inline int ttsvd_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d,
       int sflags = 0;
       SweepInfo saved;
       if (info) saved = *info;
-      const int rc = ttsvd_spec_impl<T, TIn>(ar, false, data, d, rmax, eps, flags, cores, ranks_host, info, st, &sflags);
+      const int rc = ttsvd_spec_impl<T, TIn>(ar, false, data, d, rmax, eps, flags, cores, ranks_host, info, st, &sflags, c0);
       if (rc == TNB_OK && sflags == 0) {
         if (info) info->speculative = 1;
         return TNB_OK;
@@ -1078,12 +1132,325 @@ inline int ttsvd_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d,
       if (info) { *info = saved; info->spec_flags = sflags; }
       ar.off = base;
       ar.ok = true;
-      return ttsvd_sync_impl<T, TIn>(ar, false, data, d, rmax, eps, flags, cores, ranks_host, info, st, (sflags & 1) != 0);
+      return ttsvd_sync_impl<T, TIn>(ar, false, data, d, rmax, eps, flags, cores, ranks_host, info, st, (sflags & 1) != 0,
+                                     c0);
     }
   }
-  const int rc = ttsvd_sync_impl<T, TIn>(ar, dry, data, d, rmax, eps, flags, cores, ranks_host, info, st);
+  const int rc = ttsvd_sync_impl<T, TIn>(ar, dry, data, d, rmax, eps, flags, cores, ranks_host, info, st, false, c0);
   if (dry && rc == TNB_OK && need_spec > ar.off - base) ar.off = base + need_spec;
   return rc;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Dense TT-SVD of a tensor in host memory (tnb_ttsvd_stream).  Only step 0 reads the input: C = T viewed
+// (rows x I_{N-1}), and a row block of C is a contiguous byte range of the host tensor.  So step 0 streams C through the
+// device in chunks of whole row blocks, twice: pass 1 sums the chunk Grams into one fp64 G (in chunk order), the eigen
+// stage and rank rule run on G as in truncate_step, and pass 2 projects each chunk into its row range of the step-0
+// carry.  A TF32 Gram that the accept rule rejects costs one more pass 1 with the exact Gram.  Steps 1..N-1 then run
+// through ttsvd_impl from that carry, which stays in memory of its own.  The device never holds more of the input than
+// the chunk ring.
+// ---------------------------------------------------------------------------------------------
+constexpr size_t STREAM_DEFAULT_CHUNK = (size_t)256 << 20;
+constexpr size_t STREAM_PIECE = (size_t)64 << 20;  // staging piece of a pageable source
+
+// Chunks of whole row blocks: `unit` rows = lcm(16, the narrow Gram's fold (1, 2 or 4), 8 inner when the carry is written
+// K-blocked: inner % 16 == 0), so every chunk keeps the full tensor's Gram kernel and the carry's 16-byte alignment; at
+// least PROJ_TC_MIN_ROWS rows when the projection runs on the tensor cores, and never fewer rows than columns (a chunk's
+// Gram is the n x n one).  A last piece shorter than that joins the chunk before it.
+struct ChunkPlan {
+  int64_t unit = 16, min_rows = 1, chunk_rows = 0, nchunks = 0, last_rows = 0;
+  int64_t max_rows() const { return std::max(chunk_rows, last_rows); }
+  int64_t rows_of(int64_t c) const { return c + 1 == nchunks ? last_rows : chunk_rows; }
+};
+inline ChunkPlan make_chunk_plan(int64_t rows, int64_t n, size_t row_bytes, size_t chunk_bytes, bool proj_tc,
+                                 int64_t kb_inner) {
+  ChunkPlan p;
+  p.unit = kb_inner > 0 ? 8 * kb_inner : 16;
+  p.min_rows = std::max<int64_t>(proj_tc ? PROJ_TC_MIN_ROWS : 1, n);
+  if (chunk_bytes == 0) chunk_bytes = STREAM_DEFAULT_CHUNK;
+  const int64_t want = (int64_t)(chunk_bytes / row_bytes) / p.unit * p.unit;
+  p.chunk_rows = std::max(want, ceil_div<int64_t>(p.min_rows, p.unit) * p.unit);
+  if (p.chunk_rows >= rows) {
+    p.chunk_rows = p.last_rows = rows;
+    p.nchunks = 1;
+    return p;
+  }
+  p.nchunks = ceil_div<int64_t>(rows, p.chunk_rows);
+  p.last_rows = rows - (p.nchunks - 1) * p.chunk_rows;
+  if (p.last_rows < p.min_rows) {
+    --p.nchunks;
+    p.last_rows += p.chunk_rows;
+  }
+  return p;
+}
+
+// The copy side of the chunk ring, one per device: a copy stream, its events and (for a pageable source) two pinned
+// staging pieces.  One streamed decomposition at a time per device uses it.
+struct StreamRing {
+  cudaStream_t copy = nullptr;
+  cudaEvent_t start = nullptr, copied[2] = {}, freed[2] = {}, piece[2] = {};
+  void* pinned[2] = {nullptr, nullptr};
+  std::mutex mu;
+  int ensure(bool staging) {
+    if (!copy) {
+      TNB_CUDA(cudaStreamCreateWithFlags(&copy, cudaStreamNonBlocking));
+      cudaEvent_t* evs[7] = {&start, &copied[0], &copied[1], &freed[0], &freed[1], &piece[0], &piece[1]};
+      for (cudaEvent_t* e : evs) TNB_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    }
+    for (int i = 0; i < 2 && staging; ++i)
+      if (!pinned[i]) TNB_CUDA(cudaHostAlloc(&pinned[i], STREAM_PIECE, cudaHostAllocDefault));
+    return TNB_OK;
+  }
+  static StreamRing& get() {
+    static StreamRing rings[TNB_MAX_DEVICES];
+    return rings[current_device_index()];
+  }
+};
+
+// One pass over the host tensor: chunk c lands in buf[c & 1] on the copy stream while chunk c - 1 is computed on st
+// (events order the two: a buffer is refilled after the kernels that read it).  A pinned source is one DMA per chunk; a
+// pageable one is copied by this thread into the pinned pieces in turn, each piece's DMA overlapping the next memcpy.
+// compute(c, X, first_row, rows) enqueues the chunk's kernels on st.
+template <typename TIn, class F>
+inline int stream_pass(StreamRing& ring, const char* host, bool pinned_src, size_t row_bytes, const ChunkPlan& p,
+                       TIn* const buf[2], cudaStream_t st, F&& compute) {
+  TNB_CUDA(cudaEventRecord(ring.start, st));
+  TNB_CUDA(cudaStreamWaitEvent(ring.copy, ring.start, 0));
+  int piece = 0;
+  for (int64_t c = 0; c < p.nchunks; ++c) {
+    const int b = (int)(c & 1);
+    char* dst = reinterpret_cast<char*>(buf[b]);
+    const size_t off = (size_t)(c * p.chunk_rows) * row_bytes, bytes = (size_t)p.rows_of(c) * row_bytes;
+    if (c >= 2) TNB_CUDA(cudaStreamWaitEvent(ring.copy, ring.freed[b], 0));
+    if (pinned_src) {
+      TNB_CUDA(cudaMemcpyAsync(dst, host + off, bytes, cudaMemcpyHostToDevice, ring.copy));
+    } else {
+      for (size_t q = 0; q < bytes; q += STREAM_PIECE, ++piece) {
+        const int s = piece & 1;
+        const size_t nb = std::min(STREAM_PIECE, bytes - q);
+        TNB_CUDA(cudaEventSynchronize(ring.piece[s]));  // the DMA out of this piece has finished
+        std::memcpy(ring.pinned[s], host + off + q, nb);
+        TNB_CUDA(cudaMemcpyAsync(dst + q, ring.pinned[s], nb, cudaMemcpyHostToDevice, ring.copy));
+        TNB_CUDA(cudaEventRecord(ring.piece[s], ring.copy));
+      }
+    }
+    TNB_CUDA(cudaEventRecord(ring.copied[b], ring.copy));
+    TNB_CUDA(cudaStreamWaitEvent(st, ring.copied[b], 0));
+    TNB_TRY(compute(c, reinterpret_cast<const TIn*>(dst), c * p.chunk_rows, p.rows_of(c)));
+    TNB_CUDA(cudaEventRecord(ring.freed[b], st));
+  }
+  return TNB_OK;
+}
+
+__global__ void accumulate_kernel(double* __restrict__ G, const double* __restrict__ Gc, int64_t n) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) G[i] += Gc[i];
+}
+
+// ||T||_F^2 in fp64 over the chunks of pass 1, in a fixed order, when step 0 takes a tensor-core Gram: its trace is
+// shrunk by operand truncation or fp32 accumulation (~7e-4 for TF32 on randn), which ||T||^2 - ||core_0||^2
+// (ops.tt_relative_error_from_norm) cannot afford; an exact-product Gram's trace is the norm already.  part[b] = block
+// b's sum over the chunk (64 blocks read a chunk far faster than it arrives); part[SUMSQ_BLOCKS] accumulates the chunks.
+constexpr int SUMSQ_BLOCKS = 64;
+template <typename TIn>
+__global__ void __launch_bounds__(512) sumsq_kernel(const TIn* __restrict__ X, int64_t n, double* __restrict__ part) {
+  __shared__ double red[32];
+  double s = 0.0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const double v = gemm_ld<double>(X[i]);
+    s = fma(v, v, s);
+  }
+  s = block_reduce_sum(s, red);
+  if (threadIdx.x == 0) part[blockIdx.x] = s;
+}
+__global__ void sumsq_add_kernel(double* part, int first) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  double s = first ? 0.0 : part[SUMSQ_BLOCKS];
+  for (int b = 0; b < SUMSQ_BLOCKS; ++b) s += part[b];
+  part[SUMSQ_BLOCKS] = s;
+}
+// step 0's ||T||^2 (and the eps budget on it) from the exact sum instead of the Gram's trace
+__global__ void set_norm2_kernel(SweepScalars* sc, const double* norm2, double eps_scaled) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  sc->norm2 = *norm2;
+  sc->delta2 = eps_scaled * *norm2;
+}
+
+// true for page-locked host memory, false for pageable; device or managed memory is not a host tensor
+inline int host_memory_kind(const void* p, bool* pinned) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    cudaGetLastError();
+    *pinned = false;
+    return TNB_OK;
+  }
+  if (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged)
+    return fail(TNB_ERR_INVALID, "ttsvd_stream: data_host is device memory (decompose it with tnb_ttsvd)");
+  *pinned = a.type == cudaMemoryTypeHost;
+  return TNB_OK;
+}
+
+// *ring_bytes: the chunk ring's share of the workspace (sizing pass)
+template <typename T, typename TIn, class ArenaT>
+inline int ttsvd_stream_impl(ArenaT& ar, bool dry, const TIn* host, const SweepDims& d, const int32_t* rmax, double eps,
+                             uint32_t flags, size_t chunk_bytes, T* cores, int32_t* ranks_host, SweepInfo* info,
+                             cudaStream_t st, size_t* ring_bytes = nullptr) {
+  const int N = d.N;
+  if (N < 2) return fail(TNB_ERR_UNSUPPORTED, "ttsvd_stream: a tensor of %d mode(s) has no step to stream", N);
+  const int mu = N - 1;
+  const int64_t rows = d.rows[mu], n = d.shape[mu], kcap = d.rcap[mu];
+  if (rows < n)
+    return fail(TNB_ERR_UNSUPPORTED, "ttsvd_stream: step 0 is wide (%lld rows < %lld columns) and is not streamed",
+                (long long)rows, (long long)n);
+  if (kcap >= n)
+    return fail(TNB_ERR_WORKSPACE,
+                "ttsvd_stream: the step-0 carry (rank %lld of %lld columns) holds as many elements as the input, so it "
+                "cannot fit where the input does not; decompose on the device or lower the last rank cap",
+                (long long)kcap, (long long)n);
+  flags &= ~TNB_FLAG_PROFILE;
+  const bool allow_tc = !(flags & TNB_FLAG_NO_TENSORCORE) && (dry || tc_path_available());
+  StepCtx cx = make_step_ctx(ar, N, eps, flags, allow_tc, info, st, false);
+  const bool have_rmax = rmax && rmax[mu - 1] > 0;
+  // step 0's kernels, chosen from the full shape as truncate_step / gram_carve / project_any choose them
+  const bool tc_gram = allow_tc && (dry || cx.eps_scaled2 < 1e-20 || cx.eps_scaled2 >= 1e-4) && rows >= TC_MIN_ROWS &&
+                       gram_tc_input_ok<TIn>(rows, n);
+  const size_t ptc_bytes = project_tc_carve_bytes<TIn>(allow_tc, rows, n, kcap);
+  const int64_t inner = d.shape[N - 2];
+  const bool kb_ok = carry_kblocked<T, TIn>(d, N - 2, allow_tc) && 8 * inner * kcap * sizeof(float) <= UNBLOCK_MAX_SMEM;
+  const ChunkPlan plan = make_chunk_plan(rows, n, (size_t)n * sizeof(TIn), chunk_bytes, ptc_bytes > 0, kb_ok ? inner : 0);
+  T* carry0 = ar.template take<T>((size_t)rows * kcap);  // outside the ping-pong pair of the sweep that follows
+  const size_t mark = ar.off;
+  TIn* buf[2] = {ar.template take<TIn>((size_t)plan.max_rows() * n),
+                 plan.nchunks > 1 ? ar.template take<TIn>((size_t)plan.max_rows() * n) : nullptr};
+  if (ring_bytes) *ring_bytes = ar.off - mark;
+  GramWork gw;
+  for (int64_t r : {plan.chunk_rows, plan.last_rows}) {
+    gw.partial_elems = std::max(gw.partial_elems, plan_gemm(n, n, r, true).partial_elems);
+    if (tc_gram) gw.tc_bytes = std::max(gw.tc_bytes, gram_tc_input_workspace_bytes<TIn>(r, n));
+  }
+  gw.partial = ar.template take<double>(gw.partial_elems);
+  gw.tc_ws = tc_gram ? ar.template take<char>(gw.tc_bytes) : nullptr;
+  double* G = ar.template take<double>((size_t)n * n);
+  double* Gc = plan.nchunks > 1 ? ar.template take<double>((size_t)n * n) : nullptr;
+  EigWork<T> ew;
+  TNB_TRY(eig_carve<T>(ar, n, kcap, have_rmax, ew));
+  float* Gf = ew.chfsi && std::is_same<T, float>::value ? reinterpret_cast<float*>(ew.Gb) : nullptr;
+  T* fac = ar.template take<T>((size_t)n * kcap);
+  void* ptc_ws = ptc_bytes ? ar.template take<char>(ptc_bytes) : nullptr;
+  double* sq = tc_gram ? ar.template take<double>(SUMSQ_BLOCKS + 1) : nullptr;
+  const size_t peak = ar.off;
+  Carry0<T> c0;
+  c0.C = carry0;
+  c0.rank = kcap;
+  c0.sc = cx.sc;
+  if (!dry) {
+    if (!ar.ok) return fail(TNB_ERR_WORKSPACE, "workspace too small (need > %zu bytes)", ar.off);
+    bool pinned_src = false;
+    TNB_TRY(host_memory_kind(host, &pinned_src));
+    cx.h_sc = static_cast<int*>(pinned_scratch(sizeof(SweepScalars)));
+    if (!cx.h_sc) return fail(TNB_ERR_CUDA, "pinned scratch allocation failed");
+    StreamRing& ring = StreamRing::get();
+    std::lock_guard<std::mutex> lk(ring.mu);
+    TNB_TRY(ring.ensure(!pinned_src));
+    struct Drain {  // no DMA may still read the caller's memory or the staging pieces when this returns
+      cudaStream_t s;
+      ~Drain() { cudaStreamSynchronize(s); }
+    } drain{ring.copy};
+    const char* src = reinterpret_cast<const char*>(host);
+    const size_t row_bytes = (size_t)n * sizeof(TIn);
+    int used_tc = 0, passes = 0;
+    auto gram_pass = [&](bool use_tc) -> int {
+      const bool first_pass = ++passes == 1;
+      TNB_TRY(stream_pass<TIn>(ring, src, pinned_src, row_bytes, plan, buf, st,
+                               [&](int64_t c, const TIn* X, int64_t, int64_t rc) -> int {
+                                 if (first_pass && sq) {
+                                   sumsq_kernel<TIn><<<SUMSQ_BLOCKS, 512, 0, st>>>(X, rc * n, sq);
+                                   TNB_LAUNCH_CHECK();
+                                   sumsq_add_kernel<<<1, 32, 0, st>>>(sq, c == 0 ? 1 : 0);
+                                   TNB_LAUNCH_CHECK();
+                                 }
+                                 TNB_TRY(gram_small_side<TIn>(X, rc, n, c == 0 ? G : Gc, nullptr, gw, use_tc, &used_tc, st));
+                                 if (c > 0) {
+                                   accumulate_kernel<<<grid_for(n * n), 256, 0, st>>>(G, Gc, n * n);
+                                   TNB_LAUNCH_CHECK();
+                                 }
+                                 return TNB_OK;
+                               }));
+      if (Gf) {
+        convert_kernel<double, float><<<grid_for(n * n), 256, 0, st>>>(G, Gf, n * n);
+        TNB_LAUNCH_CHECK();
+      }
+      trace_kernel<<<1, 256, 0, st>>>(G, (int)n, (int)n, cx.sc, 1, cx.eps_scaled2);
+      TNB_LAUNCH_CHECK();
+      if (sq) {
+        set_norm2_kernel<<<1, 32, 0, st>>>(cx.sc, sq + SUMSQ_BLOCKS, cx.eps_scaled2);
+        TNB_LAUNCH_CHECK();
+      }
+      return TNB_OK;
+    };
+    const int batch_mode = (flags & TNB_FLAG_BATCH_MODE) ? 1 : 0;
+    const int32_t rm = have_rmax ? rmax[mu - 1] : 0;
+    const bool spec_tail = spec_eligible<T>(d, rmax, eps, flags, allow_tc);
+    // the eigenpairs come from fp32 rotations where the speculative device sweep takes them so (spec_step_eig_begin)
+    const bool fp32_solve = spec_tail && std::is_same<T, float>::value && jacobi2_ok((int)n, true);
+    ChfsiStats cs;
+    int solves = 0;
+    TNB_TRY(gram_pass(tc_gram));
+    TNB_TRY(eig_solve_and_rank<T>(G, reinterpret_cast<const T*>(Gf), n, ew, cx.sc, cx.h_sc, rm, batch_mode, &cs, &solves,
+                                  st, allow_tc, false, used_tc, fp32_solve));
+    const SweepScalars* hs = reinterpret_cast<const SweepScalars*>(cx.h_sc);
+    if (hs->tf32_reject) {  // too steep a spectrum for the tensor-core Gram or the fp32 solve: exact Gram, fp64 rotations
+      if (used_tc) TNB_TRY(gram_pass(false));
+      used_tc = 0;
+      TNB_TRY(eig_solve_and_rank<T>(G, reinterpret_cast<const T*>(Gf), n, ew, cx.sc, cx.h_sc, rm, batch_mode, &cs, &solves,
+                                    st, allow_tc, false, 0));
+    }
+    if (info) {
+      info->tc_grams += used_tc ? 1 : 0;
+      info->eig_solves += solves, info->chfsi_products += cs.products, info->fused_filters += cs.fused_filters;
+      info->rr_sweeps += cs.rr_sweeps, info->rr_solves += cs.outer;
+      info->norm = std::sqrt(hs->norm2 > 0 ? hs->norm2 : 0.0);
+    }
+    int64_t rank = std::min<int64_t>(hs->rank, kcap);
+    T* core = cores + d.slot[mu];
+    if (hs->zero_flag) {  // round.py:137-145: rank-1 zero factors
+      rank = 1;
+      fill_kernel<T><<<grid_for(n), 256, 0, st>>>(core, n, (T)0);
+      TNB_LAUNCH_CHECK();
+      fill_kernel<T><<<grid_for(rows), 256, 0, st>>>(carry0, rows, (T)0);
+      TNB_LAUNCH_CHECK();
+    } else {
+      c0.kblocked = kb_ok && spec_tail && rank == kcap;
+      scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(ew.V, ew.ldv, (int)n, (int)rank, ew.w, core, 0, 1);
+      TNB_LAUNCH_CHECK();
+      scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(ew.V, ew.ldv, (int)n, (int)rank, ew.w, fac, 0, 0);
+      TNB_LAUNCH_CHECK();
+      ++passes;
+      TNB_TRY(stream_pass<TIn>(ring, src, pinned_src, row_bytes, plan, buf, st,
+                               [&](int64_t, const TIn* X, int64_t r0, int64_t rc) -> int {
+                                 T* out = carry0 + (size_t)r0 * rank;
+                                 if constexpr (tc_input<TIn>())
+                                   if (ptc_ws)
+                                     return project_tc<TIn>(X, rc, n, reinterpret_cast<const float*>(fac), (int)rank,
+                                                            reinterpret_cast<float*>(out), ptc_ws, ptc_bytes, st,
+                                                            c0.kblocked ? PT_OUT_KBLOCKED : PT_ROWMAJOR,
+                                                            c0.kblocked ? inner : 0);
+                                 return project_any<T, TIn>(X, rc, n, fac, rank, out, st);
+                               }));
+    }
+    if (info) {
+      info->stream_passes = passes;
+      info->stream_chunks = (int)plan.nchunks;
+      if (spec_tail && rank != kcap) info->spec_flags = hs->zero_flag ? 32 : 16;  // spec_check_kernel's bits
+    }
+    ranks_host[0] = 1;
+    ranks_host[mu] = (int32_t)rank;
+    ranks_host[N] = 1;
+    c0.rank = rank;
+  }
+  ar.off = mark;  // the rest of the sweep reuses the chunk ring and step 0's scratch
+  TNB_TRY((ttsvd_impl<T, TIn, ArenaT>(ar, dry, nullptr, d, rmax, eps, flags, cores, ranks_host, info, st, &c0)));
+  if (dry && peak > ar.off) ar.off = peak;
+  return TNB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------

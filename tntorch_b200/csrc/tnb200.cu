@@ -45,6 +45,41 @@ inline int require_device() {
 }
 // headroom for rank-dependent re-planning between the sizing pass (rank caps) and the run (actual ranks)
 inline size_t with_slack(size_t bytes) { return bytes + bytes / 8 + (size_t)(4 << 20); }
+// f(T{}, TIn{}) for the dense TT-SVD's input code: T the carries and cores, TIn the input
+template <class F>
+inline int with_dense_types(int dtype, F&& f) {
+  switch (dtype) {
+    case TNB_F32: return f(float{}, float{});
+    case TNB_BF16: return f(float{}, __nv_bfloat16{});
+    case TNB_F16: return f(float{}, __half{});
+    case TNB_F8E4M3: return f(float{}, __nv_fp8_e4m3{});
+    case TNB_F8E5M2: return f(float{}, __nv_fp8_e5m2{});
+    default: return f(double{}, double{});
+  }
+}
+inline void write_ttsvd_info(const SweepInfo& info, double* info_host) {
+  if (!info_host) return;
+  for (int i = 0; i < 32; ++i) info_host[i] = 0.0;
+  info_host[0] = info.norm;
+  info_host[1] = info.eig_solves;
+  info_host[2] = info.chfsi_products;
+  info_host[3] = info.tc_grams;
+  info_host[7] = info.nsteps;
+  info_host[31] = info.fused_filters;
+  info_host[29] = info.rr_sweeps;
+  info_host[30] = info.rr_solves;
+  info_host[26] = info.speculative;
+  info_host[27] = info.spec_flags;
+  info_host[28] = info.kblocked_steps;
+  for (int t = 0; t < info.nsteps && t < 6; ++t) {
+    info_host[4] += info.gram_ms[t];
+    info_host[5] += info.eig_ms[t];
+    info_host[6] += info.factor_ms[t];
+    info_host[8 + 3 * t] = info.gram_ms[t];
+    info_host[9 + 3 * t] = info.eig_ms[t];
+    info_host[10 + 3 * t] = info.factor_ms[t];
+  }
+}
 }  // namespace
 
 extern "C" {
@@ -123,27 +158,53 @@ int tnb_ttsvd(int dtype, const void* data, int ndim, const int64_t* shape, const
   else
     rc = ttsvd_impl<double, double>(ar, false, static_cast<const double*>(data), d, rmax, eps, flags,
                                     static_cast<double*>(cores), ranks_host, &info, as_stream(stream));
+  write_ttsvd_info(info, info_host);
+  return rc;
+}
+
+size_t tnb_ttsvd_stream_workspace_bytes(int dtype, int ndim, const int64_t* shape, const int32_t* rmax,
+                                        size_t chunk_bytes, uint32_t flags) {
+  SweepDims d;
+  if (check_ttsvd_dtype(dtype) != TNB_OK || !shape || make_dims(ndim, shape, rmax, d) != TNB_OK) return 0;
+  ArenaSizer ar;
+  size_t ring = 0;
+  const int rc = with_dense_types(dtype, [&](auto t, auto tin) {
+    using T = decltype(t);
+    using TIn = decltype(tin);
+    return ttsvd_stream_impl<T, TIn>(ar, true, (const TIn*)nullptr, d, rmax, 0.0, flags, chunk_bytes, (T*)nullptr, nullptr,
+                                     nullptr, 0, &ring);
+  });
+  if (rc != TNB_OK) return 0;
+  return ring + with_slack(ar.off - ring);  // the chunk ring is sized exactly; the rest gets the sweep's headroom
+}
+
+int tnb_ttsvd_stream(int dtype, const void* data_host, int ndim, const int64_t* shape, const int32_t* rmax, double eps,
+                     uint32_t flags, size_t chunk_bytes, void* workspace, size_t workspace_bytes, void* cores,
+                     int64_t cores_capacity, int32_t* ranks_host, double* info_host, void* stream) {
+  TNB_TRY(check_ttsvd_dtype(dtype));
+  TNB_TRY(require_device());
+  if (!data_host || !shape || !cores || !ranks_host || !workspace)
+    return fail(TNB_ERR_INVALID, "tnb_ttsvd_stream: null argument");
+  if (rmax)
+    for (int k = 0; k < ndim - 1; ++k)
+      if (rmax[k] < 0) return fail(TNB_ERR_INVALID, "rmax[%d] must be >= 1 (or 0 for none)", k);
+  SweepDims d;
+  TNB_TRY(make_dims(ndim, shape, rmax, d));
+  if (cores_capacity < d.capacity)
+    return fail(TNB_ERR_WORKSPACE, "tnb_ttsvd_stream: cores buffer holds %lld elements, need %lld", (long long)cores_capacity,
+                (long long)d.capacity);
+  Arena ar(workspace, workspace_bytes);
+  SweepInfo info;
+  const int rc = with_dense_types(dtype, [&](auto t, auto tin) {
+    using T = decltype(t);
+    using TIn = decltype(tin);
+    return ttsvd_stream_impl<T, TIn>(ar, false, static_cast<const TIn*>(data_host), d, rmax, eps, flags, chunk_bytes,
+                                     static_cast<T*>(cores), ranks_host, &info, as_stream(stream));
+  });
+  write_ttsvd_info(info, info_host);
   if (info_host) {
-    for (int i = 0; i < 32; ++i) info_host[i] = 0.0;
-    info_host[0] = info.norm;
-    info_host[1] = info.eig_solves;
-    info_host[2] = info.chfsi_products;
-    info_host[3] = info.tc_grams;
-    info_host[7] = info.nsteps;
-    info_host[31] = info.fused_filters;
-    info_host[29] = info.rr_sweeps;
-    info_host[30] = info.rr_solves;
-    info_host[26] = info.speculative;
-    info_host[27] = info.spec_flags;
-    info_host[28] = info.kblocked_steps;
-    for (int t = 0; t < info.nsteps && t < 6; ++t) {
-      info_host[4] += info.gram_ms[t];
-      info_host[5] += info.eig_ms[t];
-      info_host[6] += info.factor_ms[t];
-      info_host[8 + 3 * t] = info.gram_ms[t];
-      info_host[9 + 3 * t] = info.eig_ms[t];
-      info_host[10 + 3 * t] = info.factor_ms[t];
-    }
+    info_host[24] = info.stream_passes;
+    info_host[25] = info.stream_chunks;
   }
   return rc;
 }

@@ -134,10 +134,74 @@ def ttsvd(data: torch.Tensor, rmax=None, eps: float = 1e-14, batch_mode: bool = 
         r0, r1 = ranks[k], ranks[k + 1]
         cores.append(cores_buf[offs[k]: offs[k] + r0 * shape[k] * r1].view(r0, shape[k], r1))
     if return_info:
-        return cores, dict(norm=info[0], eig_solves=int(info[1]), chfsi_products=int(info[2]), tc_grams=int(info[3]),
-                           fused_filters=int(info[31]), rr_sweeps=int(info[29]), outer_iterations=int(info[30]),
-                           speculative=int(info[26]), spec_flags=int(info[27]), kblocked_steps=int(info[28]))
+        return cores, _ttsvd_info(info)
     return cores
+
+
+def _ttsvd_info(info) -> dict:
+    return dict(norm=info[0], eig_solves=int(info[1]), chfsi_products=int(info[2]), tc_grams=int(info[3]),
+                fused_filters=int(info[31]), rr_sweeps=int(info[29]), outer_iterations=int(info[30]),
+                speculative=int(info[26]), spec_flags=int(info[27]), kblocked_steps=int(info[28]))
+
+
+def ttsvd_stream(X_cpu: torch.Tensor, rmax=None, eps: float = 1e-14, chunk_bytes: Optional[int] = None,
+                 return_info: bool = False):
+    """Dense tensor in host memory -> TT cores on the current CUDA device, without ever holding the whole tensor there
+    (tnb_ttsvd_stream): step 0 streams it through the device in chunks of about `chunk_bytes` (None: 256 MiB), the rest
+    of the sweep runs as in `ttsvd`.  For tensors larger than free device memory.  `X_cpu`: a CPU tensor of any dtype
+    `ttsvd` takes (pinned memory copies at full speed; pageable memory is staged through pinned pieces).  `info` is that
+    of `ttsvd` plus `passes` (over the host tensor: 2, or 3 when the tensor-core step-0 Gram was rejected for the exact
+    one) and `chunks` (per pass); its `norm` is ‖X‖_F, see `tt_relative_error_from_norm`."""
+    if X_cpu.is_cuda:
+        raise ValueError("ttsvd_stream: X_cpu must be a CPU tensor (decompose a device tensor with ttsvd)")
+    X = X_cpu.contiguous()
+    code = _dense_code(X.dtype)
+    dev = torch.device("cuda", torch.cuda.current_device())
+    N = X.dim()
+    shape = list(X.shape)
+    rm = _rmax_list(rmax, max(N - 1, 0))
+    L = lib()
+    sh = i64(shape)
+    rmc = i32(rm) if N > 1 else i32([0])
+    offs = (C.c_int64 * max(N, 1))()
+    cap = L.tnb_ttsvd_cores_capacity(N, sh, rmc, offs)
+    if cap < 0:
+        check(_lib.ERR_INVALID)
+    cb = 0 if chunk_bytes is None else int(chunk_bytes)
+    wsb = L.tnb_ttsvd_stream_workspace_bytes(code, N, sh, rmc, cb, 0)
+    if wsb == 0:
+        check(_lib.ERR_UNSUPPORTED)
+    ws = _ws(wsb, dev)
+    cores_buf = torch.empty(int(cap), dtype=_core_dtype(X.dtype), device=dev)
+    ranks = (C.c_int32 * (N + 1))()
+    info = (C.c_double * 32)()
+    with torch.cuda.device(dev):
+        check(L.tnb_ttsvd_stream(code, _ptr(X), N, sh, rmc, float(eps), 0, cb, _ptr(ws), ws.numel(), _ptr(cores_buf), cap,
+                                 ranks, info, _stream()))
+    cores = [cores_buf[offs[k]: offs[k] + ranks[k] * shape[k] * ranks[k + 1]].view(ranks[k], shape[k], ranks[k + 1])
+             for k in range(N)]
+    if return_info:
+        return cores, dict(_ttsvd_info(info), passes=int(info[24]), chunks=int(info[25]))
+    return cores
+
+
+def stream_instead_of_copy(input_bytes: int, workspace_bytes: int, free_bytes: int) -> bool:
+    """The rule `tn.Tensor(X_cpu, ranks_tt=r)` decomposes by: stream the host tensor (`ttsvd_stream`) when its device
+    image and the device call's workspace would not fit in free device memory, copy it and call `ttsvd` otherwise."""
+    return input_bytes + workspace_bytes > free_bytes
+
+
+def tt_relative_error_from_norm(norm: float, cores: Sequence[torch.Tensor]) -> float:
+    """‖T − TT(cores)‖_F / ‖T‖_F from ‖T‖_F alone (`info["norm"]` of `ttsvd` / `ttsvd_stream`), for cores in the TT-SVD
+    gauge: cores 1…N−1 have orthonormal right unfoldings, so ‖T − T̂‖² = ‖T‖² − ‖core_0‖².  This is the error of a
+    decomposition whose input never fits on the device.  It is only meaningful when the relative error is well above
+    the resolution of ‖core_0‖² in the cores' precision: about 1e-3 for float32 cores (the difference of two squared
+    norms loses the rest); below that, use `tt_relative_error` on the data."""
+    norm = float(norm)
+    if norm == 0.0:
+        return 0.0
+    c0 = float(torch.linalg.vector_norm(cores[0].detach().double()))
+    return max(norm * norm - c0 * c0, 0.0) ** 0.5 / norm
 
 
 class TTSVDPlan:

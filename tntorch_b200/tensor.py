@@ -26,6 +26,19 @@ def _default_device(device):
     return device
 
 
+def _streams(data: torch.Tensor, ranks_tt, dev) -> bool:
+    """Whether a rank-capped decomposition of `data` streams it from host memory (ops.ttsvd_stream) instead of copying
+    it to `dev`: only for a CPU tensor of two or more modes whose device image plus the device call's workspace exceeds
+    free device memory (ops.stream_instead_of_copy)."""
+    if data.is_cuda or data.dim() < 2:
+        return False
+    shape = list(data.shape)
+    rm = ops._rmax_list(ranks_tt, len(shape) - 1)
+    wsb = ops.lib().tnb_ttsvd_workspace_bytes(ops._dense_code(data.dtype), len(shape), ops.i64(shape), ops.i32(rm), 0)
+    free, _ = torch.cuda.mem_get_info(dev)
+    return ops.stream_instead_of_copy(data.numel() * data.element_size(), int(wsb), int(free))
+
+
 class Tensor(object):
     """TT tensor whose decomposition / rounding runs on H100 kernels (mirror of tntorch.Tensor)."""
 
@@ -69,7 +82,10 @@ class Tensor(object):
                     "A tntorch.Tensor may be built either from a list of cores, one NumPy ndarray, or one PyTorch tensor"
                 )
             dev = _default_device(device if device is not None else (data.device if data.is_cuda else None))
-            data = data.to(dev)
+            stream = (ranks_tt is not None and eps is None and ranks_cp is None and ranks_tucker is None and not batch
+                      and _streams(data, ranks_tt, dev))
+            if not stream:
+                data = data.to(dev)
             if data.dim() == 0:
                 if data.dtype in (torch.float8_e4m3fn, torch.float8_e5m2):  # torch has no arithmetic on float8
                     data = data.reshape(1).clone()
@@ -131,6 +147,9 @@ class Tensor(object):
                 # one library call for the whole batch: several samples in flight inside libtnb200 (tnb_ttsvd_batch)
                 per = ops.ttsvd_batch(data, rmax=ranks_tt, batch_mode=True)
                 self.cores = [torch.stack([p[k] for p in per], dim=0) for k in range(N)]
+            elif stream:
+                with torch.cuda.device(dev):
+                    self.cores = ops.ttsvd_stream(data, rmax=ranks_tt)
             else:
                 self.cores = ops.ttsvd(data, rmax=ranks_tt)
         if Us is None:
