@@ -147,7 +147,9 @@ def cross_batch(functions, domain, ranks_tt, batch=None, eps=1e-6, max_iter=25, 
         ve = torch.linalg.vector_norm(ys_val - approx, dim=1) / norm_ys_val
         val_eps = torch.where(active.bool(), ve, val_eps)
         iterations.add_(active.long())
-        active = active * (val_eps >= eps).int()  # cross.py:461-462: a converged problem stops
+        # cross.py:460-462: a converged problem stops.  Written as "not below eps" so that a NaN val_eps (the unscaled
+        # norm of a function beyond ~1e+-154 over- or underflows) keeps sweeping, as the sequential call does
+        active = active * (~(val_eps < eps)).int()
         if not bool(active.any()) or it == max_iter - 1:
             break
 

@@ -10,22 +10,33 @@ constexpr int JACOBI_MAX_N = 256;      // one-CTA solver limit (matrix in L1/L2-
 constexpr int JACOBI_SMEM_MAX_N = 104; // A and V both in shared memory up to this size
 constexpr int JACOBI_THREADS = 1024;
 
-__device__ __forceinline__ double block_reduce_sum(double v, double* red /*>=32 doubles smem*/) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+// Block-wide reduction of one double per thread with the associative `op` (identity: the value the unused slots of
+// the second stage hold); every thread returns the result.
+template <class Op>
+__device__ __forceinline__ double block_reduce(double v, double* red /*>=32 doubles smem*/, Op op, double identity) {
+  for (int o = 16; o > 0; o >>= 1) v = op(v, __shfl_xor_sync(0xffffffffu, v, o));
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   __syncthreads();
   if (lane == 0) red[w] = v;
   __syncthreads();
   const int nw = (blockDim.x + 31) >> 5;
-  double t = (threadIdx.x < nw) ? red[threadIdx.x] : 0.0;
+  double t = (threadIdx.x < nw) ? red[threadIdx.x] : identity;
   if (w == 0) {
-    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+    for (int o = 16; o > 0; o >>= 1) t = op(t, __shfl_xor_sync(0xffffffffu, t, o));
     if (lane == 0) red[0] = t;
   }
   __syncthreads();
   const double out = red[0];
   __syncthreads();
   return out;
+}
+
+struct SumOp {
+  __device__ __forceinline__ double operator()(double a, double b) const { return a + b; }
+};
+
+__device__ __forceinline__ double block_reduce_sum(double v, double* red /*>=32 doubles smem*/) {
+  return block_reduce(v, red, SumOp{}, 0.0);
 }
 
 // Rotation (c, s) that orthogonalises two columns with squared norms dpp, dqq and inner product dpq:

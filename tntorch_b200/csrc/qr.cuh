@@ -7,11 +7,25 @@
 //
 // Column operations are warp-per-column: the inner products v^T a_c are lane-strided sums finished with
 // shuffles, the reflector norm is a block reduction, one barrier per reflector.
+//
+// The reflector is formed like LAPACK dlarfg: the norm of x = col[j+1:] is taken as m * sqrt(sum (x_i/m)^2) with
+// m = max |x_i| (one more block reduction per column), and beta = -sign(alpha) hypot(alpha, ||x||).  An unscaled
+// sum of squares underflows to 0 below |x| ~ 1e-160 (every tau 0, Q = I) and overflows above ~ 1e154, so Q would
+// depend on the scale of the input; with the scaled norm Q(c A) = Q(A) and R(c A) = c R(A) to rounding for any
+// normal c.  dlarfg's extra rescaling of |beta| < 2e-292 (subnormal-range results) is not reproduced.  The max keeps
+// NaN, so a NaN input still reaches Q and R.
 #pragma once
+#include <cfloat>
+
 #include "common.cuh"
 #include "jacobi.cuh"
 
 namespace tnb {
+
+// max that keeps NaN (fmax would drop it): a NaN anywhere below the diagonal makes m, and so Q and R, NaN
+struct NanMaxOp {
+  __device__ __forceinline__ double operator()(double a, double b) const { return (b != b || b > a) ? b : a; }
+};
 
 // work: [nbatch][n][rows] (column-major copy of A, holds the reflectors), Qout: [nbatch][rows][k] row-major,
 // Rout (optional): [nbatch][k][n] row-major upper-trapezoidal factor.
@@ -33,14 +47,30 @@ __global__ void __launch_bounds__(512) householder_qr_kernel(const double* __res
   __syncthreads();
   for (int j = 0; j < k; ++j) {
     double* col = W + (size_t)j * rows;
+    double m = 0.0;
+    for (int i = j + 1 + tid; i < rows; i += nt) m = NanMaxOp{}(m, fabs(col[i]));
+    m = block_reduce(m, red, NanMaxOp{}, 0.0);
     double s = 0.0;
-    for (int i = j + 1 + tid; i < rows; i += nt) s = fma(col[i], col[i], s);
-    s = block_reduce_sum(s, red);
+    if (m != 0.0) {
+      if (m >= DBL_MIN) {  // 1/m is finite for a normal m: one reciprocal, then multiplies
+        const double inv_m = 1.0 / m;
+        for (int i = j + 1 + tid; i < rows; i += nt) {
+          const double x = col[i] * inv_m;
+          s = fma(x, x, s);
+        }
+      } else {  // subnormal (1/m would overflow) or NaN
+        for (int i = j + 1 + tid; i < rows; i += nt) {
+          const double x = col[i] / m;
+          s = fma(x, x, s);
+        }
+      }
+      s = block_reduce_sum(s, red);
+    }
     if (tid == 0) {
       const double alpha = col[j];
       double tau = 0.0, scale = 0.0, beta = alpha;
-      if (s != 0.0) {
-        beta = -copysign(sqrt(alpha * alpha + s), alpha);
+      if (m != 0.0) {
+        beta = -copysign(hypot(alpha, m * sqrt(s)), alpha);
         tau = (beta - alpha) / beta;
         scale = 1.0 / (alpha - beta);
       }
