@@ -186,7 +186,8 @@ int tnb_tt_round_batch(int dtype, const void* const* cores_in, int batch, int nd
  *              applied to the first core like the reference's `t * scalar`; at most 16 operands per call
  *   tnb_tt_sum        writes the block cores (summed ranks through tnb_tt_sum_cores_capacity)
  *   tnb_tt_sum_round  assembles them in the workspace and runs the tnb_tt_round sweeps on them in the same call: no
- *                     intermediate tensor exists on the host side; output layout as tnb_tt_round
+ *                     intermediate tensor exists on the host side; output layout as tnb_tt_round.  A workspace smaller
+ *                     than tnb_tt_sum_round_workspace_bytes is refused (TNB_ERR_WORKSPACE) before anything launches
  * ------------------------------------------------------------------------------------------ */
 int64_t tnb_tt_sum_cores_capacity(int noperands, int ndim, const int64_t* shape, const int32_t* ranks_in,
                                   int32_t* ranks_sum_host, int64_t* core_offsets_host);

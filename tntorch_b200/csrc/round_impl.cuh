@@ -557,6 +557,10 @@ inline int truncated_svd_impl(ArenaT& ar, bool dry, const T* M, int64_t m, int64
   // from the subspace solver (an eps/delta-only request and the sizing pass then carve the same amount)
   const int64_t fcap = ew.chfsi ? std::min<int64_t>(L, ew.k) : L;
   T* fac = ar.template take<T>((size_t)L * (size_t)fcap);
+  // the gauge repair of the two forms that divide by s (no F: the factor is scaled by scale_extract), for every rank the
+  // factor scratch can hold: the sizing pass carves with rmax = 240, which must cover an rmax-free direct solve up to 256
+  WideWork ww;
+  wide_carve(ar, 0, K, fcap, ww);
   if (dry) return TNB_OK;
   if (!ar.ok) return fail(TNB_ERR_WORKSPACE, "truncated_svd: workspace too small (need > %zu bytes)", ar.off);
   int* h_sc = static_cast<int*>(pinned_scratch(sizeof(SweepScalars)));
@@ -587,6 +591,12 @@ inline int truncated_svd_impl(ArenaT& ar, bool dry, const T* M, int64_t m, int64
   // batch mode: a zero sample keeps rank = min(rmax, len(S)) (its factors come out as zeros); the sign tells the
   // caller, which returns rank-1 zeros only when EVERY sample of the batch is zero (round.py:138-142)
   *rank_host = (batch_mode && hs->zero_flag) ? -(int32_t)r : (int32_t)r;
+  // The two forms that divide by s scale with d_j = max(s_j, 1e-8 s_0) (scale_extract modes 3 and 4; d = s above that
+  // floor, so their bits are those of 1/s and s) and then take the gauge repair of the dense sweep's wide step
+  // (chol_qr_repair): when a kept s_j lies at the Gram's noise floor (rmax, batch_mode or a small eps keeps more than the
+  // numerical rank), diag(1/s) U_r^T M is not orthonormal.  On a spectrum above the floor the fp64 Gram check skips the
+  // repair.  A zero sample of a batch keeps its zero factors.
+  const bool repair = !(batch_mode && hs->zero_flag);
   if (use_left) {
     if (left_ortho) {  // left = U_r ; right = U_r^T M
       scale_extract_kernel<T><<<grid_for(m * r), 256, 0, st>>>(ew.V, ew.ldv, (int)m, (int)r, ew.w, left, 0, 0);
@@ -594,21 +604,23 @@ inline int truncated_svd_impl(ArenaT& ar, bool dry, const T* M, int64_t m, int64
       TNB_TRY((gemm_direct<T, T, T, T>(r, n, m, left, r, false, M, n, false, right, n, (T)1, nullptr, 0, (T)0, nullptr, 0,
                                        (T)0, st)));
     } else {  // right = diag(1/s) U_r^T M ; left = U_r diag(s)     (round.py:170-172)
-      scale_extract_kernel<T><<<grid_for(m * r), 256, 0, st>>>(ew.V, ew.ldv, (int)m, (int)r, ew.w, fac, 1, 0);
+      scale_extract_kernel<T><<<grid_for(m * r), 256, 0, st>>>(ew.V, ew.ldv, (int)m, (int)r, ew.w, fac, 3, 0);
       TNB_LAUNCH_CHECK();
       TNB_TRY((gemm_direct<T, T, T, T>(r, n, m, fac, r, false, M, n, false, right, n, (T)1, nullptr, 0, (T)0, nullptr, 0,
                                        (T)0, st)));
-      scale_extract_kernel<T><<<grid_for(m * r), 256, 0, st>>>(ew.V, ew.ldv, (int)m, (int)r, ew.w, left, 2, 0);
+      scale_extract_kernel<T><<<grid_for(m * r), 256, 0, st>>>(ew.V, ew.ldv, (int)m, (int)r, ew.w, left, 4, 0);
       TNB_LAUNCH_CHECK();
+      if (repair) TNB_TRY((chol_qr_repair<T, true>(ww, r, right, n, left, m, st)));
     }
   } else {
     if (left_ortho) {  // left = M (V_r / s) ; right = diag(s) V_r^T     (round.py:175-179)
-      scale_extract_kernel<T><<<grid_for(n * r), 256, 0, st>>>(ew.V, ew.ldv, (int)n, (int)r, ew.w, fac, 1, 0);
+      scale_extract_kernel<T><<<grid_for(n * r), 256, 0, st>>>(ew.V, ew.ldv, (int)n, (int)r, ew.w, fac, 3, 0);
       TNB_LAUNCH_CHECK();
       TNB_TRY((gemm_direct<T, T, T, T>(m, r, n, M, n, true, fac, r, false, left, r, (T)1, nullptr, 0, (T)0, nullptr, 0,
                                        (T)0, st)));
-      scale_extract_kernel<T><<<grid_for(n * r), 256, 0, st>>>(ew.V, ew.ldv, (int)n, (int)r, ew.w, right, 2, 1);
+      scale_extract_kernel<T><<<grid_for(n * r), 256, 0, st>>>(ew.V, ew.ldv, (int)n, (int)r, ew.w, right, 4, 1);
       TNB_LAUNCH_CHECK();
+      if (repair) TNB_TRY((chol_qr_repair<T, false>(ww, r, left, m, right, n, st)));
     } else {  // left = M V_r ; right = V_r^T     (round.py:180-183)
       scale_extract_kernel<T><<<grid_for(n * r), 256, 0, st>>>(ew.V, ew.ldv, (int)n, (int)r, ew.w, fac, 0, 0);
       TNB_LAUNCH_CHECK();
@@ -657,7 +669,10 @@ __global__ void __launch_bounds__(256) recon_diff_kernel(const T* __restrict__ F
 template <typename T, typename TD, class ArenaT>
 inline int tt_relative_error_impl(ArenaT& ar, bool dry, const TD* data, const T* const* cores, int N,
                                   const int64_t* shape, const int32_t* ranks, double* result_host, cudaStream_t st) {
-  if (N < 2) return fail(TNB_ERR_UNSUPPORTED, "tt_relative_error: needs at least 2 modes");
+  if (N < 2) return fail(TNB_ERR_INVALID, "tt_relative_error: needs at least 2 modes");
+  if (ranks[0] != 1 || ranks[N] != 1) return fail(TNB_ERR_INVALID, "tt_relative_error: boundary TT ranks must be 1");
+  for (int k = 0; k < N; ++k)
+    if (ranks[k + 1] < 1 || shape[k] < 1) return fail(TNB_ERR_INVALID, "tt_relative_error: ranks and mode sizes must be >= 1");
   double* acc = ar.template take<double>(2);
   // F_k : (prod_{j<=k} I_j) x r_{k+1}; ping-pong buffers up to k = N-2
   size_t felems[2] = {1, 1};

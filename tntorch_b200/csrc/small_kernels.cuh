@@ -162,9 +162,11 @@ __global__ void convert_kernel(const TIn* __restrict__ in, int64_t n, TOut* __re
 
 // out[i][j] (or out[j][i] when transpose) = V[i][j] * f(w_j) for j < rank, i < rows.
 //   mode 0: f = 1        mode 1: f = 1/sqrt(w_j)        mode 2: f = sqrt(w_j)
+//   mode 3: f = 1/d_j    mode 4: f = d_j,   d_j = max(sqrt(w_j), 1e-8 sqrt(w_0))  (modes 1 and 2 where s_j >= 1e-8 s_0)
 template <typename TOut>
 __global__ void scale_extract_kernel(const double* __restrict__ V, int ldv, int rows, int rank,
                                      const double* __restrict__ w, TOut* __restrict__ out, int mode, int transpose) {
+  const double s0 = mode >= 3 ? sqrt(w[0] > 0.0 ? w[0] : 0.0) : 0.0;
   const int64_t total = (int64_t)rows * rank;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (int64_t)gridDim.x * blockDim.x) {
@@ -179,8 +181,8 @@ __global__ void scale_extract_kernel(const double* __restrict__ V, int ldv, int 
     double f = 1.0;
     if (mode != 0) {
       const double wj = w[j] > 0.0 ? w[j] : 0.0;
-      const double s = sqrt(wj);
-      f = (mode == 1) ? (s > 0.0 ? 1.0 / s : 0.0) : s;
+      const double s = mode >= 3 ? fmax(sqrt(wj), 1e-8 * s0) : sqrt(wj);
+      f = (mode == 1 || mode == 3) ? (s > 0.0 ? 1.0 / s : 0.0) : s;
     }
     out[idx] = (TOut)(V[(size_t)i * ldv + j] * f);
   }

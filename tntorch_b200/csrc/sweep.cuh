@@ -465,7 +465,9 @@ __global__ void __launch_bounds__(1024) wide_chol_kernel(const double* __restric
 // core row that was exactly zero (S_jj <= 1e-30 max S: U_r's direction meets a null row space of C, or the tensor is
 // zero) has no direction to keep: it becomes a fixed pseudo-random row and its Cn column zero, which leaves Cn core as it
 // was; the next step orthonormalises it against the others.
-template <typename T, bool CORE>
+// CORE picks the role (the orthonormalised factor, updated by T, or the other one, updated by R); KMAJOR the layout:
+// X[k][g] (rank x nvec, a core's rows) or X[g][k] (nvec x rank, Cn's rows).  truncated_svd's tall form has them swapped.
+template <typename T, bool CORE, bool KMAJOR = CORE>
 __global__ void __launch_bounds__(256) wide_apply_kernel(const double* __restrict__ M, const double* __restrict__ S, int rank,
                                                          int64_t nvec, T* __restrict__ X, int fill, const int* ctrl) {
   extern __shared__ __align__(16) unsigned char wide_apply_smem[];
@@ -480,7 +482,7 @@ __global__ void __launch_bounds__(256) wide_apply_kernel(const double* __restric
     for (int idx = threadIdx.x; idx < rank * 32; idx += blockDim.x) {
       const int k = idx / 32, v = idx % 32;
       const int64_t g = v0 + v;
-      x[idx] = g < nvec ? (double)(CORE ? X[(size_t)k * nvec + g] : X[(size_t)g * rank + k]) : 0.0;
+      x[idx] = g < nvec ? (double)(KMAJOR ? X[(size_t)k * nvec + g] : X[(size_t)g * rank + k]) : 0.0;
     }
     __syncthreads();
     const int64_t g = v0 + lane;
@@ -500,7 +502,7 @@ __global__ void __launch_bounds__(256) wide_apply_kernel(const double* __restric
             acc = 0.0;
           }
         }
-        if (CORE) X[(size_t)j * nvec + g] = (T)acc;
+        if (KMAJOR) X[(size_t)j * nvec + g] = (T)acc;
         else X[(size_t)g * rank + j] = (T)acc;
       }
   }
@@ -510,6 +512,43 @@ __global__ void __launch_bounds__(256) wide_apply_kernel(const double* __restric
 // diag(1/d) U_r^T C leaves them within ~eps_64 lambda_0 / lambda_{r-1} of it, plus the storage rounding).
 template <typename T>
 constexpr double wide_orth_tol() { return std::is_same<T, double>::value ? 1e-13 : 1e-6; }
+
+// The gauge repair of a split Q P (Q: `rank` vectors of length nq that should be orthonormal; P: the other factor, np
+// vectors of length rank): the fp64 Gram of Q's vectors (split-K GEMM, ww.splits); when it is within wide_orth_tol of I
+// the rest is skipped on the device; otherwise two Cholesky-QR steps (one-CTA Cholesky of the rank x rank Gram, in-place
+// triangular updates of Q and P on the whole GPU, a second Gram).  Q_KMAJOR: Q is rank x nq row-major and P np x rank
+// (a wide step's core and Cn), else Q is nq x rank and P rank x np (truncated_svd's tall form, left and right).
+// Positive diagonals keep the basis; the product Q^T P^T (or Q P) is unchanged but for rounding.
+template <typename T, bool Q_KMAJOR>
+inline int chol_qr_repair(const WideWork& ww, int64_t rank, T* Q, int64_t nq, T* P, int64_t np, cudaStream_t st) {
+  const GemmPlan pl = plan_gemm(rank, rank, nq, true, ww.splits);
+  const size_t csm = (size_t)2 * rank * (rank | 1) * sizeof(double), asm_bytes = (size_t)rank * 32 * sizeof(double);
+  const bool fits = csm <= 180 * 1024;
+  static PerDeviceFlag attr_chol, attr_q, attr_p;
+  TNB_CUDA(ensure_dyn_smem(attr_chol, wide_chol_kernel<double>, 180 * 1024));
+  TNB_CUDA(ensure_dyn_smem(attr_q, wide_apply_kernel<T, true, Q_KMAJOR>, 64 * 1024));
+  TNB_CUDA(ensure_dyn_smem(attr_p, wide_apply_kernel<T, false, !Q_KMAJOR>, 64 * 1024));
+  const int grid_q = (int)std::min<int64_t>(ceil_div<int64_t>(nq, 32), 8 * usable_sms());
+  const int grid_p = (int)std::min<int64_t>(ceil_div<int64_t>(np, 32), 8 * usable_sms());
+  const int ldq = Q_KMAJOR ? (int)nq : (int)rank;
+  // two Cholesky-QR steps, all of them skipped on the device when the first Gram finds the vectors orthonormal
+  for (int pass = 0; pass < 2; ++pass) {
+    TNB_TRY((gemm_splitk<T, T, double, double, float>(pl, rank, rank, nq, Q, ldq, Q_KMAJOR, Q, ldq, Q_KMAJOR, ww.partial, ww.S,
+                                                      rank, 1.0, nullptr, 0, 0.0, nullptr, 0, 0.0, true, (float*)nullptr, 0, st,
+                                                      pass ? ww.ctrl : nullptr, 0)));
+    if (pass == 0) {
+      wide_check_kernel<<<1, 32, 0, st>>>(ww.S, (int)rank, wide_orth_tol<T>(), ww.ctrl);
+      TNB_LAUNCH_CHECK();
+    }
+    wide_chol_kernel<double><<<1, 1024, fits ? csm : 0, st>>>(ww.S, (int)rank, ww.scratch, ww.Tm, fits ? 1 : 0, ww.Rm, ww.ctrl);
+    TNB_LAUNCH_CHECK();
+    wide_apply_kernel<T, true, Q_KMAJOR><<<grid_q, 256, asm_bytes, st>>>(ww.Tm, ww.S, (int)rank, nq, Q, pass == 0, ww.ctrl);
+    TNB_LAUNCH_CHECK();
+    wide_apply_kernel<T, false, !Q_KMAJOR><<<grid_p, 256, asm_bytes, st>>>(ww.Rm, ww.S, (int)rank, np, P, pass == 0, ww.ctrl);
+    TNB_LAUNCH_CHECK();
+  }
+  return TNB_OK;
+}
 
 // The end of a truncation step at rank `rank`, from the step's eigenpairs (w descending, V with leading dimension ldv):
 //   tall (rows >= n): core = V_r^T (rank x n);  Cn = C V_r;
@@ -544,32 +583,7 @@ inline int step_factors(const StepCtx& cx, const TIn* C, int64_t rows, int64_t n
   TNB_LAUNCH_CHECK();
   TNB_TRY((gemm_direct<double, TIn, double, T>(rank, n, rows, ww.F, rank, false, C, n, false, core, n, 1.0, nullptr, 0, 0.0,
                                                nullptr, 0, 0.0, st)));
-  const GemmPlan pl = plan_gemm(rank, rank, n, true, ww.splits);
-  const size_t csm = (size_t)2 * rank * (rank | 1) * sizeof(double), asm_bytes = (size_t)rank * 32 * sizeof(double);
-  const bool fits = csm <= 180 * 1024;
-  static PerDeviceFlag attr_chol, attr_core, attr_cn;
-  TNB_CUDA(ensure_dyn_smem(attr_chol, wide_chol_kernel<double>, 180 * 1024));
-  TNB_CUDA(ensure_dyn_smem(attr_core, wide_apply_kernel<T, true>, 64 * 1024));
-  TNB_CUDA(ensure_dyn_smem(attr_cn, wide_apply_kernel<T, false>, 64 * 1024));
-  const int grid_core = (int)std::min<int64_t>(ceil_div<int64_t>(n, 32), 8 * usable_sms());
-  const int grid_cn = (int)std::min<int64_t>(ceil_div<int64_t>(rows, 32), 8 * usable_sms());
-  // two Cholesky-QR steps, all of them skipped on the device when the first Gram finds the rows orthonormal
-  for (int pass = 0; pass < 2; ++pass) {
-    TNB_TRY((gemm_splitk<T, T, double, double, float>(pl, rank, rank, n, core, n, true, core, n, true, ww.partial, ww.S, rank,
-                                                      1.0, nullptr, 0, 0.0, nullptr, 0, 0.0, true, (float*)nullptr, 0, st,
-                                                      pass ? ww.ctrl : nullptr, 0)));
-    if (pass == 0) {
-      wide_check_kernel<<<1, 32, 0, st>>>(ww.S, (int)rank, wide_orth_tol<T>(), ww.ctrl);
-      TNB_LAUNCH_CHECK();
-    }
-    wide_chol_kernel<double><<<1, 1024, fits ? csm : 0, st>>>(ww.S, (int)rank, ww.scratch, ww.Tm, fits ? 1 : 0, ww.Rm, ww.ctrl);
-    TNB_LAUNCH_CHECK();
-    wide_apply_kernel<T, true><<<grid_core, 256, asm_bytes, st>>>(ww.Tm, ww.S, (int)rank, n, core, pass == 0, ww.ctrl);
-    TNB_LAUNCH_CHECK();
-    wide_apply_kernel<T, false><<<grid_cn, 256, asm_bytes, st>>>(ww.Rm, ww.S, (int)rank, rows, Cn, pass == 0, ww.ctrl);
-    TNB_LAUNCH_CHECK();
-  }
-  return TNB_OK;
+  return chol_qr_repair<T, true>(ww, rank, core, n, Cn, rows, st);
 }
 
 // TIn: the element type of C (the dense input at step 0, else T).

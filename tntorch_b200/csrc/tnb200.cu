@@ -431,7 +431,11 @@ int tnb_tt_sum_round(int dtype, const void* const* cores_in, int noperands, cons
   if (cores_capacity < rd.capacity) return fail(TNB_ERR_WORKSPACE, "tnb_tt_sum_round: cores buffer too small");
   const size_t esz = dtype == TNB_F32 ? 4 : 8;
   const size_t abytes = align_up((size_t)sd.capacity * esz);
-  if (workspace_bytes < abytes) return fail(TNB_ERR_WORKSPACE, "tnb_tt_sum_round: workspace too small");
+  // the whole requirement (assembled cores + the rounding's workspace) is checked before the assembly launches
+  const size_t need = tnb_tt_sum_round_workspace_bytes(dtype, noperands, ndim, shape, ranks_in, rmax);
+  if (need == 0) return fail(TNB_ERR_UNSUPPORTED, "tnb_tt_sum_round: unsupported shape");
+  if (workspace_bytes < need)
+    return fail(TNB_ERR_WORKSPACE, "tnb_tt_sum_round: workspace too small (need %zu bytes, got %zu)", need, workspace_bytes);
   char* base = static_cast<char*>(workspace);
   std::vector<const void*> ptrs(ndim);
   cudaStream_t st = as_stream(stream);

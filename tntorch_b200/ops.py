@@ -1066,6 +1066,10 @@ def tt_relative_error(data: torch.Tensor, cores: Sequence[torch.Tensor]) -> floa
     code = _dense_code(data.dtype)
     if data.dtype in _DT_LOW and any(c.dtype != torch.float32 for c in cores):
         raise ValueError(f"tt_relative_error: {str(data.dtype).replace('torch.', '')} data needs float32 cores")
+    if len(cores) != N or any(c.dim() != 3 for c in cores) or [c.shape[1] for c in cores] != list(data.shape):
+        raise ValueError("tt_relative_error: the cores' mode sizes must match data.shape")
+    if any(cores[k].shape[2] != cores[k + 1].shape[0] for k in range(N - 1)):
+        raise ValueError("tt_relative_error: consecutive core ranks do not match")
     ranks = [cores[0].shape[0]] + [c.shape[2] for c in cores]
     L = lib()
     sh, rk = i64(list(data.shape)), i32(ranks)
