@@ -1,5 +1,5 @@
 """A/B of the in-flight batch schedule (tnb_ttsvd_batch): prints ms per tensor for the 64^5 / r=32 workload.
-Environment switch read by the library: TNB_NO_GATE=1.  Usage: batch_exp.py [inflight] [reserve]"""
+Usage: batch_exp.py [inflight] [reserve]"""
 import sys
 
 import torch

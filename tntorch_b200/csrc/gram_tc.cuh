@@ -97,15 +97,6 @@ struct GramTcParams {
   float* partial;  // [ksplit][num_tiles][128][tn]
   int fold;              // > 1: the matrix was viewed as (rows/fold) x (fold*n_orig); G = sum of the diagonal blocks
   int n_orig;
-  // direct epilogue (general A^T B with ksplit == 1): C = alpha * acc + beta * D + gamma * E written by the
-  // MMA warps, no partial tiles and no finalize kernel.  One CTA per output tile: the narrow form used
-  // when several decompositions share the GPU (few SMs busy per product instead of all of them).
-  int direct;
-  float* C;
-  const float* D;
-  const float* E;
-  int ldc, ldd, lde;
-  float alpha, beta, gamma;
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -650,7 +641,7 @@ __device__ __forceinline__ void gram_tc_transposer(unsigned char* stage_base, un
 
 template <int NT>
 __device__ __forceinline__ void gram_tc_epilogue(const GramTcParams& p, const float (&acc)[NT * 16], int cm, int lane,
-                                                 int tile_id, int split, int a_col0, int b_col0);
+                                                 int tile_id, int split);
 
 // One pipeline stage of a consumer warp: A fragments of stage `it` into `af`, four k8 wgmma into `acc`, then release
 // the slab slot and, once the previous stage's group has completed, its transposed-B buffer.
@@ -682,7 +673,7 @@ template <int NT>
 __device__ __forceinline__ void gram_tc_consumer(const GramTcParams& p, const unsigned char* stage_base,
                                                  const unsigned char* tb_base, uint64_t* full_bar, uint64_t* empty_bar,
                                                  uint64_t* tb_full, uint64_t* tb_empty, int64_t iters, int a_box,
-                                                 int tile_id, int split, int a_col0, int b_col0) {
+                                                 int tile_id, int split) {
   const int ct = threadIdx.x - 128;
   const int lane = ct & 31, w = (ct >> 5) & 3;
   const int cm = 64 * (ct >> 7) + 16 * w;  // first of this warp's 16 rows of the tile
@@ -704,15 +695,14 @@ __device__ __forceinline__ void gram_tc_consumer(const GramTcParams& p, const un
   }
   wgmma_wait<0>();
   wgmma_fence_operand(acc);
-  gram_tc_epilogue<NT>(p, acc, cm, lane, tile_id, split, a_col0, b_col0);
+  gram_tc_epilogue<NT>(p, acc, cm, lane, tile_id, split);
 }
 
 // Consumer warpgroup cw of the K-blocked mode (tn = 256): both operands through descriptors of the stage's k8 slices.  B slice kk is at kk * 8 KB; A (this warpgroup's 64 rows) at a_off + kk * a_slice + 64 * cw rows.  A slot is
 // released once the wgmma group that read it has completed, i.e. one stage later.
 __device__ __forceinline__ void gram_tc_consumer_blocked(const GramTcParams& p, const unsigned char* stage_base,
                                                          uint64_t* full_bar, uint64_t* empty_bar, int64_t iters,
-                                                         int a_off, int a_slice, int tile_id, int split, int a_col0,
-                                                         int b_col0) {
+                                                         int a_off, int a_slice, int tile_id, int split) {
   const int ct = threadIdx.x - 128;
   const int lane = ct & 31, w = (ct >> 5) & 3, cw = ct >> 7;
   const int cm = 64 * cw + 16 * w;
@@ -736,7 +726,7 @@ __device__ __forceinline__ void gram_tc_consumer_blocked(const GramTcParams& p, 
   }
   wgmma_wait<0>();
   wgmma_fence_operand(acc);
-  gram_tc_epilogue<8>(p, acc, cm, lane, tile_id, split, a_col0, b_col0);
+  gram_tc_epilogue<8>(p, acc, cm, lane, tile_id, split);
 }
 
 // Consumer warpgroup cw of the bf16 mode (tn = 128): A (this warpgroup's 64 columns of C, box a_box + cw) and B (the
@@ -754,7 +744,7 @@ __device__ __forceinline__ void gram_tc_consumer_blocked(const GramTcParams& p, 
 template <typename T16, typename T8 = void>
 __device__ __forceinline__ void gram_tc_consumer_bf16(const GramTcParams& p, const unsigned char* stage_base,
                                                       uint64_t* full_bar, uint64_t* empty_bar, int64_t iters, int a_box,
-                                                      int tile_id, int split, int a_col0, int b_col0) {
+                                                      int tile_id, int split) {
   using R = TcRing<TC_BF16>;
   constexpr bool DIAG64 = !std::is_void<T8>::value;
   constexpr int NACC = DIAG64 ? 32 : 64;
@@ -800,7 +790,7 @@ __device__ __forceinline__ void gram_tc_consumer_bf16(const GramTcParams& p, con
     __syncwarp();
     if (it > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % R::STAGES]);
   }
-  if constexpr (DIAG64) {  // columns 64 cw .. 64 cw + 63 of the partial tile (a folded Gram is never direct)
+  if constexpr (DIAG64) {  // columns 64 cw .. 64 cw + 63 of the partial tile
     const int g = lane >> 2, t = lane & 3;
     float* out = p.partial + ((size_t)split * p.num_tiles + tile_id) * 128 * (size_t)p.tn + 64 * cw + 2 * t;
 #pragma unroll
@@ -810,34 +800,15 @@ __device__ __forceinline__ void gram_tc_consumer_bf16(const GramTcParams& p, con
         *reinterpret_cast<float2*>(out + (size_t)(cm + g + 8 * h) * p.tn + 8 * j) =
             make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
   } else {
-    gram_tc_epilogue<4>(p, acc, cm, lane, tile_id, split, a_col0, b_col0);
+    gram_tc_epilogue<4>(p, acc, cm, lane, tile_id, split);
   }
 }
 
 // Output of one consumer warp: acc[4j + 2h + e] is (row cm + g + 8h, column 8j + 2t + e) of the 128 x tn tile.
 template <int NT>
 __device__ __forceinline__ void gram_tc_epilogue(const GramTcParams& p, const float (&acc)[NT * 16], int cm, int lane,
-                                                 int tile_id, int split, int a_col0, int b_col0) {
+                                                 int tile_id, int split) {
   const int g = lane >> 2, t = lane & 3;
-  if (p.direct) {
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int gi = a_col0 + cm + g + 8 * h;
-#pragma unroll
-      for (int j = 0; j < 4 * NT; ++j)
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int gj = b_col0 + 8 * j + 2 * t + e;
-          if (gi < p.m && gj < p.n) {
-            float x = p.alpha * acc[4 * j + 2 * h + e];
-            if (p.D) x += p.beta * p.D[(size_t)gi * p.ldd + gj];
-            if (p.E) x += p.gamma * p.E[(size_t)gi * p.lde + gj];
-            p.C[(size_t)gi * p.ldc + gj] = x;
-          }
-        }
-    }
-    return;
-  }
   float* out = p.partial + ((size_t)split * p.num_tiles + tile_id) * 128 * (size_t)p.tn;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -939,23 +910,21 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
   if constexpr (BF16) {  // tn = 128
     if constexpr (F8) {
       if (p.fold > 1)
-        gram_tc_consumer_bf16<__half, T16>(p, stage_base, raw_bar, empty_bar, iters, a_box, tile_id, split, a_col0,
-                                           b_col0);
+        gram_tc_consumer_bf16<__half, T16>(p, stage_base, raw_bar, empty_bar, iters, a_box, tile_id, split);
       else
-        gram_tc_consumer_bf16<__half>(p, stage_base, full_bar, empty_bar, iters, a_box, tile_id, split, a_col0, b_col0);
+        gram_tc_consumer_bf16<__half>(p, stage_base, full_bar, empty_bar, iters, a_box, tile_id, split);
     } else {
-      gram_tc_consumer_bf16<T16>(p, stage_base, full_bar, empty_bar, iters, a_box, tile_id, split, a_col0, b_col0);
+      gram_tc_consumer_bf16<T16>(p, stage_base, full_bar, empty_bar, iters, a_box, tile_id, split);
     }
     return;
   } else if constexpr (BLOCKED) {  // tn == 256; A inside B: its k8 slices are rows of B's (8 KB apart), else 128-row slices in slot 8
     gram_tc_consumer_blocked(p, stage_base, full_bar, empty_bar, iters,
                              a_in_b ? (a_col0 - b_col0) * 32 : 8 * TC_BOX_BYTES, a_in_b ? 256 * 32 : 128 * 32, tile_id,
-                             split, a_col0, b_col0);
+                             split);
     return;
   } else {
 #define TNB_GRAM_CONSUME(NT)                                                                                          \
-  gram_tc_consumer<NT>(p, stage_base, tb_base, full_bar, empty_bar, tb_full, tb_empty, iters, a_box, tile_id, split, \
-                       a_col0, b_col0)
+  gram_tc_consumer<NT>(p, stage_base, tb_base, full_bar, empty_bar, tb_full, tb_empty, iters, a_box, tile_id, split)
   switch (nbox_b) {
     case 1: TNB_GRAM_CONSUME(1); break;
     case 2: TNB_GRAM_CONSUME(2); break;
@@ -1083,12 +1052,6 @@ inline void gram_tc_plan(int64_t rows, int64_t n, GramTcParams& p, int64_t m_col
   p.partial = nullptr;
   p.fold = 1;
   p.n_orig = (int)n;
-  p.direct = 0;
-  p.C = nullptr;
-  p.D = p.E = nullptr;
-  p.ldc = p.ldd = p.lde = 0;
-  p.alpha = 1.f;
-  p.beta = p.gamma = 0.f;
 }
 
 // Narrow matrices (n = 32 or 64) are viewed as (rows/f) x 128, f = 128/n: one full-width 128 x 128 tile with
@@ -1261,22 +1224,14 @@ inline size_t atb_tc_workspace_bytes(int64_t K, int64_t m, int64_t n) {
 
 inline int atb_tc_f32(const float* A, int64_t K, int64_t m, const float* B, int64_t n, float* C, int ldc, float alpha,
                       const float* D, int ldd, float beta, const float* E, int lde, float gamma, void* ws,
-                      size_t ws_bytes, cudaStream_t st, bool narrow = false) {
+                      size_t ws_bytes, cudaStream_t st) {
   if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "atb_tc: TMA tensor-core path needs an sm_90 device");
   if (!atb_tc_shape_ok(K, m, n)) return fail(TNB_ERR_UNSUPPORTED, "atb_tc: unsupported shape K=%lld m=%lld n=%lld", (long long)K, (long long)m, (long long)n);
   if (((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(B)) & 15u) != 0)
     return fail(TNB_ERR_INVALID, "atb_tc: operands must be 16-byte aligned");
   GramTcParams p;
   gram_tc_plan(K, n, p, m);
-  if (narrow) {  // one CTA per output tile, epilogue writes C directly
-    p.ksplit = 1;
-    p.iters_per_split = p.iters_total;
-    p.direct = 1;
-    p.C = C; p.ldc = ldc; p.alpha = alpha;
-    p.D = beta != 0.f ? D : nullptr; p.ldd = ldd; p.beta = beta;
-    p.E = gamma != 0.f ? E : nullptr; p.lde = lde; p.gamma = gamma;
-  }
-  const size_t need = narrow ? 0 : (size_t)p.ksplit * p.num_tiles * 128 * p.tn * sizeof(float);
+  const size_t need = (size_t)p.ksplit * p.num_tiles * 128 * p.tn * sizeof(float);
   if (ws_bytes < need) return fail(TNB_ERR_WORKSPACE, "atb_tc: workspace %zu < %zu", ws_bytes, need);
   p.partial = static_cast<float*>(ws);
   CUtensorMap ta, tb;
@@ -1287,7 +1242,6 @@ inline int atb_tc_f32(const float* A, int64_t K, int64_t m, const float* B, int6
   dim3 grid((unsigned)p.num_tiles, (unsigned)p.ksplit);
   gram_tc_kernel<TC_ROWMAJOR><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(ta, tb, p);
   TNB_LAUNCH_CHECK();
-  if (narrow) return TNB_OK;
   const int64_t total = m * n;
   atb_tc_finalize_kernel<<<(unsigned)std::min<int64_t>((total + 255) / 256, 4096), 256, 0, st>>>(p, C, ldc, alpha, D, ldd,
                                                                                                  beta, E, lde, gamma);

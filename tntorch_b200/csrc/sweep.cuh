@@ -243,7 +243,6 @@ inline int eig_run(const double* G, const TBk* Gb_in, int64_t L, EigWork<TBk>& e
   if (!e.chfsi) return jacobi2_eigh(G, (int)L, (int)L, e.w, e.V, e.jscratch, e.jinfo, st, fp32_solve, fp32_solve ? 2e-7 : 0.0);
   e.cw.use_tc = allow_tc;
   e.cw.shared_gpu = shared_gpu;
-  e.cw.narrow = shared_gpu && getenv("TNB_NARROW") != nullptr;
   e.k_run = (k_try > 0 && k_try < e.k) ? k_try : e.k;
   e.b_run = chfsi_default_block((int)L, e.k_run);
   if (e.b_run > e.b) e.b_run = e.b;
