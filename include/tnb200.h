@@ -79,7 +79,8 @@ int tnb_has_tensorcore_path(void);
  *   cores      output buffer; core k is written at element offset core_offsets_host[k] with shape
  *              [ranks_host[k], shape[k], ranks_host[k+1]]; capacity from tnb_ttsvd_cores_capacity()
  *   ranks_host ndim+1 ints (host), ranks_host[0] = ranks_host[ndim] = 1
- *   info_host  optional (may be NULL) 32 doubles: [0]=||T||_F, [1]=#eig solves, [2]=#ChFSI matrix products,
+ *   info_host  optional (may be NULL) 32 doubles: [0]=||T||_F from the trace of step 0's Gram (shrunk behind a
+ *              tensor-core Gram, see tnb_ttsvd_batch's norms_host; tnb_ttsvd_stream sums the squares exactly), [1]=#eig solves, [2]=#ChFSI matrix products,
  *              [3]=#tensor-core Gram launches; with TNB_FLAG_PROFILE also [4]=Gram ms, [5]=eigen ms,
  *              [6]=factor/projection ms (totals), [7]=#steps, [8+3t..10+3t]=the same three for step t < 6;
  *              [26]=1 when the speculative (single-synchronisation) sweep was accepted, [27]=the device flags that
@@ -107,7 +108,12 @@ int tnb_ttsvd(int dtype, const void* data, int ndim, const int64_t* shape, const
  *                       then the eigen stages of all tensors interleaved, then every projection) and synchronised ONCE; `stream` is forked from
  *                       and joined to.  tnb_ttsvd_batch_workspace_bytes() returns the recommended size (8 in flight)
  *                       and, through per_tensor_bytes, the unit.
- *   norms_host          optional, batch doubles: ||T_i||_F
+ *   norms_host          optional, batch doubles: ||T_i||_F as the square root of the trace of step 0's Gram
+ *                       (info_host[0] of tnb_ttsvd), not a separate pass over the input: exact to rounding after an
+ *                       exact-product Gram, shrunk by
+ *                       the tensor-core Gram's operand truncation and fp32 accumulation otherwise: the trace is
+ *                       (1 - c) ||T_i||^2, so the norm is (1 - c)^(1/2) ||T_i||, about c / 2 below it (c ~ 7e-4 to
+ *                       1.1e-3 for TF32 on fp32 input, below 2e-6 for 16-bit and fp8 input)
  *   speculative_host    optional, batch ints: 1 if tensor i was accepted from the single-synchronisation sweep
  * Tensors need rank caps on every bond for the in-flight path (see TNB_FLAG_NO_SPECULATE); otherwise, and for tensors
  * whose speculation the device rejected, the decomposition runs one tensor at a time like tnb_ttsvd.

@@ -151,8 +151,9 @@ inline std::atomic<int>& reserved_sms_ref() {
   static std::atomic<int> r{0};
   return r;
 }
+inline int device_sms() { return device_info().valid ? device_info().sm_count : 132; }
 inline int usable_sms() {
-  const int sms = device_info().valid ? device_info().sm_count : 132;
+  const int sms = device_sms();
   int r = reserved_sms_ref().load(std::memory_order_relaxed);
   if (r < 0) r = 0;
   if (r > sms - 8) r = sms - 8;

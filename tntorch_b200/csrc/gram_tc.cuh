@@ -1013,8 +1013,29 @@ inline bool gram_tc_shape_ok(int64_t rows, int64_t n) {
   return n >= 16 && n % 4 == 0 && n <= 16384 && rows >= 1 && rows < ((int64_t)1 << 31) - 64;
 }
 
-// max_tn: widest column tile (256; 128 for the bf16 mode)
-inline void gram_tc_plan(int64_t rows, int64_t n, GramTcParams& p, int64_t m_cols = -1, int max_tn = 256) {
+// split-K factor for cnt tiles of iters_total stages on sms SMs: at least sms / cnt and enough splits that no fp32
+// accumulation chain is longer than TC_MAX_SPLIT_ITERS stages (the splits are summed in fp64), then up to 8x that if it
+// fills the last wave of CTAs better while every split keeps >= 64 stages (72 tiles of 262144 rows on 128 SMs: 16
+// splits, 9 full waves)
+inline int64_t gram_tc_ksplit(int64_t iters_total, int cnt, int sms) {
+  const int64_t base = std::max<int64_t>(cnt < sms ? sms / cnt : 1, (iters_total + TC_MAX_SPLIT_ITERS - 1) / TC_MAX_SPLIT_ITERS);
+  int64_t ks = base;
+  double best = 0.0;
+  for (int64_t k = base; k <= 8 * base && k <= iters_total && (k == base || 64 * k <= iters_total); ++k) {
+    const int64_t ctas = k * cnt, waves = (ctas + sms - 1) / sms;
+    const double eff = (double)ctas / (double)(waves * sms);
+    if (eff > best + 0.02) { best = eff; ks = k; }
+  }
+  return std::min(ks, iters_total);
+}
+
+// max_tn: widest column tile (256; 128 for the bf16 mode).  sms: the SMs the kernel may fill (usable_sms()).  The
+// split-K scratch is carved for the whole device's factor (gram_tc_workspace_bytes), so a workspace sized under one
+// tnb_set_reserved_sms() count fits a run under any other: with SMs reserved the factor is clamped to the whole
+// device's.  The factor is not monotone in the SM count (2^24 x 64 folded: 32.7 MiB of scratch at 132 SMs, 32.0 at 128,
+// 38.5 at 124).
+inline void gram_tc_plan(int64_t rows, int64_t n, GramTcParams& p, int64_t m_cols = -1, int max_tn = 256,
+                         int sms = usable_sms()) {
   p.rows = rows;
   p.n = (int)n;
   p.symmetric = m_cols < 0 ? 1 : 0;
@@ -1033,19 +1054,8 @@ inline void gram_tc_plan(int64_t rows, int64_t n, GramTcParams& p, int64_t m_col
   }
   p.num_tiles = cnt;
   p.iters_total = (rows + TC_KC - 1) / TC_KC;
-  // split-K factor: at least sms / cnt and enough splits that no fp32 accumulation chain is longer than
-  // TC_MAX_SPLIT_ITERS stages (the splits are summed in fp64), then up to 8x that if it fills the last wave of CTAs better
-  // while every split keeps >= 64 stages (72 tiles of 262144 rows on 128 SMs: 16 splits, 9 full waves)
-  const int sms = usable_sms();
-  const int64_t base = std::max<int64_t>(cnt < sms ? sms / cnt : 1, (p.iters_total + TC_MAX_SPLIT_ITERS - 1) / TC_MAX_SPLIT_ITERS);
-  int64_t ks = base;
-  double best = 0.0;
-  for (int64_t k = base; k <= 8 * base && k <= p.iters_total && (k == base || 64 * k <= p.iters_total); ++k) {
-    const int64_t ctas = k * cnt, waves = (ctas + sms - 1) / sms;
-    const double eff = (double)ctas / (double)(waves * sms);
-    if (eff > best + 0.02) { best = eff; ks = k; }
-  }
-  if (ks > p.iters_total) ks = p.iters_total;
+  int64_t ks = gram_tc_ksplit(p.iters_total, cnt, sms);
+  if (sms != device_sms()) ks = std::min(ks, gram_tc_ksplit(p.iters_total, cnt, device_sms()));
   p.iters_per_split = (p.iters_total + ks - 1) / ks;
   ks = (p.iters_total + p.iters_per_split - 1) / p.iters_per_split;
   p.ksplit = (int)ks;
@@ -1066,7 +1076,7 @@ inline int gram_tc_fold(int64_t rows, int64_t n) {
 inline size_t gram_tc_workspace_bytes(int64_t rows, int64_t n, int max_tn = 256) {
   GramTcParams p;
   const int f = gram_tc_fold(rows, n);
-  gram_tc_plan(rows / f, n * f, p, -1, max_tn);
+  gram_tc_plan(rows / f, n * f, p, -1, max_tn, device_sms());
   return align_up((size_t)p.ksplit * p.num_tiles * 128 * p.tn * sizeof(float));
 }
 
@@ -1218,7 +1228,7 @@ inline bool atb_tc_shape_ok(int64_t K, int64_t m, int64_t n) {
 }
 inline size_t atb_tc_workspace_bytes(int64_t K, int64_t m, int64_t n) {
   GramTcParams p;
-  gram_tc_plan(K, n, p, m);
+  gram_tc_plan(K, n, p, m, 256, device_sms());
   return align_up((size_t)p.ksplit * p.num_tiles * 128 * p.tn * sizeof(float));
 }
 

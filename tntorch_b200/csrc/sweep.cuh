@@ -648,11 +648,13 @@ inline int truncate_step(ArenaT& ar, bool dry, const StepCtx& cx, const TIn* C, 
   if (first_step && cx.info) cx.info->norm = std::sqrt(hs->norm2 > 0 ? hs->norm2 : 0.0);
   int64_t rank = hs->rank;
   if (rank > kcap) rank = kcap;
-  if (hs->zero_flag) {  // round.py:137-145: rank-1 zero factors
-    rank = 1;
-    fill_kernel<T><<<grid_for(n), 256, 0, st>>>(core, n, (T)0);
+  if (hs->zero_flag) {
+    // round.py:137-145: rank-1 zero factors; the batch rank rule (round.py:149-150) has no zero branch and keeps
+    // rank = min(rmax, L), so a zero sample's factors are zero at that rank, like the other samples' of its batch
+    if (!batch_mode) rank = 1;
+    fill_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(core, n * rank, (T)0);
     TNB_LAUNCH_CHECK();
-    fill_kernel<T><<<grid_for(rows), 256, 0, st>>>(Cn, rows, (T)0);
+    fill_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(Cn, rows * rank, (T)0);
     TNB_LAUNCH_CHECK();
   } else {
     TNB_TRY((step_factors<T, TIn>(cx, C, rows, n, rank, ew.w, ew.V, ew.ldv, fac, ww, ptc_ws, ptc_bytes, core, Cn)));
@@ -1425,11 +1427,11 @@ inline int ttsvd_stream_impl(ArenaT& ar, bool dry, const TIn* host, const SweepD
     }
     int64_t rank = std::min<int64_t>(hs->rank, kcap);
     T* core = cores + d.slot[mu];
-    if (hs->zero_flag) {  // round.py:137-145: rank-1 zero factors
-      rank = 1;
-      fill_kernel<T><<<grid_for(n), 256, 0, st>>>(core, n, (T)0);
+    if (hs->zero_flag) {  // round.py:137-145: rank-1 zero factors (zero factors at the rank cap under the batch rule)
+      if (!batch_mode) rank = 1;
+      fill_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(core, n * rank, (T)0);
       TNB_LAUNCH_CHECK();
-      fill_kernel<T><<<grid_for(rows), 256, 0, st>>>(carry0, rows, (T)0);
+      fill_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(carry0, rows * rank, (T)0);
       TNB_LAUNCH_CHECK();
     } else {
       c0.kblocked = kb_ok && spec_tail && rank == kcap;
