@@ -440,6 +440,29 @@ size_t tnb_tt_decompress_workspace_bytes(int core_dtype, int out_dtype, int ndim
 int tnb_tt_decompress(int core_dtype, int out_dtype, const void* const* cores, int ndim, const int64_t* shape,
                       const int32_t* ranks, void* out, void* workspace, size_t workspace_bytes, void* stream);
 
+/* TT-matrix times a batch: Y (batch x O) = X (batch x I) M, where M (I = prod input_dims rows, O = prod output_dims
+ * columns, both indexed row-major over their modes) is given by d cores, core k ranks[k] x input_dims[k] x
+ * output_dims[k] x ranks[k+1] (row-major), and is never formed.  X and Y are row-major; X is read in place.
+ * Stream-ordered, no host synchronisation, no allocation.  dtype TNB_F32 or TNB_F64 (X, Y and the cores); any other
+ * dtype returns TNB_ERR_UNSUPPORTED and sizes to 0.  ranks has d + 1 entries with ranks[0] == ranks[d] == 1;
+ * 1 <= d <= 64, every dim and rank >= 1, batch >= 1 (else TNB_ERR_INVALID); batch < 2^31 and X, Y, every core and every
+ * intermediate within 2^46 elements (else TNB_ERR_UNSUPPORTED).  Null pointers are TNB_ERR_INVALID, a workspace below
+ * tnb_tt_multiply_workspace_bytes TNB_ERR_WORKSPACE, all before anything is launched.
+ * d steps, one launch each: step k contracts (i_k, r_k) of the running intermediate (batch index outermost, then
+ * i_k .. i_{d-1}, o_0 .. o_{k-1}, r_k) with core k.  A step runs on the tensor cores at fp32 accuracy (3xTF32) when the
+ * cores are fp32, 4 <= r_k <= 256 with r_k % 4 == 0, o_k r_{k+1} is even, the step has at least 64 rows per batch element
+ * and 2^20 output elements and (last step) Y is 8-byte aligned; on the generic CUDA-core tiles otherwise, which includes
+ * step 0 (r_0 = 1) and every fp64 step.  When some step runs on the tensor cores, one more launch first writes the TF32
+ * hi / lo images of those cores.
+ * The workspace holds two ping-pong intermediates of the largest step output (one when d == 2, none when d == 1) and the
+ * cores' TF32 images; never M and never a copy of X.  Its size does not depend on the pointers.
+ * Replaces: tntorch.tt_multiply matrix.py:420-443 (X.T and one torch.einsum per core). */
+size_t tnb_tt_multiply_workspace_bytes(int dtype, int d, const int64_t* input_dims, const int64_t* output_dims,
+                                       const int32_t* ranks, int64_t batch);
+int tnb_tt_multiply(int dtype, const void* const* cores, int d, const int64_t* input_dims, const int64_t* output_dims,
+                    const int32_t* ranks, const void* X, int64_t batch, void* Y, void* workspace, size_t workspace_bytes,
+                    void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -127,6 +127,9 @@ SIGNATURES = {
     "tnb_tt_relative_error": (C.c_int, [C.c_int, _vp, C.POINTER(_vp), C.c_int, _i64p, _i32p, _vp, C.c_size_t, _f64p, _vp]),
     "tnb_tt_decompress_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, _i64p, _i32p]),
     "tnb_tt_decompress": (C.c_int, [C.c_int, C.c_int, C.POINTER(_vp), C.c_int, _i64p, _i32p, _vp, _vp, C.c_size_t, _vp]),
+    "tnb_tt_multiply_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, _i64p, _i64p, _i32p, C.c_int64]),
+    "tnb_tt_multiply": (C.c_int, [C.c_int, C.POINTER(_vp), C.c_int, _i64p, _i64p, _i32p, _vp, C.c_int64, _vp, _vp,
+                                  C.c_size_t, _vp]),
 }
 
 

@@ -4,9 +4,11 @@
   hadamard_sum  metrics.py:321-450    sum of the elementwise product of K tensors, re-rounding the running product
   shift_mode    tools.py:650-697      move one mode through a TT, one truncated_svd per position
   TTMatrix      matrix.py:12-140      matrix -> d-way (i_k x o_k) tensor -> TT-SVD (plain or batched)
+  tt_multiply   matrix.py:420-443     X @ M for a TTMatrix M, one library call that never forms M
 
-Only the parts that sit on the hot path are mirrored (construction, decompression, the re-rounding loops); the
-TT-matrix algebra (kron det/inv, tt_multiply) stays out of scope (DESIGN.md §9)."""
+Only the parts that sit on the hot path are mirrored (construction, decompression, the product with a batch, the
+re-rounding loops); the rest of the TT-matrix algebra (trace, det, inv, cholesky, CPMatrix) stays out of scope
+(DESIGN.md §7)."""
 from __future__ import annotations
 
 import math
@@ -151,3 +153,27 @@ class TTMatrix:
 
     def numpy(self):
         return self.torch().detach().cpu().numpy()
+
+
+def _tt_multiply_einsum(tt_matrix: TTMatrix, tensor: torch.Tensor) -> torch.Tensor:
+    """The reference's chain (matrix.py:432-443): X.T, then one einsum per core.  The differentiable path."""
+    idims = tt_matrix.input_dims.tolist()
+    b = tensor.reshape(-1, math.prod(idims)).shape[0]
+    result = tensor.reshape(b, -1).T.reshape(idims[0], -1)
+    result = torch.einsum("id,lior->ldor", result, tt_matrix.cores[0])
+    for k in range(1, tt_matrix.d):
+        result = result.reshape(idims[k], -1, tt_matrix.cores[k].shape[0])
+        result = torch.einsum("idr,riob->dob", result, tt_matrix.cores[k])
+    return result.reshape(b, -1)
+
+
+def tt_multiply(tt_matrix: TTMatrix, tensor: torch.Tensor) -> torch.Tensor:
+    """tntorch.tt_multiply (matrix.py:420-443): `tensor` viewed as [b, I] times the TT-matrix, a fresh [b, O] tensor in
+    the cores' dtype.  On the device (ops.tt_multiply, tnb_tt_multiply) unless `tensor` or a core requires grad, which
+    runs the reference's einsum chain in torch so that autograd sees it."""
+    assert len(tensor.shape) > 1
+    if tt_matrix.batch:
+        raise NotImplementedError("tt_multiply: batched TT-matrices are not supported")
+    if tensor.requires_grad or any(c.requires_grad for c in tt_matrix.cores):
+        return _tt_multiply_einsum(tt_matrix, tensor)
+    return ops.tt_multiply(tt_matrix.cores, tensor)

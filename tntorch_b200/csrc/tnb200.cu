@@ -14,6 +14,7 @@
 #include "cross_kernels.cuh"
 #include "peak_tf32.cuh"
 #include "expand_tc.cuh"
+#include "tt_multiply.cuh"
 
 using namespace tnb;
 
@@ -994,6 +995,35 @@ int tnb_tt_decompress(int core_dtype, int out_dtype, const void* const* cores, i
     return fail(TNB_ERR_WORKSPACE, "tnb_tt_decompress: workspace too small");
   Arena ar(workspace, workspace_bytes);
   return tt_decompress_dispatch(ar, false, core_dtype, out_dtype, cores, ndim, shape, ranks, out, as_stream(stream));
+}
+
+// ------------------------------------------------------------------ TT-matrix times a batch
+size_t tnb_tt_multiply_workspace_bytes(int dtype, int d, const int64_t* input_dims, const int64_t* output_dims,
+                                       const int32_t* ranks, int64_t batch) {
+  if ((dtype != TNB_F32 && dtype != TNB_F64) || !input_dims || !output_dims || !ranks ||
+      ttm_check_dims(d, input_dims, output_dims, ranks, batch) != TNB_OK)
+    return 0;
+  ArenaSizer ar;
+  if (tt_multiply_dispatch(ar, true, dtype, nullptr, d, input_dims, output_dims, ranks, nullptr, batch, nullptr, 0) != TNB_OK)
+    return 0;
+  return ar.off > 256 ? ar.off : 256;  // never 0 for a supported call: 0 is the refusal
+}
+
+int tnb_tt_multiply(int dtype, const void* const* cores, int d, const int64_t* input_dims, const int64_t* output_dims,
+                    const int32_t* ranks, const void* X, int64_t batch, void* Y, void* workspace, size_t workspace_bytes,
+                    void* stream) {
+  if (dtype != TNB_F32 && dtype != TNB_F64)
+    return fail(TNB_ERR_UNSUPPORTED, "tnb_tt_multiply: dtype %d is not built (TNB_F32, TNB_F64)", dtype);
+  if (!cores || !input_dims || !output_dims || !ranks || !X || !Y || !workspace)
+    return fail(TNB_ERR_INVALID, "tnb_tt_multiply: null argument");
+  TNB_TRY(ttm_check_dims(d, input_dims, output_dims, ranks, batch));
+  for (int k = 0; k < d; ++k)
+    if (!cores[k]) return fail(TNB_ERR_INVALID, "tnb_tt_multiply: core %d is null", k);
+  TNB_TRY(require_device());
+  if (workspace_bytes < tnb_tt_multiply_workspace_bytes(dtype, d, input_dims, output_dims, ranks, batch))
+    return fail(TNB_ERR_WORKSPACE, "tnb_tt_multiply: workspace too small");
+  Arena ar(workspace, workspace_bytes);
+  return tt_multiply_dispatch(ar, false, dtype, cores, d, input_dims, output_dims, ranks, X, batch, Y, as_stream(stream));
 }
 
 }  // extern "C"

@@ -1124,3 +1124,54 @@ def tt_decompress(cores: Sequence[torch.Tensor], dtype: Optional[torch.dtype] = 
     with torch.cuda.device(c0.device):
         check(L.tnb_tt_decompress(code, ocode, ptrs, N, sh, rk, _ptr(out), _ptr(ws), wsb, _stream()))
     return out
+
+
+def tt_multiply(cores: Sequence[torch.Tensor], X: torch.Tensor) -> torch.Tensor:
+    """Y = X.reshape(-1, I) @ M for the TT-matrix M of cores [r_k, i_k, o_k, r_{k+1}] (one dtype, one CUDA device,
+    boundary ranks 1), in one library call (tnb_tt_multiply) that never forms M: stream-ordered, no host
+    synchronisation.  Returns a fresh [b, O] tensor in the cores' dtype (I = prod i_k, O = prod o_k).  X must have at
+    least two dimensions and the cores' dtype and device; it is read in place when it is contiguous."""
+    cores = list(cores)
+    if cores and any(c.dim() == 5 for c in cores):
+        raise NotImplementedError("tt_multiply: batched TT-matrices (5-D cores) are not supported")
+    if not cores or any(c.dim() != 4 for c in cores):
+        raise ValueError("tt_multiply: cores must be 4-D tensors [r, i, o, r']")
+    c0 = cores[0]
+    _require_cuda(c0, "tt_multiply")
+    if any(c.dtype != c0.dtype or c.device != c0.device for c in cores):
+        raise ValueError("tt_multiply: cores must share one dtype and one device")
+    ranks = [c0.shape[0]] + [c.shape[3] for c in cores]
+    if ranks[0] != 1 or ranks[-1] != 1:
+        raise ValueError(f"tt_multiply: boundary ranks must be 1, got {ranks[0]} and {ranks[-1]}")
+    if any(a.shape[3] != b.shape[0] for a, b in zip(cores[:-1], cores[1:])):
+        raise ValueError("tt_multiply: core ranks do not match")
+    assert X.dim() > 1
+    if X.dtype != c0.dtype:
+        raise RuntimeError(f"tt_multiply: X is {X.dtype} but the cores are {c0.dtype}")
+    if X.device != c0.device:
+        raise RuntimeError(f"tt_multiply: X is on {X.device} but the cores are on {c0.device}")
+    code = _dtype_code(c0)
+    idims, odims = [c.shape[1] for c in cores], [c.shape[2] for c in cores]
+    I = 1
+    for n in idims:
+        I *= n
+    O = 1
+    for n in odims:
+        O *= n
+    X = X.reshape(-1, I).contiguous()
+    b = X.shape[0]
+    Y = torch.empty(b, O, dtype=c0.dtype, device=c0.device)
+    if b == 0:
+        return Y
+    cores = [c.contiguous() for c in cores]
+    d = len(cores)
+    L = lib()
+    ii, oo, rk = i64(idims), i64(odims), i32(ranks)
+    wsb = L.tnb_tt_multiply_workspace_bytes(code, d, ii, oo, rk, b)
+    if wsb == 0:
+        check(_lib.ERR_UNSUPPORTED)
+    ws = _ws(wsb, c0.device)
+    ptrs = (C.c_void_p * d)(*[c.data_ptr() for c in cores])
+    with torch.cuda.device(c0.device):
+        check(L.tnb_tt_multiply(code, ptrs, d, ii, oo, rk, _ptr(X), b, _ptr(Y), _ptr(ws), wsb, _stream()))
+    return Y
