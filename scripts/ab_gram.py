@@ -1,13 +1,16 @@
 """A/B of two builds of this repository on one GPU: bench.py alternating between them, their outputs on the same seeded
 input, and the TF32 noise floor of their Gram kernels.
 
-    python scripts/ab_gram.py OTHER_TREE --out DIR [--runs 3] [--steps 5] [--warmup 3]
+    python scripts/ab_gram.py OTHER_TREE --out DIR [--runs 3] [--steps 5] [--warmup 3] [--skip-noise]
 
 OTHER_TREE is a second checkout with its library already built (e.g. the parent commit).  Every bench.py run is a fresh
-process; the JSON written to DIR/ab_gram.json holds, per run, value, ms_per_step, phases_ms.gram_ms, the roofline,
-sweep_roofline.single_call_ms and run.speculative_sweeps_accepted, plus the card's name and power limit.  Gram noise:
-||G_tf32 - (1 - c) G_fp64||_2 / ||G_fp64||_2 on randn(262144, 2048), c the least-squares truncation bias, for the
-row-major Gram and, where the build has it, the Gram of the same matrix stored K-blocked.
+process, alternating the two builds; the JSON written to DIR/ab_gram.json holds, per run, value, ms_per_step,
+phases_ms.gram_ms, the roofline, sweep_roofline.single_call_ms and run.speculative_sweeps_accepted, plus the card's name
+and power limit; its summary gives per build the median, min, max and spread of value and of each step's Gram time,
+and whether every sweep was speculative.  Outputs: whether the dumped cores of the seeded bench input are bitwise equal
+between the builds.  Gram noise: ||G_tf32 - (1 - c) G_fp64||_2 / ||G_fp64||_2 on randn(262144, 2048), c the
+least-squares truncation bias, for the row-major Gram and, where the build has it, the Gram of the same matrix stored
+K-blocked; the two builds' G of each kind are also compared bitwise.
 """
 import argparse
 import json
@@ -19,7 +22,7 @@ import sys
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def gram_noise(tree):
+def gram_noise(tree, save_dir):
     sys.path.insert(0, tree)
     import torch
 
@@ -35,6 +38,7 @@ def gram_noise(tree):
     del A64
     out = {"tree": tree}
     for k, G in grams.items():
+        torch.save(G.cpu(), os.path.join(save_dir, f"G_{k}.pt"))
         c = 1.0 - float((G * ref).sum() / (ref * ref).sum())
         E = G - (1.0 - c) * ref
         noise = float(torch.linalg.matrix_norm(E, ord=2) / torch.linalg.matrix_norm(ref, ord=2))
@@ -59,6 +63,11 @@ def bench(tree, args, dump):
             "rel_error_twin": res.get("rel_error_twin")}
 
 
+def _bytes(path):
+    with open(path, "rb") as f:
+        return f.read()
+
+
 def compare_dumps(a, b):
     import numpy as np
 
@@ -75,12 +84,28 @@ def compare_dumps(a, b):
             continue
         # cores agree up to the sign of each rank-one pair; compare magnitudes
         worst = max(worst, float(np.abs(np.abs(x) - np.abs(y)).max() / max(np.abs(x).max(), 1e-30)))
-    return {"same_files": True, "core_shapes_equal": shapes_equal, "max_rel_abs_core_diff": worst}
+    bitwise = all(_bytes(os.path.join(a, f)) == _bytes(os.path.join(b, f)) for f in fa)
+    return {"same_files": True, "core_shapes_equal": shapes_equal, "max_rel_abs_core_diff": worst,
+            "bitwise_equal": bitwise}
+
+
+def spread(xs):
+    return {"median": statistics.median(xs), "min": min(xs), "max": max(xs), "spread": max(xs) - min(xs)}
+
+
+def same_grams(a, b):
+    import torch
+
+    out = {}
+    for f in sorted(os.listdir(a)):
+        if f.startswith("G_") and os.path.exists(os.path.join(b, f)):
+            out[f[2:-3] + "_bitwise_equal"] = bool(torch.equal(torch.load(os.path.join(a, f)), torch.load(os.path.join(b, f))))
+    return out
 
 
 def main():
-    if len(sys.argv) > 2 and sys.argv[1] == "--noise":
-        print(json.dumps(gram_noise(sys.argv[2])))
+    if len(sys.argv) > 3 and sys.argv[1] == "--noise":
+        print(json.dumps(gram_noise(sys.argv[2], sys.argv[3])))
         return
     ap = argparse.ArgumentParser()
     ap.add_argument("other")
@@ -88,6 +113,7 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--out", required=True, help="directory for ab_gram.json and the dumped cores of both builds")
+    ap.add_argument("--skip-noise", action="store_true", help="skip the Gram noise measurement (two fp64 Grams per build)")
     args = ap.parse_args()
     other = os.path.abspath(args.other)
     args.out = os.path.abspath(args.out)  # bench.py runs in each tree's directory
@@ -103,17 +129,25 @@ def main():
             print(k, i, json.dumps({x: r[x] for x in ("value", "ms_per_step", "gram_ms", "factor_ms", "single_call_ms")}),
                   flush=True)
     noise = {}
-    for k, tree in trees.items():
-        out = subprocess.run([sys.executable, os.path.abspath(__file__), "--noise", tree], capture_output=True, text=True)
+    for k, tree in ({} if args.skip_noise else trees).items():
+        gdir = os.path.join(args.out, f"gram_{k}")
+        os.makedirs(gdir, exist_ok=True)
+        out = subprocess.run([sys.executable, os.path.abspath(__file__), "--noise", tree, gdir], capture_output=True,
+                             text=True)
         noise[k] = json.loads(out.stdout.strip().splitlines()[-1]) if out.returncode == 0 else {"error": out.stderr[-2000:]}
+    if not args.skip_noise:
+        noise["grams"] = same_grams(os.path.join(args.out, "gram_other"), os.path.join(args.out, "gram_this"))
     summary = {}
     for k in trees:
         v = [r["value"] for r in runs[k]]
-        summary[k] = {"median_value": statistics.median(v), "spread": max(v) - min(v),
+        summary[k] = {"median_value": statistics.median(v), "spread": max(v) - min(v), "value": spread(v),
                       "median_gram_ms": [statistics.median(r["gram_ms"][j] for r in runs[k]) for j in range(2)]
                       if runs[k][0]["gram_ms"] else None,
+                      "gram_ms": [spread([r["gram_ms"][j] for r in runs[k]]) for j in range(2)]
+                      if runs[k][0]["gram_ms"] else None,
                       "median_factor_ms": [statistics.median(r["factor_ms"][j] for r in runs[k]) for j in range(2)]
-                      if runs[k][0]["factor_ms"] else None}
+                      if runs[k][0]["factor_ms"] else None,
+                      "speculative_sweeps_accepted": [r["speculative_sweeps_accepted"] for r in runs[k]]}
     result = {"nvidia_smi": smi, "runs": runs, "summary": summary, "noise": noise,
               "dumps": compare_dumps(os.path.join(args.out, "dump_other"), os.path.join(args.out, "dump_this"))}
     json.dump(result, open(os.path.join(args.out, "ab_gram.json"), "w"), indent=1)

@@ -22,7 +22,11 @@
 // the next step.  Each 8 x 4 core matrix is 128 contiguous bytes and the 8 rows of a k8 step over 256 columns are one
 // contiguous 8 KB run, so TMA loads both operands (256-byte lines, no swizzle) straight into the layout tf32 wgmma reads
 // from shared memory: no transposers, A and B through descriptors, and the freed shared memory holds a
-// TC_BLK_STAGES-deep slab ring.  The 8 rows each k8 step sums are the same 8 rows as in the row-major mode.
+// TC_BLK_STAGES-deep slab ring.  The 8 rows each k8 step sums are the same 8 rows as in the row-major mode.  The tiles
+// 2j, 2j + 1 of a column tile run as a pair in a cluster of two CTAs that share their 256-column B strip: each CTA loads
+// half of every B stage into both by TMA multicast, and its own 128-column A strip (none on the diagonal, where A lies
+// inside B).  At 2048 columns that cuts the bytes read from L2 by a third (26.8 GB -> 17.2 GB for 262144 rows), which
+// is what feeds the tensor cores of this mode.
 //
 // bf16 mode (gram_tc_bf16): C is a row-major bf16 matrix (the dense TT-SVD's input).  wgmma takes 16-bit operands from
 // shared memory MN-major, so TMA loads boxes of 64 bf16 columns x TC_KC rows (128-byte rows, 128-byte swizzle) and both
@@ -163,6 +167,32 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* t
       :
       : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
+}
+// The same 3-D box written to the same shared-memory offset, and completing on the mbarrier at the same offset, in every
+// CTA of the cluster named in cta_mask.
+__device__ __forceinline__ void tma_load_3d_multicast(void* smem_dst, const CUtensorMap* tmap, uint64_t* bar, int c0,
+                                                      int c1, int c2, uint16_t cta_mask) {
+  asm volatile(
+      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%4, %5, %6}], [%2], %3;"
+      :
+      : "r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "h"(cta_mask), "r"(c0),
+        "r"(c1), "r"(c2)
+      : "memory");
+}
+// Arrive on the mbarrier at the same shared-memory offset as `bar` in cluster CTA `cta`.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}" ::"r"(smem_u32(bar)),
+      "r"(cta)
+      : "memory");
+}
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
 }
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
@@ -522,13 +552,15 @@ static_assert(TcRing<TC_BF16>::STAGES <= TC_MAX_RING && TcRing<TC_KBLOCKED>::STA
 
 // Loads of pipeline iteration `it` (rows it_begin + it) into its ring slot, once the transposers and the consumers have
 // released it.  B first (slots 0..nbox_b), then A (slots A_SLOT..).  Row-major: boxes of 32 columns.  bf16: boxes of 64
-// columns.  K-blocked: one box of (64, tn / 8 column groups, 4 row groups) for B and one of (64, 16, 4) for A, i.e.
-// four k8 slices of tn (128) columns x 32 bytes.  F8 (bf16 mode, fp8 input): boxes of 128 fp8 columns into the raw
-// slots TC_F8_RAW_SLOT (B) and TC_F8_RAW_SLOT + 1 (A), completing on `full_bar` = the converters' raw barriers.
+// columns.  K-blocked: B is four k8 slices of 256 columns x 32 bytes, shared by the two CTAs of a pair: CTA `rank` loads
+// slices 2 rank, 2 rank + 1 (one box of (64, 32 column groups, 2 row groups)) into both CTAs; A is one box of (64, 16,
+// 4), four k8 slices of 128 columns, loaded by each CTA for itself.  Either CTA's full barrier counts the whole B stage
+// and its own A.  F8 (bf16 mode, fp8 input): boxes of 128 fp8 columns into the raw slots TC_F8_RAW_SLOT (B) and
+// TC_F8_RAW_SLOT + 1 (A), completing on `full_bar` = the converters' raw barriers.
 template <int MODE, bool F8 = false>
 __device__ __forceinline__ void gram_tc_produce(const CUtensorMap* tmap, const CUtensorMap* tmap_b, unsigned char* stage_base,
                                                 uint64_t* full_bar, uint64_t* empty_bar, int64_t it, int64_t it_begin,
-                                                int nbox_a, int nbox_b, int a_col0, int b_col0) {
+                                                int nbox_a, int nbox_b, int a_col0, int b_col0, int rank = 0) {
   using R = TcRing<MODE>;
   constexpr int BOX_COLS = F8 ? 128 : R::BOX_COLS, B_SLOT = F8 ? TC_F8_RAW_SLOT : 0;
   constexpr int A_SLOT = F8 ? TC_F8_RAW_SLOT + 1 : R::A_SLOT;
@@ -539,7 +571,8 @@ __device__ __forceinline__ void gram_tc_produce(const CUtensorMap* tmap, const C
   mbar_expect_tx(&full_bar[stage], (uint32_t)(nbox_a + nbox_b) * TC_BOX_BYTES);
   const int row0 = (int)((it_begin + it) * TC_KC);
   if constexpr (MODE == TC_KBLOCKED) {
-    tma_load_3d(sb, tmap_b, &full_bar[stage], 0, b_col0 / 8, row0 / 8);
+    tma_load_3d_multicast(sb + rank * 4 * TC_BOX_BYTES, tmap_b, &full_bar[stage], 0, b_col0 / 8, row0 / 8 + 2 * rank,
+                          0x3);
     if (nbox_a) tma_load_3d(sb + 8 * TC_BOX_BYTES, tmap, &full_bar[stage], 0, a_col0 / 8, row0 / 8);
   } else {
     for (int j = 0; j < nbox_b; ++j)
@@ -699,10 +732,11 @@ __device__ __forceinline__ void gram_tc_consumer(const GramTcParams& p, const un
 }
 
 // Consumer warpgroup cw of the K-blocked mode (tn = 256): both operands through descriptors of the stage's k8 slices.  B slice kk is at kk * 8 KB; A (this warpgroup's 64 rows) at a_off + kk * a_slice + 64 * cw rows.  A slot is
-// released once the wgmma group that read it has completed, i.e. one stage later.
+// released once the wgmma group that read it has completed, i.e. one stage later, in this CTA and in the `peer` CTA of
+// the pair, whose producer writes half of its B into this CTA.  tile_id < 0: the pair's padding CTA, which writes nothing.
 __device__ __forceinline__ void gram_tc_consumer_blocked(const GramTcParams& p, const unsigned char* stage_base,
                                                          uint64_t* full_bar, uint64_t* empty_bar, int64_t iters,
-                                                         int a_off, int a_slice, int tile_id, int split) {
+                                                         int a_off, int a_slice, int tile_id, int split, uint32_t peer) {
   const int ct = threadIdx.x - 128;
   const int lane = ct & 31, w = (ct >> 5) & 3, cw = ct >> 7;
   const int cm = 64 * cw + 16 * w;
@@ -722,11 +756,14 @@ __device__ __forceinline__ void gram_tc_consumer_blocked(const GramTcParams& p, 
     wgmma_commit();
     wgmma_wait<1>();
     __syncwarp();
-    if (it > 0 && lane == 0) mbar_arrive(&empty_bar[(it - 1) % TC_BLK_STAGES]);
+    if (it > 0 && lane == 0) {
+      mbar_arrive(&empty_bar[(it - 1) % TC_BLK_STAGES]);
+      mbar_arrive_cluster(&empty_bar[(it - 1) % TC_BLK_STAGES], peer);
+    }
   }
   wgmma_wait<0>();
   wgmma_fence_operand(acc);
-  gram_tc_epilogue<8>(p, acc, cm, lane, tile_id, split);
+  if (tile_id >= 0) gram_tc_epilogue<8>(p, acc, cm, lane, tile_id, split);
 }
 
 // Consumer warpgroup cw of the bf16 mode (tn = 128): A (this warpgroup's 64 columns of C, box a_box + cw) and B (the
@@ -819,8 +856,18 @@ __device__ __forceinline__ void gram_tc_epilogue(const GramTcParams& p, const fl
   }
 }
 
+// K-blocked mode (symmetric, tn = 256): tile rows 2j and 2j + 1 keep the same column tiles, bn >= j, so the kept tiles
+// pair off as (2j, bn), (2j + 1, bn), numbered j-major then bn.  When the tile-row count is odd, the last row's pairs
+// (only bn = j there) end in a tile 2j + 1 past the matrix.  Both tiles of a pair read the same 256-column B strip.
+inline int gram_tc_num_pairs(int num_bm, int num_bn) {
+  int cnt = 0;
+  for (int j = 0; 2 * j < num_bm; ++j) cnt += num_bn - j;
+  return cnt;
+}
+
 // TC_KBLOCKED: the operands are K-blocked (see the top of the file); tmap / tmap_b are 3-D maps with boxes (64, 16, 4)
-// and (64, 32, 4).  TC_ROWMAJOR: row-major fp32, 2-D maps with boxes of 32 columns x TC_KC rows.  TC_BF16: row-major
+// and (64, 32, 2); the kernel runs in clusters of two CTAs, one pair of tiles (gram_tc_num_pairs) per cluster, blockIdx.x
+// = 2 pair + rank.  TC_ROWMAJOR: row-major fp32, 2-D maps with boxes of 32 columns x TC_KC rows.  TC_BF16: row-major
 // T16 (bf16 or fp16; the other modes ignore it), 2-D maps with boxes of 64 columns x TC_KC rows; T16 fp8 (e4m3 or
 // e5m2): UINT8 maps with boxes of 128 columns x TC_KC rows, widened to fp16 in shared memory.
 template <int MODE, typename T16 = __nv_bfloat16>
@@ -843,12 +890,19 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
   uint64_t* raw_bar = reinterpret_cast<uint64_t*>(tile_smem + 2);     // fp8 input: TMA -> converters
   static_assert((2 * TC_MAX_RING + 2 * TC_TB_STAGES + 1 + TC_MAX_RING) * 8 <= 256, "barriers must fit their 256 bytes");
 
-  const int tile_id = blockIdx.x, split = blockIdx.y;
+  const int split = blockIdx.y;
+  int tile_id = blockIdx.x;
+  const uint32_t rank = BLOCKED ? cluster_ctarank() : 0u;
 
   if (threadIdx.x == 0) {
     // flat tile id -> (bm, bn) among the tiles that touch the upper triangle
     int cnt = 0, fbm = 0, fbn = 0;
-    if (p.symmetric) {
+    if (BLOCKED) {  // pair blockIdx.x / 2 -> (j, bn); this CTA's tile row 2j + rank
+      int q = blockIdx.x >> 1, j = 0;
+      while (q >= p.num_bn - j) q -= p.num_bn - j++;
+      fbm = 2 * j + (int)rank;
+      fbn = j + q;
+    } else if (p.symmetric) {
       for (int bm = 0; bm < p.num_bm; ++bm)
         for (int bn = 0; bn < p.num_bn; ++bn)
           if ((bn + 1) * p.tn > bm * 128) {
@@ -864,8 +918,8 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
     for (int s = 0; s < TcRing<MODE>::STAGES; ++s) {
       mbar_init(&full_bar[s], F8 ? TC_TRANSPOSE_THREADS : 1);  // fp8: the converters, per thread
       if constexpr (F8) mbar_init(&raw_bar[s], 1);
-      // per warp: transposers and consumers (K-blocked, bf16: consumers only)
-      mbar_init(&empty_bar[s], (MODE == TC_ROWMAJOR ? TC_TRANSPOSE_THREADS / 32 : 0) + 8);
+      // per warp: transposers and consumers (bf16: consumers only; K-blocked: the consumers of both CTAs of the pair)
+      mbar_init(&empty_bar[s], MODE == TC_ROWMAJOR ? TC_TRANSPOSE_THREADS / 32 + 8 : BLOCKED ? 16 : 8);
     }
     for (int b = 0; b < TC_TB_STAGES; ++b) {
       mbar_init(&tb_full[b], TC_TRANSPOSE_THREADS);  // per thread: each orders its own stores for the async proxy
@@ -873,9 +927,18 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  __syncthreads();
+  // K-blocked: the peer CTA multicasts into this CTA's ring and arrives on its empty barriers
+  if constexpr (BLOCKED)
+    cluster_sync_all();
+  else
+    __syncthreads();
 
   const int bm = tile_smem[0], bn = tile_smem[1];
+  if constexpr (BLOCKED) {  // flat id among the kept tiles (gram_tc_finalize_kernel's order); -1: a padding CTA
+    tile_id = bn - bm / 2;
+    for (int a = 0; a < bm; ++a) tile_id += p.num_bn - a / 2;
+    if (bm >= p.num_bm) tile_id = -1;
+  }
   const int a_col0 = bm * 128, b_col0 = bn * p.tn;
   constexpr int BOX_COLS = TcRing<MODE>::BOX_COLS;
   const int nbox_b = p.tn / BOX_COLS;
@@ -900,9 +963,13 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
     } else if (threadIdx.x == 0) {
       for (int64_t it = 0; it < iters; ++it)
         gram_tc_produce<MODE>(&tmap, &tmap_b, stage_base, full_bar, empty_bar, it, it_begin, nbox_a, nbox_b, a_col0,
-                              b_col0);
+                              b_col0, (int)rank);
     } else if (MODE == TC_ROWMAJOR && threadIdx.x >= 32) {
       gram_tc_transposer(stage_base, tb_base, full_bar, empty_bar, tb_full, tb_empty, iters, nbox_b);
+    }
+    if constexpr (BLOCKED) {  // no CTA leaves while its peer may still write into it or arrive on its barriers
+      __syncwarp();
+      cluster_sync_all();
     }
     return;
   }
@@ -920,7 +987,8 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
   } else if constexpr (BLOCKED) {  // tn == 256; A inside B: its k8 slices are rows of B's (8 KB apart), else 128-row slices in slot 8
     gram_tc_consumer_blocked(p, stage_base, full_bar, empty_bar, iters,
                              a_in_b ? (a_col0 - b_col0) * 32 : 8 * TC_BOX_BYTES, a_in_b ? 256 * 32 : 128 * 32, tile_id,
-                             split);
+                             split, rank ^ 1u);
+    cluster_sync_all();
     return;
   } else {
 #define TNB_GRAM_CONSUME(NT)                                                                                          \
@@ -1112,11 +1180,12 @@ inline int encode_rowmajor_f32(CUtensorMap* tmap, const T* ptr, int64_t rows, in
 }
 
 // 3-D map over a K-blocked matrix (64 floats per 8 rows x 8 columns, cols / 8 column groups, rows / 8 row groups):
-// box (64, box_cols / 8, TC_KC / 8) lands in shared memory as TC_KC / 8 k8 slices of box_cols columns x 32 bytes.
-inline int encode_kblocked_f32(CUtensorMap* tmap, const float* ptr, int64_t rows, int64_t cols, int box_cols) {
+// box (64, box_cols / 8, box_k8) lands in shared memory as box_k8 k8 slices of box_cols columns x 32 bytes.
+inline int encode_kblocked_f32(CUtensorMap* tmap, const float* ptr, int64_t rows, int64_t cols, int box_cols,
+                               int box_k8 = TC_KC / 8) {
   cuuint64_t gdim[3] = {64, (cuuint64_t)(cols / 8), (cuuint64_t)(rows / 8)};
   cuuint64_t gstride[2] = {64 * sizeof(float), (cuuint64_t)cols * 8 * sizeof(float)};
-  cuuint32_t box[3] = {64, (cuuint32_t)box_cols / 8, TC_KC / 8};
+  cuuint32_t box[3] = {64, (cuuint32_t)box_cols / 8, (cuuint32_t)box_k8};
   cuuint32_t estr[3] = {1, 1, 1};
   CUresult cr = get_encode_tiled()(tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(ptr), gdim, gstride, box,
                                    estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
@@ -1125,8 +1194,47 @@ inline int encode_kblocked_f32(CUtensorMap* tmap, const float* ptr, int64_t rows
   return TNB_OK;
 }
 
+// Launch of the K-blocked Gram: clusters of two CTAs (one pair of tiles), TC_SMEM_BYTES each; `attr` backs the config.
+inline cudaLaunchConfig_t gram_tc_pair_config(cudaLaunchAttribute& attr, dim3 grid, cudaStream_t st) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = grid;
+  cfg.blockDim = dim3(TC_THREADS);
+  cfg.dynamicSmemBytes = TC_SMEM_BYTES;
+  cfg.stream = st;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = 2;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  return cfg;
+}
+
+// Whether a cluster of two K-blocked Gram CTAs, each with TC_SMEM_BYTES of shared memory, fits the current device; asked
+// once per device.  True where no sm_90 device is current: nothing is launched there, and sizing stays that of an H100.
+inline bool gram_tc_pairs_fit() {
+  static PerDeviceFlag known;  // 0: not asked yet, 1: fits, 2: does not
+  if (!tc_path_available()) return true;
+  std::atomic<int>& v = known.v[current_device_index()];
+  int s = v.load(std::memory_order_acquire);
+  if (s == 0) {
+    cudaLaunchAttribute attr;
+    const cudaLaunchConfig_t cfg = gram_tc_pair_config(attr, dim3(2), nullptr);
+    int nc = 0;
+    if (cudaFuncSetAttribute(gram_tc_kernel<TC_KBLOCKED>, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM_BYTES) !=
+            cudaSuccess ||
+        cudaOccupancyMaxActiveClusters(&nc, gram_tc_kernel<TC_KBLOCKED>, &cfg) != cudaSuccess)
+      nc = 0;
+    cudaGetLastError();
+    s = nc > 0 ? 1 : 2;
+    v.store(s, std::memory_order_release);
+  }
+  return s == 1;
+}
+
+// K-blocked input: the pairs of the K-blocked Gram must fit; otherwise the carry stays row-major (carry_kblocked).
 inline bool gram_tc_kblocked_shape_ok(int64_t rows, int64_t n) {
-  return gram_tc_shape_ok(rows, n) && n >= 256 && n % 8 == 0 && rows % 8 == 0;
+  return gram_tc_shape_ok(rows, n) && n >= 256 && n % 8 == 0 && rows % 8 == 0 && gram_tc_pairs_fit();
 }
 
 // bf16 / fp16 input: 16-byte rows (n % 8 == 0) and 128-column tiles: a folded n = 32 / 64, n = 128, or n >= 256 (where
@@ -1178,12 +1286,18 @@ inline int gram_tc(const T* A, int64_t rows, int64_t n, double* G, float* Gf, vo
     TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel<TC_BF16, T>, TC_SMEM_BYTES));
     gram_tc_kernel<TC_BF16, T><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(tmap, tmap, p);
   } else if (kblocked) {
+    // Pairs of tiles in clusters of two CTAs (gram_tc_kblocked_shape_ok checked that they fit), on the split-K factor of
+    // the single tiles: for an even tile-row count on an even SM count it is the factor of the pairs on half the SMs
+    // (2048 columns, 128 SMs: 36 pairs x 16 splits, 9 waves of 64 pairs).
     CUtensorMap ta, tb;
     TNB_TRY(encode_kblocked_f32(&ta, A, rows, n, 128));
-    TNB_TRY(encode_kblocked_f32(&tb, A, rows, n, 256));
+    TNB_TRY(encode_kblocked_f32(&tb, A, rows, n, 256, TC_KC / 16));
     static PerDeviceFlag attr_done;
     TNB_CUDA(ensure_dyn_smem(attr_done, gram_tc_kernel<TC_KBLOCKED>, TC_SMEM_BYTES));
-    gram_tc_kernel<TC_KBLOCKED><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(ta, tb, p);
+    cudaLaunchAttribute attr;
+    const cudaLaunchConfig_t cfg =
+        gram_tc_pair_config(attr, dim3(2 * (unsigned)gram_tc_num_pairs(p.num_bm, p.num_bn), (unsigned)p.ksplit), st);
+    TNB_CUDA(cudaLaunchKernelEx(&cfg, gram_tc_kernel<TC_KBLOCKED>, ta, tb, p));
   } else {
     CUtensorMap tmap;
     TNB_TRY(encode_rowmajor_f32(&tmap, A, rows, n));
