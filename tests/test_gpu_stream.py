@@ -1,8 +1,8 @@
 """-m gpu: the dense TT-SVD of a tensor in host memory (ops.ttsvd_stream / tnb_ttsvd_stream), against ops.ttsvd on the
 device copy of the same data: equal ranks, relative error within 1e-6, and reconstructions that agree.  Every input
 type, chunk budgets from one chunk to as many as the chunk minimums allow, pinned and pageable sources, the goldens of
-the reference, an eps budget, the speculative tail's fallback, the exact-Gram re-stream, the K-blocked carry selected or
-not, tn.Tensor's routing, and the error from the norm alone."""
+the reference, an eps budget, the speculative tail's fallback, the exact-Gram re-stream, the re-solve that needs no
+re-stream, the K-blocked carry selected or not, tn.Tensor's routing, and the error from the norm alone."""
 import os
 
 import numpy as np
@@ -161,6 +161,22 @@ def test_rejected_tf32_gram_is_restreamed_exactly():
     assert info["passes"] == 3 and info["chunks"] == 4, info  # 3 chunks of 21840 rows and one of 16
     g = np.load(os.path.join(GOLD, "lownoise.npz"))
     assert abs(e - float(g[f"{name}/svd/relerr"])) <= 1e-5
+
+
+def test_rejected_fp32_solve_of_an_exact_gram_is_not_restreamed():
+    """fp32 with 12^3 = 1728 step-0 rows, below the tensor-core Gram's 2048: step 0's Gram is exact, and with a
+    speculative tail ahead its eigenpairs come from fp32 rotations, whose noise floor the low-noise spectrum (tail ~1e-11
+    of the trace) does not clear.  The rejected solve is repeated with fp64 rotations on the same Gram: two passes over
+    the host tensor, not three, and one eigensolve more than the device call, whose host-driven repeat solves each step
+    once (the stream's tail is rejected the same way and repeated host-driven too)."""
+    X = torch.as_tensor(cases.make_dense(dict(kind="tt_noise", shape=(12, 12, 12, 32), rank=6, noise=1e-5, seed=31,
+                                              dtype="float32")))
+    from tntorch_b200 import ops
+
+    _, info, _ = _compare(X, 6, chunk_bytes=X.numel() * 4 // 3)
+    _, rinfo = ops.ttsvd(X.cuda(), rmax=6, eps=1e-14, return_info=True)
+    assert info["passes"] == 2 and info["chunks"] == 3 and info["tc_grams"] == 0, info
+    assert info["eig_solves"] == rinfo["eig_solves"] + 1 and rinfo["speculative"] == 0, (info, rinfo)
 
 
 def test_tensor_routing_follows_free_memory(monkeypatch):

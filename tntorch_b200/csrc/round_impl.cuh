@@ -94,7 +94,7 @@ inline int tt_round_impl(ArenaT& ar, bool dry, const T* const* cores_in, const R
                          double eps, uint32_t flags, T* cores_out, int32_t* ranks_host, cudaStream_t st) {
   const int N = d.N;
   // TT cores are small: the generic fp64-accumulating kernels are used throughout
-  StepCtx cx = make_step_ctx(ar, N, eps, flags, false, nullptr, st, false);
+  StepCtx cx = make_step_ctx(ar, dry, N, eps, flags | TNB_FLAG_NO_TENSORCORE, nullptr, st, false);
   if (!dry) {
     cx.h_sc = static_cast<int*>(pinned_scratch(sizeof(SweepScalars)));
     if (!cx.h_sc) return fail(TNB_ERR_CUDA, "pinned scratch allocation failed");
@@ -250,7 +250,7 @@ template <typename T, class ArenaT>
 inline int tt_round_spec_enqueue(ArenaT& ar, bool dry, const T* const* cores_in, const RoundDims& d, const int32_t* rmax,
                                  double eps, uint32_t flags, T* cores_out, SpecHostBack* hb, cudaStream_t st) {
   const int N = d.N;
-  StepCtx cx = make_step_ctx(ar, N, eps, flags, false, nullptr, st, true);
+  StepCtx cx = make_step_ctx(ar, dry, N, eps, flags | TNB_FLAG_NO_TENSORCORE, nullptr, st, true);
   int* d_chol = ar.template take<int>(4);
   size_t maxcore = 0;
   for (int k = 0; k < N; ++k) maxcore = std::max<size_t>(maxcore, (size_t)d.ra[k] * d.shape[k] * d.rin[k + 1]);

@@ -132,6 +132,12 @@ struct GramWork {  // untyped buffers: the same for every input type
   size_t tc_bytes = 0;
 };
 
+// Has a (rows x n) matrix of T a tensor-core Gram: tall, and enough rows for it to pay.
+template <typename T>
+inline bool gram_tc_tall_ok(int64_t rows, int64_t n) {
+  return rows >= n && rows >= TC_MIN_ROWS && gram_tc_input_ok<T>(rows, n);
+}
+
 template <typename T, class ArenaT>
 inline void gram_carve(ArenaT& ar, int64_t rows, int64_t n, bool allow_tc, GramWork& w) {  // T: the input type
   const bool tall = rows >= n;
@@ -142,7 +148,7 @@ inline void gram_carve(ArenaT& ar, int64_t rows, int64_t n, bool allow_tc, GramW
   w.partial = ar.template take<double>(pl.partial_elems);
   w.tc_bytes = 0;
   w.tc_ws = nullptr;
-  if (allow_tc && tall && rows >= TC_MIN_ROWS && gram_tc_input_ok<T>(rows, n)) {
+  if (allow_tc && gram_tc_tall_ok<T>(rows, n)) {
     w.tc_bytes = gram_tc_input_workspace_bytes<T>(rows, n);
     w.tc_ws = ar.template take<char>(w.tc_bytes);
   }
@@ -369,15 +375,28 @@ struct StepCtx {
   // speculative (sync-free) sweep
   int* d_flags = nullptr;       // device flags raised by spec_check_kernel / cd_finish_kernel
   int32_t* d_ranks = nullptr;   // device copy of the ranks the rule chose, [N + 1]
+
+  // May a host-driven step take a tensor-core Gram?  The TF32 Gram equals (1 - c) * G, c ~ 7e-4 (operand truncation
+  // shrinks every product alike: harmless, the rank rule works on ratios) plus noise of ~1.6e-6 * ||G|| (measured,
+  // tests/test_model.py) — a floor under the tail energies the rank rule can resolve.  An eps budget between "inactive"
+  // and 1e-4 of the trace needs finer resolution than that: those sweeps take the exact-product fp64-accumulating Gram
+  // instead.  The sizing pass sizes for the tensor-core Gram whatever the budget.
+  bool tc_gram(bool dry) const { return allow_tc && !exact_gram && (dry || eps_scaled2 < 1e-20 || eps_scaled2 >= 1e-4); }
 };
+
+// The tensor-core kernels may run: the caller did not turn them off and the device has them (the sizing pass, which
+// cannot ask the device, sizes for them).
+inline bool tc_allowed(uint32_t flags, bool dry) {
+  return !(flags & TNB_FLAG_NO_TENSORCORE) && (dry || tc_path_available());
+}
 
 // The context of a sweep over N modes.  Carves the device scalars and, for a speculative sweep, then its flags and ranks.
 template <class ArenaT>
-inline StepCtx make_step_ctx(ArenaT& ar, int N, double eps, uint32_t flags, bool allow_tc, SweepInfo* info,
-                             cudaStream_t st, bool speculative) {
+inline StepCtx make_step_ctx(ArenaT& ar, bool dry, int N, double eps, uint32_t flags, SweepInfo* info, cudaStream_t st,
+                             bool speculative) {
   StepCtx cx;
   cx.flags = flags;
-  cx.allow_tc = allow_tc;
+  cx.allow_tc = tc_allowed(flags, dry);
   cx.info = info;
   cx.st = st;
   const double epsN = eps / std::max(1.0, std::sqrt((double)(N - 1)));
@@ -549,6 +568,28 @@ inline int chol_qr_repair(const WideWork& ww, int64_t rank, T* Q, int64_t nq, T*
   return TNB_OK;
 }
 
+// A tall step's factors from its eigenpairs (w descending, V with leading dimension ldv): core = V_r^T (rank x n) and
+// fac = V_r (n x rank), the operand of the projection Cn = C V_r.
+template <typename T>
+inline int tall_factors(const double* w, const double* V, int ldv, int64_t n, int64_t rank, T* core, T* fac,
+                        cudaStream_t st) {
+  scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(V, ldv, (int)n, (int)rank, w, core, 0, 1);
+  TNB_LAUNCH_CHECK();
+  scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(V, ldv, (int)n, (int)rank, w, fac, 0, 0);
+  TNB_LAUNCH_CHECK();
+  return TNB_OK;
+}
+
+// The factors of a zero unfolding at the rank host_step_solve gives it (round.py:137-145).
+template <typename T>
+inline int zero_factors(int64_t rows, int64_t n, int64_t rank, T* core, T* Cn, cudaStream_t st) {
+  fill_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(core, n * rank, (T)0);
+  TNB_LAUNCH_CHECK();
+  fill_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(Cn, rows * rank, (T)0);
+  TNB_LAUNCH_CHECK();
+  return TNB_OK;
+}
+
 // The end of a truncation step at rank `rank`, from the step's eigenpairs (w descending, V with leading dimension ldv):
 //   tall (rows >= n): core = V_r^T (rank x n);  Cn = C V_r;
 //   wide:             core = diag(1/d) U_r^T C (accumulated in fp64), Cn = U_r diag(d), d_j = max(s_j, 1e-8 s_0), then
@@ -567,10 +608,7 @@ inline int step_factors(const StepCtx& cx, const TIn* C, int64_t rows, int64_t n
                         T* Cn, int layout = PT_ROWMAJOR, int64_t out_inner = 0) {
   cudaStream_t st = cx.st;
   if (rows >= n) {
-    scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(V, ldv, (int)n, (int)rank, w, core, 0, 1);
-    TNB_LAUNCH_CHECK();
-    scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(V, ldv, (int)n, (int)rank, w, fac, 0, 0);
-    TNB_LAUNCH_CHECK();
+    TNB_TRY(tall_factors<T>(w, V, ldv, n, rank, core, fac, st));
     BigKernelGate gate(st, (cx.flags & TNB_FLAG_CONCURRENT) && rows >= PROJ_TC_MIN_ROWS);
     if constexpr (tc_input<TIn>())
       if (layout != PT_ROWMAJOR)
@@ -585,80 +623,100 @@ inline int step_factors(const StepCtx& cx, const TIn* C, int64_t rows, int64_t n
   return chol_qr_repair<T, true>(ww, rank, core, n, Cn, rows, st);
 }
 
+// A host-driven truncation step of a (rows x n) matrix C of TIn, apart from its Gram scratch (GramWork): the fp64 Gram
+// G (L x L), the eigen stage (its block precision follows the data), and the factors' scratch: fac = V_r (tall steps)
+// or ww (wide steps), and ptc_ws the tensor-core projection's workspace (project_tc_carve_bytes).
+template <typename T>
+struct HostStep {
+  int64_t L = 0, kcap = 0;
+  double* G = nullptr;
+  EigWork<T> ew;
+  T* fac = nullptr;
+  WideWork ww;
+  void* ptc_ws = nullptr;
+  size_t ptc_bytes = 0;
+  float* Gf() const { return reinterpret_cast<float*>(ew.Gb); }  // G in fp32 for an fp32 subspace solve, else nullptr
+};
+template <typename T, typename TIn, class ArenaT>
+inline int host_step_carve(ArenaT& ar, const StepCtx& cx, int64_t rows, int64_t n, int64_t rank_cap, bool have_rmax,
+                           HostStep<T>& s) {
+  s.L = std::min(rows, n);
+  s.kcap = std::min<int64_t>(rank_cap, s.L);
+  s.G = ar.template take<double>((size_t)s.L * s.L);
+  TNB_TRY(eig_carve<T>(ar, s.L, s.kcap, have_rmax, s.ew));
+  if (rows >= n) s.fac = ar.template take<T>((size_t)s.L * (size_t)s.kcap);
+  else wide_carve(ar, rows, n, s.kcap, s.ww);
+  s.ptc_bytes = project_tc_carve_bytes<TIn>(cx.allow_tc, rows, n, s.kcap);
+  s.ptc_ws = s.ptc_bytes ? ar.template take<char>(s.ptc_bytes) : nullptr;
+  return TNB_OK;
+}
+
+// The Gram, eigen stage and rank rule of a host-driven step.  gram(use_tc, &used_tc) makes s.G (and s.Gf()) and the
+// step scalars' trace, and reports which Gram ran (gram_small_side's *used_tc).  Eigenpairs the accept rule rejects
+// (tf32_reject: too steep a spectrum for a tensor-core Gram's or the fp32 solve's noise floor) are solved again with
+// fp64 rotations, on a new exact Gram if the rejected one came from the tensor cores.  prof (nullptr: none) records
+// the step's first three events, the caller the fourth.  Returns the step's rank, at most s.kcap, and whether the
+// unfolding is zero: then the rank is 1 (round.py:137-145), but the batch rank rule (round.py:149-150) has no zero
+// branch and keeps min(rmax, L), so a zero sample's factors are zero at that rank, like the other samples' of its batch.
+template <typename T, class GramF>
+inline int host_step_solve(const StepCtx& cx, HostStep<T>& s, GramF&& gram, bool use_tc, int32_t rm, bool first_step,
+                           bool shared_gpu, bool fp32_solve, Prof* prof, int64_t* rank, bool* zero) {
+  const int batch_mode = (cx.flags & TNB_FLAG_BATCH_MODE) ? 1 : 0;
+  const SweepScalars* hs = reinterpret_cast<const SweepScalars*>(cx.h_sc);
+  if (prof) prof->mark(cx.st);
+  int used_tc = 0;
+  TNB_TRY(gram(use_tc, &used_tc));
+  if (prof) prof->mark(cx.st);
+  ChfsiStats cs;
+  int solves = 0;
+  TNB_TRY(eig_solve_and_rank<T>(s.G, s.ew.Gb, s.L, s.ew, cx.sc, cx.h_sc, rm, batch_mode, &cs, &solves, cx.st,
+                                cx.allow_tc, shared_gpu, used_tc, fp32_solve));
+  if (hs->tf32_reject) {
+    if (used_tc) TNB_TRY(gram(false, &used_tc));
+    TNB_TRY(eig_solve_and_rank<T>(s.G, s.ew.Gb, s.L, s.ew, cx.sc, cx.h_sc, rm, batch_mode, &cs, &solves, cx.st,
+                                  cx.allow_tc, shared_gpu, 0));
+  }
+  if (prof) prof->mark(cx.st);
+  if (cx.info) {
+    cx.info->tc_grams += used_tc ? 1 : 0;
+    cx.info->eig_solves += solves, cx.info->chfsi_products += cs.products, cx.info->fused_filters += cs.fused_filters;
+    cx.info->rr_sweeps += cs.rr_sweeps, cx.info->rr_solves += cs.outer;
+    if (first_step) cx.info->norm = std::sqrt(hs->norm2 > 0 ? hs->norm2 : 0.0);
+  }
+  *zero = hs->zero_flag != 0;
+  *rank = *zero && !batch_mode ? 1 : std::min<int64_t>(hs->rank, s.kcap);
+  return TNB_OK;
+}
+
 // TIn: the element type of C (the dense input at step 0, else T).
 template <typename T, typename TIn, class ArenaT>
 inline int truncate_step(ArenaT& ar, bool dry, const StepCtx& cx, const TIn* C, int64_t rows, int64_t n, int64_t rank_cap,
                          bool have_rmax, int32_t rm, bool first_step, T* core, T* Cn, int64_t* rank_out) {
-  typedef T TBk;  // block precision of the subspace eigensolver follows the data
-  const bool tall = rows >= n;
-  const int64_t L = tall ? n : rows;
-  const int batch_mode = (cx.flags & TNB_FLAG_BATCH_MODE) ? 1 : 0;
   cudaStream_t st = cx.st;
+  const bool tc_gram = cx.tc_gram(dry);
   GramWork gw;
-  EigWork<TBk> ew;
-  // The TF32 Gram equals (1 - c) * G, c ~ 7e-4 (operand truncation shrinks every product alike: harmless, the rank
-  // rule works on ratios) plus noise of ~1.6e-6 * ||G|| (measured, tests/test_model.py) — a floor under the tail
-  // energies the rank rule can resolve.  An eps budget between "inactive" and 1e-4 of the trace needs finer
-  // resolution than that: those sweeps take the exact-product fp64-accumulating Gram instead.
-  const bool tc_gram = cx.allow_tc && !cx.exact_gram && (dry || cx.eps_scaled2 < 1e-20 || cx.eps_scaled2 >= 1e-4);
   gram_carve<TIn>(ar, rows, n, tc_gram, gw);
-  double* G = ar.template take<double>((size_t)L * L);
-  float* Gf = nullptr;
-  const int64_t kcap = std::min<int64_t>(rank_cap, L);
-  TNB_TRY(eig_carve<TBk>(ar, L, kcap, have_rmax, ew));
-  if (ew.chfsi && std::is_same<TBk, float>::value) Gf = reinterpret_cast<float*>(ew.Gb);
-  T* fac = tall ? ar.template take<T>((size_t)L * (size_t)kcap) : nullptr;  // V_r
-  WideWork ww;
-  if (!tall) wide_carve(ar, rows, n, kcap, ww);
-  const size_t ptc_bytes = project_tc_carve_bytes<TIn>(cx.allow_tc, rows, n, kcap);
-  void* ptc_ws = ptc_bytes ? ar.template take<char>(ptc_bytes) : nullptr;
+  HostStep<T> s;
+  TNB_TRY((host_step_carve<T, TIn>(ar, cx, rows, n, rank_cap, have_rmax, s)));
   if (dry) return TNB_OK;
   if (!ar.ok) return fail(TNB_ERR_WORKSPACE, "workspace too small (need > %zu bytes)", ar.off);
-  Prof& prof = Prof::get();
-  prof.mark(st);
-  int used_tc = 0;
   const bool concurrent = (cx.flags & TNB_FLAG_CONCURRENT) != 0;
-  {
-    BigKernelGate gate(st, concurrent && gw.tc_ws != nullptr);
-    TNB_TRY(gram_small_side<TIn>(C, rows, n, G, Gf, gw, tc_gram, &used_tc, st));
-  }
-  if (cx.info) cx.info->tc_grams += used_tc ? 1 : 0;
-  trace_kernel<<<1, 256, 0, st>>>(G, (int)L, (int)L, cx.sc, first_step ? 1 : 0, cx.eps_scaled2);
-  TNB_LAUNCH_CHECK();
-  prof.mark(st);
-  ChfsiStats cs;
-  int solves = 0;
-  TNB_TRY(eig_solve_and_rank<TBk>(G, reinterpret_cast<const TBk*>(Gf), L, ew, cx.sc, cx.h_sc, rm, batch_mode, &cs, &solves, st,
-                                  cx.allow_tc, concurrent, used_tc));
-  if (used_tc && reinterpret_cast<const SweepScalars*>(cx.h_sc)->tf32_reject) {
-    // the spectrum is too steep for the TF32 noise floor (small_kernels.cuh::tf32_gram_rejected): same step again on
-    // the exact-product, fp64-accumulated Gram
-    if (cx.info) cx.info->tc_grams -= 1;
-    used_tc = 0;
-    TNB_TRY(gram_small_side<TIn>(C, rows, n, G, Gf, gw, false, nullptr, st));
-    trace_kernel<<<1, 256, 0, st>>>(G, (int)L, (int)L, cx.sc, first_step ? 1 : 0, cx.eps_scaled2);
+  auto gram = [&](bool use_tc, int* used_tc) -> int {
+    {
+      BigKernelGate gate(st, concurrent && use_tc && gw.tc_ws != nullptr);
+      TNB_TRY(gram_small_side<TIn>(C, rows, n, s.G, s.Gf(), gw, use_tc, used_tc, st));
+    }
+    trace_kernel<<<1, 256, 0, st>>>(s.G, (int)s.L, (int)s.L, cx.sc, first_step ? 1 : 0, cx.eps_scaled2);
     TNB_LAUNCH_CHECK();
-    TNB_TRY(eig_solve_and_rank<TBk>(G, reinterpret_cast<const TBk*>(Gf), L, ew, cx.sc, cx.h_sc, rm, batch_mode, &cs, &solves,
-                                    st, cx.allow_tc, concurrent, 0));
-  }
-  if (cx.info) cx.info->eig_solves += solves, cx.info->chfsi_products += cs.products, cx.info->fused_filters += cs.fused_filters,
-        cx.info->rr_sweeps += cs.rr_sweeps, cx.info->rr_solves += cs.outer;
-  prof.mark(st);
-  const SweepScalars* hs = reinterpret_cast<const SweepScalars*>(cx.h_sc);
-  if (first_step && cx.info) cx.info->norm = std::sqrt(hs->norm2 > 0 ? hs->norm2 : 0.0);
-  int64_t rank = hs->rank;
-  if (rank > kcap) rank = kcap;
-  if (hs->zero_flag) {
-    // round.py:137-145: rank-1 zero factors; the batch rank rule (round.py:149-150) has no zero branch and keeps
-    // rank = min(rmax, L), so a zero sample's factors are zero at that rank, like the other samples' of its batch
-    if (!batch_mode) rank = 1;
-    fill_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(core, n * rank, (T)0);
-    TNB_LAUNCH_CHECK();
-    fill_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(Cn, rows * rank, (T)0);
-    TNB_LAUNCH_CHECK();
-  } else {
-    TNB_TRY((step_factors<T, TIn>(cx, C, rows, n, rank, ew.w, ew.V, ew.ldv, fac, ww, ptc_ws, ptc_bytes, core, Cn)));
-  }
+    return TNB_OK;
+  };
+  Prof& prof = Prof::get();
+  int64_t rank = 0;
+  bool zero = false;
+  TNB_TRY(host_step_solve<T>(cx, s, gram, tc_gram, rm, first_step, concurrent, false, &prof, &rank, &zero));
+  TNB_TRY((zero ? zero_factors<T>(rows, n, rank, core, Cn, st)
+                : step_factors<T, TIn>(cx, C, rows, n, rank, s.ew.w, s.ew.V, s.ew.ldv, s.fac, s.ww, s.ptc_ws, s.ptc_bytes,
+                                       core, Cn)));
   prof.mark(st);
   *rank_out = rank;
   return TNB_OK;
@@ -868,8 +926,7 @@ inline int ttsvd_sync_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDim
                            uint32_t flags, T* cores, int32_t* ranks_host, SweepInfo* info, cudaStream_t st,
                            bool exact_gram = false, const Carry0<T>* c0 = nullptr) {
   const int N = d.N;
-  StepCtx cx = make_step_ctx(ar, N, eps, flags, !(flags & TNB_FLAG_NO_TENSORCORE) && (dry || tc_path_available()), info,
-                             st, false);
+  StepCtx cx = make_step_ctx(ar, dry, N, eps, flags, info, st, false);
   cx.exact_gram = exact_gram;
   if (c0 && !dry) {
     TNB_CUDA(cudaMemcpyAsync(cx.sc, c0->sc, sizeof(SweepScalars), cudaMemcpyDeviceToDevice, st));
@@ -946,8 +1003,9 @@ inline int ttsvd_sync_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDim
 // Speculative dense TT-SVD: the whole right-to-left sweep enqueued in one go, ONE synchronisation at the end.
 // ---------------------------------------------------------------------------------------------
 template <typename T>
-inline bool spec_eligible(const SweepDims& d, const int32_t* rmax, double eps, uint32_t flags, bool allow_tc) {
+inline bool spec_eligible(const SweepDims& d, const int32_t* rmax, double eps, uint32_t flags) {
   if ((flags & TNB_FLAG_NO_SPECULATE) || d.N < 2 || !rmax) return false;
+  const bool allow_tc = tc_allowed(flags, false);
   const double epsN = eps / std::max(1.0, std::sqrt((double)(d.N - 1)));
   if (!(epsN * epsN < 1e-20)) return false;  // an active eps budget decides ranks: host-driven path
   for (int mu = d.N - 1; mu >= 1; --mu) {
@@ -983,8 +1041,7 @@ inline int spec_begin(SpecRun<T, TIn, ArenaT>& r, ArenaT& ar, bool dry, const TI
                       uint32_t flags, T* cores, SweepInfo* info, cudaStream_t st, SpecHostBack* hb,
                       const Carry0<T>* c0 = nullptr) {
   r.ar = &ar;
-  r.cx = make_step_ctx(ar, d.N, eps, flags, !(flags & TNB_FLAG_NO_TENSORCORE) && (dry || tc_path_available()), info, st,
-                       true);
+  r.cx = make_step_ctx(ar, dry, d.N, eps, flags, info, st, true);
   carve_carries(ar, d, r.carry, c0 ? 1 : 0);
   r.data = data;
   r.C = c0 ? c0->C : nullptr;
@@ -1117,10 +1174,9 @@ template <typename T, typename TIn, class ArenaT>
 inline int ttsvd_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d, const int32_t* rmax, double eps,
                       uint32_t flags, T* cores, int32_t* ranks_host, SweepInfo* info, cudaStream_t st,
                       const Carry0<T>* c0 = nullptr) {
-  const bool allow_tc = !(flags & TNB_FLAG_NO_TENSORCORE) && (dry || tc_path_available());
   // the sizing pass cannot ask the device what it supports: size for both paths
   const bool spec = dry ? (d.N >= 2 && rmax != nullptr)
-                        : spec_eligible<T>(d, rmax, eps, flags, allow_tc) && (!c0 || c0->rank == d.rcap[d.N - 1]);
+                        : spec_eligible<T>(d, rmax, eps, flags) && (!c0 || c0->rank == d.rcap[d.N - 1]);
   const size_t base = ar.off;
   size_t need_spec = 0;
   if (spec) {
@@ -1160,10 +1216,10 @@ inline int ttsvd_impl(ArenaT& ar, bool dry, const TIn* data, const SweepDims& d,
 // Dense TT-SVD of a tensor in host memory (tnb_ttsvd_stream).  Only step 0 reads the input: C = T viewed
 // (rows x I_{N-1}), and a row block of C is a contiguous byte range of the host tensor.  So step 0 streams C through the
 // device in chunks of whole row blocks, twice: pass 1 sums the chunk Grams into one fp64 G (in chunk order), the eigen
-// stage and rank rule run on G as in truncate_step, and pass 2 projects each chunk into its row range of the step-0
-// carry.  A TF32 Gram that the accept rule rejects costs one more pass 1 with the exact Gram.  Steps 1..N-1 then run
-// through ttsvd_impl from that carry, which stays in memory of its own.  The device never holds more of the input than
-// the chunk ring.
+// stage and rank rule run on G through host_step_solve as in truncate_step, and pass 2 projects each chunk into its row
+// range of the step-0 carry.  A TF32 Gram that the accept rule rejects costs one more pass 1 with the exact Gram.
+// Steps 1..N-1 then run through ttsvd_impl from that carry, which stays in memory of its own.  The device never holds
+// more of the input than the chunk ring.
 // ---------------------------------------------------------------------------------------------
 constexpr size_t STREAM_DEFAULT_CHUNK = (size_t)256 << 20;
 constexpr size_t STREAM_PIECE = (size_t)64 << 20;  // staging piece of a pageable source
@@ -1322,21 +1378,22 @@ inline int ttsvd_stream_impl(ArenaT& ar, bool dry, const TIn* host, const SweepD
                 "cannot fit where the input does not; decompose on the device or lower the last rank cap",
                 (long long)kcap, (long long)n);
   flags &= ~TNB_FLAG_PROFILE;
-  const bool allow_tc = !(flags & TNB_FLAG_NO_TENSORCORE) && (dry || tc_path_available());
-  StepCtx cx = make_step_ctx(ar, N, eps, flags, allow_tc, info, st, false);
+  StepCtx cx = make_step_ctx(ar, dry, N, eps, flags, info, st, false);
   const bool have_rmax = rmax && rmax[mu - 1] > 0;
-  // step 0's kernels, chosen from the full shape as truncate_step / gram_carve / project_any choose them
-  const bool tc_gram = allow_tc && (dry || cx.eps_scaled2 < 1e-20 || cx.eps_scaled2 >= 1e-4) && rows >= TC_MIN_ROWS &&
-                       gram_tc_input_ok<TIn>(rows, n);
-  const size_t ptc_bytes = project_tc_carve_bytes<TIn>(allow_tc, rows, n, kcap);
-  const int64_t inner = d.shape[N - 2];
-  const bool kb_ok = carry_kblocked<T, TIn>(d, N - 2, allow_tc) && 8 * inner * kcap * sizeof(float) <= UNBLOCK_MAX_SMEM;
-  const ChunkPlan plan = make_chunk_plan(rows, n, (size_t)n * sizeof(TIn), chunk_bytes, ptc_bytes > 0, kb_ok ? inner : 0);
   T* carry0 = ar.template take<T>((size_t)rows * kcap);  // outside the ping-pong pair of the sweep that follows
   const size_t mark = ar.off;
+  HostStep<T> s;
+  TNB_TRY((host_step_carve<T, TIn>(ar, cx, rows, n, kcap, have_rmax, s)));
+  // the chunks keep the full tensor's kernels: its Gram, its projection and its carry's layout
+  const bool tc_gram = cx.tc_gram(dry) && gram_tc_tall_ok<TIn>(rows, n);
+  const int64_t inner = d.shape[N - 2];
+  const bool kb_ok = carry_kblocked<T, TIn>(d, N - 2, cx.allow_tc) && 8 * inner * kcap * sizeof(float) <= UNBLOCK_MAX_SMEM;
+  const ChunkPlan plan = make_chunk_plan(rows, n, (size_t)n * sizeof(TIn), chunk_bytes, s.ptc_bytes > 0, kb_ok ? inner : 0);
+  const size_t ring_start = ar.off;
   TIn* buf[2] = {ar.template take<TIn>((size_t)plan.max_rows() * n),
                  plan.nchunks > 1 ? ar.template take<TIn>((size_t)plan.max_rows() * n) : nullptr};
-  if (ring_bytes) *ring_bytes = ar.off - mark;
+  if (ring_bytes) *ring_bytes = ar.off - ring_start;
+  // a chunk's Gram scratch is carved for the larger need of the two chunk sizes: it is not monotone in the row count
   GramWork gw;
   for (int64_t r : {plan.chunk_rows, plan.last_rows}) {
     gw.partial_elems = std::max(gw.partial_elems, plan_gemm(n, n, r, true).partial_elems);
@@ -1344,19 +1401,10 @@ inline int ttsvd_stream_impl(ArenaT& ar, bool dry, const TIn* host, const SweepD
   }
   gw.partial = ar.template take<double>(gw.partial_elems);
   gw.tc_ws = tc_gram ? ar.template take<char>(gw.tc_bytes) : nullptr;
-  double* G = ar.template take<double>((size_t)n * n);
   double* Gc = plan.nchunks > 1 ? ar.template take<double>((size_t)n * n) : nullptr;
-  EigWork<T> ew;
-  TNB_TRY(eig_carve<T>(ar, n, kcap, have_rmax, ew));
-  float* Gf = ew.chfsi && std::is_same<T, float>::value ? reinterpret_cast<float*>(ew.Gb) : nullptr;
-  T* fac = ar.template take<T>((size_t)n * kcap);
-  void* ptc_ws = ptc_bytes ? ar.template take<char>(ptc_bytes) : nullptr;
   double* sq = tc_gram ? ar.template take<double>(SUMSQ_BLOCKS + 1) : nullptr;
   const size_t peak = ar.off;
-  Carry0<T> c0;
-  c0.C = carry0;
-  c0.rank = kcap;
-  c0.sc = cx.sc;
+  Carry0<T> c0{carry0, kcap, false, cx.sc};
   if (!dry) {
     if (!ar.ok) return fail(TNB_ERR_WORKSPACE, "workspace too small (need > %zu bytes)", ar.off);
     bool pinned_src = false;
@@ -1372,8 +1420,8 @@ inline int ttsvd_stream_impl(ArenaT& ar, bool dry, const TIn* host, const SweepD
     } drain{ring.copy};
     const char* src = reinterpret_cast<const char*>(host);
     const size_t row_bytes = (size_t)n * sizeof(TIn);
-    int used_tc = 0, passes = 0;
-    auto gram_pass = [&](bool use_tc) -> int {
+    int passes = 0;
+    auto gram_pass = [&](bool use_tc, int* used_tc) -> int {
       const bool first_pass = ++passes == 1;
       TNB_TRY(stream_pass<TIn>(ring, src, pinned_src, row_bytes, plan, buf, st,
                                [&](int64_t c, const TIn* X, int64_t, int64_t rc) -> int {
@@ -1383,18 +1431,18 @@ inline int ttsvd_stream_impl(ArenaT& ar, bool dry, const TIn* host, const SweepD
                                    sumsq_add_kernel<<<1, 32, 0, st>>>(sq, c == 0 ? 1 : 0);
                                    TNB_LAUNCH_CHECK();
                                  }
-                                 TNB_TRY(gram_small_side<TIn>(X, rc, n, c == 0 ? G : Gc, nullptr, gw, use_tc, &used_tc, st));
+                                 TNB_TRY(gram_small_side<TIn>(X, rc, n, c == 0 ? s.G : Gc, nullptr, gw, use_tc, used_tc, st));
                                  if (c > 0) {
-                                   accumulate_kernel<<<grid_for(n * n), 256, 0, st>>>(G, Gc, n * n);
+                                   accumulate_kernel<<<grid_for(n * n), 256, 0, st>>>(s.G, Gc, n * n);
                                    TNB_LAUNCH_CHECK();
                                  }
                                  return TNB_OK;
                                }));
-      if (Gf) {
-        convert_kernel<double, float><<<grid_for(n * n), 256, 0, st>>>(G, Gf, n * n);
+      if (s.Gf()) {
+        convert_kernel<double, float><<<grid_for(n * n), 256, 0, st>>>(s.G, s.Gf(), n * n);
         TNB_LAUNCH_CHECK();
       }
-      trace_kernel<<<1, 256, 0, st>>>(G, (int)n, (int)n, cx.sc, 1, cx.eps_scaled2);
+      trace_kernel<<<1, 256, 0, st>>>(s.G, (int)n, (int)n, cx.sc, 1, cx.eps_scaled2);
       TNB_LAUNCH_CHECK();
       if (sq) {
         set_norm2_kernel<<<1, 32, 0, st>>>(cx.sc, sq + SUMSQ_BLOCKS, cx.eps_scaled2);
@@ -1402,64 +1450,39 @@ inline int ttsvd_stream_impl(ArenaT& ar, bool dry, const TIn* host, const SweepD
       }
       return TNB_OK;
     };
-    const int batch_mode = (flags & TNB_FLAG_BATCH_MODE) ? 1 : 0;
-    const int32_t rm = have_rmax ? rmax[mu - 1] : 0;
-    const bool spec_tail = spec_eligible<T>(d, rmax, eps, flags, allow_tc);
-    // the eigenpairs come from fp32 rotations where the speculative device sweep takes them so (spec_step_eig_begin)
+    const bool spec_tail = spec_eligible<T>(d, rmax, eps, flags);
+    // the eigenpairs come from fp32 rotations where the speculative device sweep takes them so (spec_step_eig_begin).
+    // Whatever TNB_FLAG_CONCURRENT says, step 0's Gram is not gated and its solve does not share the GPU.
     const bool fp32_solve = spec_tail && std::is_same<T, float>::value && jacobi2_ok((int)n, true);
-    ChfsiStats cs;
-    int solves = 0;
-    TNB_TRY(gram_pass(tc_gram));
-    TNB_TRY(eig_solve_and_rank<T>(G, reinterpret_cast<const T*>(Gf), n, ew, cx.sc, cx.h_sc, rm, batch_mode, &cs, &solves,
-                                  st, allow_tc, false, used_tc, fp32_solve));
-    const SweepScalars* hs = reinterpret_cast<const SweepScalars*>(cx.h_sc);
-    if (hs->tf32_reject) {  // too steep a spectrum for the tensor-core Gram or the fp32 solve: exact Gram, fp64 rotations
-      if (used_tc) TNB_TRY(gram_pass(false));
-      used_tc = 0;
-      TNB_TRY(eig_solve_and_rank<T>(G, reinterpret_cast<const T*>(Gf), n, ew, cx.sc, cx.h_sc, rm, batch_mode, &cs, &solves,
-                                    st, allow_tc, false, 0));
-    }
-    if (info) {
-      info->tc_grams += used_tc ? 1 : 0;
-      info->eig_solves += solves, info->chfsi_products += cs.products, info->fused_filters += cs.fused_filters;
-      info->rr_sweeps += cs.rr_sweeps, info->rr_solves += cs.outer;
-      info->norm = std::sqrt(hs->norm2 > 0 ? hs->norm2 : 0.0);
-    }
-    int64_t rank = std::min<int64_t>(hs->rank, kcap);
+    int64_t rank = 0;
+    bool zero = false;
+    TNB_TRY(host_step_solve<T>(cx, s, gram_pass, tc_gram, have_rmax ? rmax[mu - 1] : 0, true, false, fp32_solve, nullptr,
+                               &rank, &zero));
     T* core = cores + d.slot[mu];
-    if (hs->zero_flag) {  // round.py:137-145: rank-1 zero factors (zero factors at the rank cap under the batch rule)
-      if (!batch_mode) rank = 1;
-      fill_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(core, n * rank, (T)0);
-      TNB_LAUNCH_CHECK();
-      fill_kernel<T><<<grid_for(rows * rank), 256, 0, st>>>(carry0, rows * rank, (T)0);
-      TNB_LAUNCH_CHECK();
+    if (zero) {
+      TNB_TRY(zero_factors<T>(rows, n, rank, core, carry0, st));
     } else {
       c0.kblocked = kb_ok && spec_tail && rank == kcap;
-      scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(ew.V, ew.ldv, (int)n, (int)rank, ew.w, core, 0, 1);
-      TNB_LAUNCH_CHECK();
-      scale_extract_kernel<T><<<grid_for(n * rank), 256, 0, st>>>(ew.V, ew.ldv, (int)n, (int)rank, ew.w, fac, 0, 0);
-      TNB_LAUNCH_CHECK();
+      TNB_TRY(tall_factors<T>(s.ew.w, s.ew.V, s.ew.ldv, n, rank, core, s.fac, st));
       ++passes;
       TNB_TRY(stream_pass<TIn>(ring, src, pinned_src, row_bytes, plan, buf, st,
                                [&](int64_t, const TIn* X, int64_t r0, int64_t rc) -> int {
                                  T* out = carry0 + (size_t)r0 * rank;
                                  if constexpr (tc_input<TIn>())
-                                   if (ptc_ws)
-                                     return project_tc<TIn>(X, rc, n, reinterpret_cast<const float*>(fac), (int)rank,
-                                                            reinterpret_cast<float*>(out), ptc_ws, ptc_bytes, st,
+                                   if (s.ptc_ws)
+                                     return project_tc<TIn>(X, rc, n, reinterpret_cast<const float*>(s.fac), (int)rank,
+                                                            reinterpret_cast<float*>(out), s.ptc_ws, s.ptc_bytes, st,
                                                             c0.kblocked ? PT_OUT_KBLOCKED : PT_ROWMAJOR,
                                                             c0.kblocked ? inner : 0);
-                                 return project_any<T, TIn>(X, rc, n, fac, rank, out, st);
+                                 return project_any<T, TIn>(X, rc, n, s.fac, rank, out, st);
                                }));
     }
     if (info) {
       info->stream_passes = passes;
       info->stream_chunks = (int)plan.nchunks;
-      if (spec_tail && rank != kcap) info->spec_flags = hs->zero_flag ? 32 : 16;  // spec_check_kernel's bits
+      if (spec_tail && rank != kcap) info->spec_flags = zero ? 32 : 16;  // spec_check_kernel's bits
     }
-    ranks_host[0] = 1;
-    ranks_host[mu] = (int32_t)rank;
-    ranks_host[N] = 1;
+    ranks_host[mu] = (int32_t)rank;  // the rest of the sweep sets the others
     c0.rank = rank;
   }
   ar.off = mark;  // the rest of the sweep reuses the chunk ring and step 0's scratch
@@ -1512,8 +1535,7 @@ inline int ttsvd_batch_impl(void* workspace, size_t per_tensor_bytes, int inflig
                             const SweepDims& d, const int32_t* rmax, double eps, uint32_t flags, T* const* cores,
                             int32_t* ranks_host, double* norms_host, int32_t* spec_host, cudaStream_t st) {
   const int N = d.N;
-  const bool allow_tc = !(flags & TNB_FLAG_NO_TENSORCORE) && tc_path_available();
-  const bool spec = batch > 0 && spec_eligible<T>(d, rmax, eps, flags, allow_tc);
+  const bool spec = batch > 0 && spec_eligible<T>(d, rmax, eps, flags);
   char* ws = static_cast<char*>(workspace);
   if (!spec || inflight < 2 || batch < 2) {  // one at a time through the dispatcher (speculative when eligible)
     for (int i = 0; i < batch; ++i) {
