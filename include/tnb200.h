@@ -223,6 +223,11 @@ int tnb_measure_tf32_peak(int32_t reps, int32_t per_commit, int32_t trials, doub
  * accumulators; `reps` commit groups of 4 x `per_commit` wgmma per warpgroup. */
 int tnb_measure_wgmma_tf32_peak(int32_t reps, int32_t per_commit, int32_t trials, double* tflops_host, double* ms_host,
                                 void* stream);
+/* The same for mma.sync.m16n8k16 .f64 (DMMA), the instruction of tnb_tt_dot's tensor-core path: two CTAs per SM, every
+ * warp issuing it back to back on register operands into eight accumulators.  The denominator of tnb_tt_dot's fractions
+ * of the fp64 tensor-core peak. */
+int tnb_measure_f64_mma_peak(int32_t reps, int32_t per_commit, int32_t trials, double* tflops_host, double* ms_host,
+                             void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Two-factor rank-revealing split  M (m x n)  ->  left (m x r), right (r x n).
@@ -462,6 +467,30 @@ size_t tnb_tt_multiply_workspace_bytes(int dtype, int d, const int64_t* input_di
 int tnb_tt_multiply(int dtype, const void* const* cores, int d, const int64_t* input_dims, const int64_t* output_dims,
                     const int32_t* ranks, const void* X, int64_t batch, void* Y, void* workspace, size_t workspace_bytes,
                     void* stream);
+
+/* Inner products of npairs pairs of tensor trains: out[p] = <a_p, b_p> (fp64, on the device), neither tensor formed.
+ * cores_a[p * ndim + k] is core k of train a of pair p, ranks_a[p * (ndim + 1) + k] x shape[k] x
+ * ranks_a[p * (ndim + 1) + k + 1] (row-major); likewise b.  Every train has the one shape; each pair has its own rank
+ * profiles (host arrays of npairs * (ndim + 1) ints), with boundary ranks 1.  A pair may pass the same cores for a and b
+ * (a squared norm).  dtype TNB_F32 or TNB_F64 for every core; any other dtype returns TNB_ERR_UNSUPPORTED and sizes to 0.
+ * The arithmetic is fp64 in both: fp32 cores are widened exactly as they are loaded.
+ * Null pointers, ndim < 1, npairs < 1, a mode size or rank below 1 or boundary ranks other than 1 are TNB_ERR_INVALID;
+ * ndim above 1024, a rank at or above 2^25 or a core above 2^46 elements TNB_ERR_UNSUPPORTED; a workspace below
+ * tnb_tt_dot_workspace_bytes TNB_ERR_WORKSPACE; all before anything is launched.
+ * Stream-ordered, no host synchronisation, no allocation.  The same call on the same inputs gives bitwise identical
+ * results (fixed-order reductions, no atomics, a split that depends on the shapes and npairs only).
+ * Per mode k, F_{k+1} = sum_i A_k[:, i, :]^T F_k B_k[:, i, :] in the cheaper of the two association orders, split over
+ * chunks of i so that all pairs together fill the GPU; a pair's mode runs on the fp64 tensor cores (mma.sync m16n8k16
+ * .f64) when all four ranks involved are in [16, 256], on fp64 CUDA-core tiles otherwise (always the boundary modes).
+ * Launches per call: for each mode and each group of 32 pairs, one launch per path in use and one reduction, so 2 or 3
+ * per mode and group.  The workspace holds one F_k per pair and one mode's partial sums; never a copy of a core.
+ * Replaces: tntorch.metrics.dot (metrics.py:28-116) for k = None on trains of equal length (one torch.einsum chain per
+ * pair, in the cores' precision). */
+size_t tnb_tt_dot_workspace_bytes(int dtype, int npairs, int ndim, const int64_t* shape, const int32_t* ranks_a,
+                                  const int32_t* ranks_b);
+int tnb_tt_dot(int dtype, const void* const* cores_a, const void* const* cores_b, int npairs, int ndim,
+               const int64_t* shape, const int32_t* ranks_a, const int32_t* ranks_b, double* out, void* workspace,
+               size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }

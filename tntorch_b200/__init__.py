@@ -7,7 +7,7 @@ from .round import reduce, relative_error, round, round_tt, round_tucker, trunca
 from .tensor import Tensor  # noqa: F401
 from .cross import cross, cross_forward, meshgrid  # noqa: F401
 from .cross_batch import cross_batch  # noqa: F401
-from .callers import TTMatrix, dot, hadamard_sum, shift_mode, tt_multiply  # noqa: F401
+from .callers import TTMatrix, dist, dot, hadamard_sum, norm, normsq, shift_mode, tt_multiply  # noqa: F401
 from . import ops  # noqa: F401
 
 __version__ = "0.1.0"

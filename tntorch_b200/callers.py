@@ -1,6 +1,8 @@
 """Callers of the rounding path that re-round in loops (SURVEY.md §8(f)-3), on the device entry points:
 
-  dot           metrics.py:28-116     <a, b> through the small interface matrices
+  dot           metrics.py:28-116     <a, b> through the small interface matrices, one library call (tnb_tt_dot)
+  normsq, norm  metrics.py:298-319    <t, t> and its square root
+  dist          metrics.py:119-132    ||t1 - t2|| from three dots in one call
   hadamard_sum  metrics.py:321-450    sum of the elementwise product of K tensors, re-rounding the running product
   shift_mode    tools.py:650-697      move one mode through a TT, one truncated_svd per position
   TTMatrix      matrix.py:12-140      matrix -> d-way (i_k x o_k) tensor -> TT-SVD (plain or batched)
@@ -14,16 +16,73 @@ from __future__ import annotations
 import math
 from typing import List, Sequence, Union
 
+import numpy as np
 import torch
 
 from . import ops
 from .tensor import Tensor
 
 
-def dot(t1: Tensor, t2: Tensor):
-    """metrics.dot for two TT(-Tucker) tensors of the same shape; fp64 interface matrices."""
-    assert list(t1.shape) == list(t2.shape)
-    return t1._tt_dot(t2)
+def _trains(t: Tensor):
+    """The plain TT cores of `t`, one list per sample of a batch=True tensor."""
+    if not t.batch:
+        return [t._tt_cores()]
+    if any(U is not None for U in t.Us) or any(c.dim() != 4 for c in t.cores):
+        raise NotImplementedError("dot products of batched Tucker or CP tensors are not supported")
+    return [[c[b] for c in t.cores] for b in range(t.cores[0].shape[0])]
+
+
+def _check_pair(t1: Tensor, t2: Tensor, k=None):
+    if k is not None:
+        raise NotImplementedError("tn.dot: partial contractions (k=) are not supported")
+    if t1.dim() != t2.dim():
+        raise NotImplementedError(f"tn.dot: tensors of unequal dimension ({t1.dim()} and {t2.dim()}) are not supported")
+    if t1.batch != t2.batch:
+        raise NotImplementedError("tn.dot: a batched tensor with a plain one is not supported")
+    if not np.array_equal(t1.shape, t2.shape):  # metrics.py:75-80
+        raise ValueError("Dot product requires leading dimensions to be equal, but they are {} and {}".format(
+            t1.shape, t2.shape))
+
+
+def _dots(*pairs):
+    """<t1, t2> for several pairs from one library call (ops.tt_dot_batch): a 0-d float64 tensor per pair, or a [B]
+    one when the pair is batched (one dot per sample)."""
+    spec, flat = [], []
+    for t1, t2 in pairs:
+        a = _trains(t1)
+        b = a if t2 is t1 else _trains(t2)
+        if len(a) != len(b):
+            raise ValueError(f"tn.dot: batch sizes differ ({len(a)} and {len(b)})")
+        spec.append((len(flat), len(a), t1.batch))
+        flat += list(zip(a, b))
+    out = ops.tt_dot_batch(flat)
+    return [out[s:s + n] if batch else out[s] for s, n, batch in spec]
+
+
+def dot(t1: Tensor, t2: Tensor, k=None):
+    """metrics.dot (k = None) for two TT(-Tucker, -CP) tensors of the same shape: a 0-d float64 tensor, or [B] for
+    batch=True tensors, from one library call (tnb_tt_dot, fp64 on the device).  k= and tensors of unequal dimension
+    raise NotImplementedError; a shape mismatch raises ValueError like the reference."""
+    _check_pair(t1, t2, k)
+    return _dots((t1, t2))[0]
+
+
+def normsq(t: Tensor):
+    """metrics.normsq: <t, t>."""
+    return dot(t, t)
+
+
+def norm(t: Tensor):
+    """metrics.norm: sqrt(max(<t, t>, 0))."""
+    return torch.sqrt(torch.clamp(normsq(t), min=0))
+
+
+def dist(t1: Tensor, t2: Tensor):
+    """metrics.dist for two TT tensors: sqrt(<t1, t1> + <t2, t2> - 2 max(<t1, t2>, 0)), the three dots from one call.
+    Like the reference's, this cannot resolve distances below about 1e-8 of the norms (the squares cancel)."""
+    _check_pair(t1, t2)
+    aa, bb, ab = _dots((t1, t1), (t2, t2), (t1, t2))
+    return torch.sqrt(aa + bb - 2 * ab.clamp(0))
 
 
 def _sum_all(cores: Sequence[torch.Tensor]):

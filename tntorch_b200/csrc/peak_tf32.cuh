@@ -7,9 +7,12 @@
 // from registers and B from a fixed K-major SWIZZLE_128B shared-memory buffer, two warpgroups per CTA, one CTA per SM,
 // each warpgroup into its own 128 accumulators (the shape and operand sources of the Gram's 128 x 256 tile).
 // `reps` commit groups of 4 x `per_commit` wgmma per warpgroup; FLOP = 2*64*256*8 per wgmma.
+// The TT inner product (tt_dot.cuh) issues mma.sync m16n8k16 .f64 (DMMA): peak_f64_kernel measures it the way
+// peak_tf32_kernel measures the TF32 MMA, two 256-thread CTAs per SM; FLOP = 2*16*8*16 per MMA.
 #pragma once
 #include "common.cuh"
 #include "gram_tc.cuh"
+#include "tt_dot.cuh"
 
 namespace tnb {
 
@@ -28,6 +31,20 @@ __global__ void __launch_bounds__(PK_THREADS) peak_tf32_kernel(int reps, int per
 #pragma unroll
   for (int a = 0; a < PK_ACC; ++a) s += acc[a][0] + acc[a][1] + acc[a][2] + acc[a][3];
   if (sink && s == 12345.f) sink[0] = s;  // keeps the products live; never true for these operands
+}
+
+__global__ void __launch_bounds__(PK_THREADS) peak_f64_kernel(int reps, int per_commit, double* sink) {
+  const double x = 1.0 + (double)(threadIdx.x & 7) * 0.125, y = 0.5 + (double)(threadIdx.x >> 5) * 0.0625;
+  const double a[8] = {x, y, x, y, x, y, x, y}, b[4] = {y, x, y, x};
+  double acc[PK_ACC][4] = {};
+  for (int r = 0; r < reps; ++r)
+    for (int m = 0; m < per_commit; ++m)
+#pragma unroll
+      for (int k = 0; k < PK_ACC; ++k) dmma_16816(acc[k], a, b);
+  double s = 0.0;
+#pragma unroll
+  for (int k = 0; k < PK_ACC; ++k) s += acc[k][0] + acc[k][1] + acc[k][2] + acc[k][3];
+  if (sink && s == 12345.0) sink[0] = s;  // keeps the products live; never true for these operands
 }
 
 constexpr int PKW_THREADS = 256;
@@ -61,12 +78,13 @@ __global__ void __launch_bounds__(PKW_THREADS, 1) peak_tf32_wgmma_kernel(int rep
   if (sink && s == 12345.f) sink[0] = s;  // keeps the products live; never true for these operands
 }
 
-// Returns TFLOP/s of the best of `trials` timed launches (CUDA events on `st`); wgmma selects peak_tf32_wgmma_kernel.
+// Returns TFLOP/s of the best of `trials` timed launches (CUDA events on `st`); wgmma selects peak_tf32_wgmma_kernel,
+// f64 peak_f64_kernel.
 inline int measure_tf32_peak(int reps, int per_commit, int trials, double* tflops_out, double* ms_out, cudaStream_t st,
-                             bool wgmma = false) {
+                             bool wgmma = false, bool f64 = false) {
   if (!tc_path_available()) return fail(TNB_ERR_UNSUPPORTED, "tensor-core path not available on this device");
   const int blocks = (wgmma ? 1 : 2) * device_info().sm_count;
-  float* sink = nullptr;
+  void* sink = nullptr;
   TNB_CUDA(cudaMalloc(&sink, 256));
   cudaEvent_t e0, e1;
   TNB_CUDA(cudaEventCreate(&e0));
@@ -74,10 +92,12 @@ inline int measure_tf32_peak(int reps, int per_commit, int trials, double* tflop
   double best = 1e30;
   for (int t = 0; t < trials + 2; ++t) {
     TNB_CUDA(cudaEventRecord(e0, st));
-    if (wgmma)
-      peak_tf32_wgmma_kernel<<<blocks, PKW_THREADS, 0, st>>>(reps, per_commit, sink);
+    if (f64)
+      peak_f64_kernel<<<blocks, PK_THREADS, 0, st>>>(reps, per_commit, static_cast<double*>(sink));
+    else if (wgmma)
+      peak_tf32_wgmma_kernel<<<blocks, PKW_THREADS, 0, st>>>(reps, per_commit, static_cast<float*>(sink));
     else
-      peak_tf32_kernel<<<blocks, PK_THREADS, 0, st>>>(reps, per_commit, sink);
+      peak_tf32_kernel<<<blocks, PK_THREADS, 0, st>>>(reps, per_commit, static_cast<float*>(sink));
     TNB_CUDA(cudaEventRecord(e1, st));
     TNB_CUDA(cudaEventSynchronize(e1));
     TNB_COUNT_LAUNCH();
@@ -90,7 +110,8 @@ inline int measure_tf32_peak(int reps, int per_commit, int trials, double* tflop
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
   cudaFree(sink);
-  const double flop = wgmma ? 2.0 * 64 * 256 * 8 * 4 * (double)reps * per_commit * (PKW_THREADS / 128) * blocks
+  const double flop = f64 ? 2.0 * 16 * 8 * 16 * PK_ACC * (double)reps * per_commit * (PK_THREADS / 32) * blocks
+                    : wgmma ? 2.0 * 64 * 256 * 8 * 4 * (double)reps * per_commit * (PKW_THREADS / 128) * blocks
                             : 2.0 * 16 * 8 * 8 * PK_ACC * (double)reps * per_commit * (PK_THREADS / 32) * blocks;
   *tflops_out = flop / (best * 1e-3) / 1e12;
   if (ms_out) *ms_out = best;

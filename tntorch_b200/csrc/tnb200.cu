@@ -15,6 +15,7 @@
 #include "peak_tf32.cuh"
 #include "expand_tc.cuh"
 #include "tt_multiply.cuh"
+#include "tt_dot.cuh"
 
 using namespace tnb;
 
@@ -660,6 +661,14 @@ int tnb_measure_wgmma_tf32_peak(int32_t reps, int32_t per_commit, int32_t trials
   return measure_tf32_peak(reps, per_commit, trials, tflops_host, ms_host, as_stream(stream), /*wgmma=*/true);
 }
 
+int tnb_measure_f64_mma_peak(int32_t reps, int32_t per_commit, int32_t trials, double* tflops_host, double* ms_host,
+                             void* stream) {
+  TNB_TRY(require_device());
+  if (!tflops_host || reps < 1 || per_commit < 1 || trials < 1)
+    return fail(TNB_ERR_INVALID, "tnb_measure_f64_mma_peak: bad argument");
+  return measure_tf32_peak(reps, per_commit, trials, tflops_host, ms_host, as_stream(stream), false, /*f64=*/true);
+}
+
 int tnb_matmul(int dtype, const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, void* stream) {
   TNB_TRY(check_dtype(dtype));
   TNB_TRY(require_device());
@@ -1024,6 +1033,41 @@ int tnb_tt_multiply(int dtype, const void* const* cores, int d, const int64_t* i
     return fail(TNB_ERR_WORKSPACE, "tnb_tt_multiply: workspace too small");
   Arena ar(workspace, workspace_bytes);
   return tt_multiply_dispatch(ar, false, dtype, cores, d, input_dims, output_dims, ranks, X, batch, Y, as_stream(stream));
+}
+
+// ------------------------------------------------------------------ inner products of TT pairs
+size_t tnb_tt_dot_workspace_bytes(int dtype, int npairs, int ndim, const int64_t* shape, const int32_t* ranks_a,
+                                  const int32_t* ranks_b) {
+  if ((dtype != TNB_F32 && dtype != TNB_F64) || !shape || !ranks_a || !ranks_b ||
+      ttd_check_dims(npairs, ndim, shape, ranks_a, ranks_b) != TNB_OK)
+    return 0;
+  ArenaSizer ar;
+  if (tt_dot_impl<double>(ar, true, nullptr, nullptr, npairs, ndim, shape, ranks_a, ranks_b, nullptr, 0) != TNB_OK)
+    return 0;
+  return ar.off > 256 ? ar.off : 256;  // never 0 for a supported call: 0 is the refusal
+}
+
+int tnb_tt_dot(int dtype, const void* const* cores_a, const void* const* cores_b, int npairs, int ndim,
+               const int64_t* shape, const int32_t* ranks_a, const int32_t* ranks_b, double* out, void* workspace,
+               size_t workspace_bytes, void* stream) {
+  if (dtype != TNB_F32 && dtype != TNB_F64)
+    return fail(TNB_ERR_UNSUPPORTED, "tnb_tt_dot: dtype %d is not built (TNB_F32, TNB_F64)", dtype);
+  if (!cores_a || !cores_b || !shape || !ranks_a || !ranks_b || !out || !workspace)
+    return fail(TNB_ERR_INVALID, "tnb_tt_dot: null argument");
+  TNB_TRY(ttd_check_dims(npairs, ndim, shape, ranks_a, ranks_b));
+  for (int64_t j = 0; j < (int64_t)npairs * ndim; ++j)
+    if (!cores_a[j] || !cores_b[j]) return fail(TNB_ERR_INVALID, "tnb_tt_dot: core %lld is null", (long long)j);
+  TNB_TRY(require_device());
+  if (workspace_bytes < tnb_tt_dot_workspace_bytes(dtype, npairs, ndim, shape, ranks_a, ranks_b))
+    return fail(TNB_ERR_WORKSPACE, "tnb_tt_dot: workspace too small");
+  Arena ar(workspace, workspace_bytes);
+  if (dtype == TNB_F64)
+    return tt_dot_impl<double>(ar, false, reinterpret_cast<const double* const*>(cores_a),
+                               reinterpret_cast<const double* const*>(cores_b), npairs, ndim, shape, ranks_a, ranks_b, out,
+                               as_stream(stream));
+  return tt_dot_impl<float>(ar, false, reinterpret_cast<const float* const*>(cores_a),
+                            reinterpret_cast<const float* const*>(cores_b), npairs, ndim, shape, ranks_a, ranks_b, out,
+                            as_stream(stream));
 }
 
 }  // extern "C"

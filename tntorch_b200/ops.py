@@ -96,6 +96,13 @@ def measure_wgmma_tf32_peak(reps: int = 64, per_commit: int = 64, trials: int = 
     return float(tf[0]), float(ms[0])
 
 
+def measure_f64_mma_peak(reps: int = 200, per_commit: int = 64, trials: int = 5):
+    """Dense fp64 mma.sync (m16n8k16 .f64, the MMA of tt_dot) peak of the current GPU in TFLOP/s (csrc/peak_tf32.cuh)."""
+    tf, ms = (C.c_double * 1)(), (C.c_double * 1)()
+    check(lib().tnb_measure_f64_mma_peak(int(reps), int(per_commit), int(trials), tf, ms, _stream()))
+    return float(tf[0]), float(ms[0])
+
+
 def has_tensorcore_path() -> bool:
     return bool(lib().tnb_has_tensorcore_path())
 
@@ -189,6 +196,12 @@ def stream_instead_of_copy(input_bytes: int, workspace_bytes: int, free_bytes: i
     """The rule `tn.Tensor(X_cpu, ranks_tt=r)` decomposes by: stream the host tensor (`ttsvd_stream`) when its device
     image and the device call's workspace would not fit in free device memory, copy it and call `ttsvd` otherwise."""
     return input_bytes + workspace_bytes > free_bytes
+
+
+def dot_instead_of_dense(dense_bytes: int, free_bytes: int) -> bool:
+    """The rule `tn.relative_error(TT, TT)` measures by: the dot-product formula on the trains (tt_dot_batch) when the
+    two dense tensors would not fit in free device memory, decompress both and compare them otherwise."""
+    return dense_bytes > free_bytes
 
 
 def tt_relative_error_from_norm(norm: float, cores: Sequence[torch.Tensor]) -> float:
@@ -1175,3 +1188,73 @@ def tt_multiply(cores: Sequence[torch.Tensor], X: torch.Tensor) -> torch.Tensor:
     with torch.cuda.device(c0.device):
         check(L.tnb_tt_multiply(code, ptrs, d, ii, oo, rk, _ptr(X), b, _ptr(Y), _ptr(ws), wsb, _stream()))
     return Y
+
+
+def _tt_ranks(cores, what: str):
+    if not cores or any(c.dim() != 3 for c in cores):
+        raise ValueError(f"{what}: cores must be 3-D tensors [r, I, r']")
+    ranks = [cores[0].shape[0]] + [c.shape[2] for c in cores]
+    if ranks[0] != 1 or ranks[-1] != 1:
+        raise ValueError(f"{what}: boundary ranks must be 1, got {ranks[0]} and {ranks[-1]}")
+    if any(a.shape[2] != b.shape[0] for a, b in zip(cores[:-1], cores[1:])):
+        raise ValueError(f"{what}: core ranks do not match")
+    return ranks
+
+
+def tt_dot_batch(pairs) -> torch.Tensor:
+    """[<a_p, b_p> for each pair (a_cores, b_cores)] as a [P] float64 tensor, from one library call (tnb_tt_dot) that
+    forms neither tensor: stream-ordered, no host synchronisation.  Every train has the same shape (ValueError
+    otherwise) and its own ranks; boundary ranks 1.  The arithmetic is fp64: float32 cores are widened exactly as they
+    are read, bfloat16 and float16 cores are converted to float32 first (exactly), and a call with any other floating
+    type among its cores reads them all as float64.  A pair may be (cores, cores): a squared norm."""
+    pairs = [(list(a), list(b)) for a, b in pairs]
+    if not pairs:
+        raise ValueError("tt_dot_batch: no pairs")
+    shape = None
+    ranks_a, ranks_b = [], []
+    for a, b in pairs:
+        if len(a) != len(b):
+            raise NotImplementedError(f"tt_dot: trains of unequal length ({len(a)} and {len(b)} cores) are not supported")
+        for cores, rk in ((a, ranks_a), (b, ranks_b)):
+            rk += _tt_ranks(cores, "tt_dot")
+            sh = [c.shape[1] for c in cores]
+            if shape is None:
+                shape = sh
+            elif sh != shape:
+                raise ValueError(f"tt_dot: every train must have the shape {shape}, got {sh}")
+    c0 = pairs[0][0][0]
+    _require_cuda(c0, "tt_dot")
+    allc = [c for a, b in pairs for c in a + b]
+    if any(c.device != c0.device for c in allc):
+        raise ValueError("tt_dot: cores must share one CUDA device")
+    if any(c.requires_grad for c in allc):
+        raise ValueError("tt_dot: cores that require grad are not supported")
+    dts = {c.dtype for c in allc}
+    if any(not dt.is_floating_point for dt in dts):
+        raise ValueError(f"tt_dot: floating-point cores expected, got {sorted(map(str, dts))}")
+    dt = torch.float32 if dts <= {torch.float32, torch.bfloat16, torch.float16} else torch.float64
+
+    ca, cb = [], []
+    for a, b in pairs:
+        a2 = [c.to(dt).contiguous() for c in a]
+        ca += a2
+        cb += a2 if all(x is y for x, y in zip(a, b)) else [c.to(dt).contiguous() for c in b]
+    P, N = len(pairs), len(shape)
+    code = _DT[dt]
+    L = lib()
+    sh, ra, rb = i64(shape), i32(ranks_a), i32(ranks_b)
+    wsb = L.tnb_tt_dot_workspace_bytes(code, P, N, sh, ra, rb)
+    if wsb == 0:
+        check(_lib.ERR_UNSUPPORTED)
+    ws = _ws(wsb, c0.device)
+    out = torch.empty(P, dtype=torch.float64, device=c0.device)
+    pa = (C.c_void_p * (P * N))(*[c.data_ptr() for c in ca])
+    pb = (C.c_void_p * (P * N))(*[c.data_ptr() for c in cb])
+    with torch.cuda.device(c0.device):
+        check(L.tnb_tt_dot(code, pa, pb, P, N, sh, ra, rb, _ptr(out), _ptr(ws), wsb, _stream()))
+    return out
+
+
+def tt_dot(a_cores: Sequence[torch.Tensor], b_cores: Sequence[torch.Tensor]) -> torch.Tensor:
+    """<a, b> of two tensor trains of one shape as a 0-d float64 tensor on their device (tt_dot_batch with one pair)."""
+    return tt_dot_batch([(a_cores, b_cores)])[0]

@@ -1,6 +1,7 @@
 """Module-level mirrors of tntorch/round.py:7-187 (clone-then-round wrappers, truncated_svd)."""
 from __future__ import annotations
 
+import math
 from typing import Optional
 
 import torch
@@ -91,13 +92,23 @@ def reduce(ts, function, eps=0, rmax=None, algorithm="svd", verbose=False, **kwa
 
 
 def relative_error(gt, approx):
-    """metrics.py:135-151 for (dense torch tensor, Tensor)."""
+    """metrics.py:135-151.  (dense torch tensor, Tensor): one device reconstruct-and-diff call.  (Tensor, Tensor): both
+    are decompressed as before when their dense tensors fit in free device memory; otherwise (ops.dot_instead_of_dense)
+    the reference's formula on three TT dots from one call, sqrt(max(<g, g> + <a, a> - 2 <g, a>, 0) / max(<g, g>, 0)),
+    which cannot resolve errors below about 1e-8."""
     from .tensor import Tensor
 
     if isinstance(gt, torch.Tensor) and isinstance(approx, Tensor) and not approx.batch and all(c.dim() == 3 for c in approx.cores):
         if any(U is not None for U in approx.Us):
             approx = approx.decompress_tucker_factors()
         return ops.tt_relative_error(gt.to(approx.cores[0].device), approx.cores)
+    if isinstance(gt, Tensor) and isinstance(approx, Tensor) and not gt.batch and not approx.batch:
+        dense = math.prod(gt.shape) * gt.cores[0].element_size() + math.prod(approx.shape) * approx.cores[0].element_size()
+        free, _ = torch.cuda.mem_get_info(gt.cores[0].device)
+        if ops.dot_instead_of_dense(dense, int(free)):
+            a, b = gt._tt_cores(), approx._tt_cores()
+            gg, aa, ga = ops.tt_dot_batch([(a, a), (b, b), (a, b)])
+            return float(torch.sqrt((gg + aa - 2 * ga).clamp(0)) / torch.sqrt(gg.clamp(0)))
     a = gt.torch() if isinstance(gt, Tensor) else gt
     b = approx.torch() if isinstance(approx, Tensor) else approx
     return float(torch.dist(a, b) / torch.norm(a))

@@ -478,19 +478,36 @@ class Tensor(object):
                 self.right_orthogonalize(mu)
 
     def _tt_dot(self, other):
-        """<self, other> for two TT(-Tucker) tensors (metrics.dot): small interface matrices, fp64."""
-        a, b = self.decompress_tucker_factors(), other.decompress_tucker_factors()
-        f = torch.ones(1, 1, dtype=torch.float64, device=a.cores[0].device)
-        for ca, cb in zip(a.cores, b.cores):
-            f = torch.einsum("ab,aic,bid->cd", f, ca.double(), cb.double())
-        return f[0, 0]
+        """<self, other> for two TT(-Tucker, -CP) tensors (metrics.dot) as a 0-d float64 tensor: one library call
+        (ops.tt_dot) on the cores `_tt_cores()` gives."""
+        return ops.tt_dot(self._tt_cores(), other._tt_cores())
+
+    def dot(self, other, **kwargs):
+        """tensor.py:2104-2109: see callers.dot."""
+        from .callers import dot
+
+        return dot(self, other, **kwargs)
+
+    def norm(self):
+        """tensor.py:2139-2144: see callers.norm."""
+        from .callers import norm
+
+        return norm(self)
+
+    def normsq(self):
+        """tensor.py:2146-2151: see callers.normsq."""
+        from .callers import normsq
+
+        return normsq(self)
 
     def round(self, eps: float = 1e-14, **kwargs):
         """tensor.py:2085-2098: TT rounding, then Tucker rounding with the left-over error budget."""
         copy = self.clone()
         self.round_tt(eps, **kwargs)
-        d = (copy._tt_dot(copy) + self._tt_dot(self) - 2 * copy._tt_dot(self)).clamp(min=0)
-        reached = float(torch.sqrt(d) / torch.sqrt(copy._tt_dot(copy).clamp(min=0)))  # metrics.relative_error
+        a, b = copy._tt_cores(), self._tt_cores()
+        aa, bb, ab = ops.tt_dot_batch([(a, a), (b, b), (a, b)])  # the three dots of metrics.relative_error, one call
+        d = (aa + bb - 2 * ab).clamp(min=0)
+        reached = float(torch.sqrt(d) / torch.sqrt(aa.clamp(min=0)))
         if reached < eps:
             kw = {k: v for k, v in kwargs.items() if k in ("rmax", "algorithm")}
             self.round_tucker((1 + eps) / (1 + reached) - 1, **kw)
