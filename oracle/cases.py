@@ -219,6 +219,66 @@ TUCKER_CASES = {
     "tt_round_tucker_rmax": dict(kind="tt", spec=dict(shape=(12, 14, 10, 9), rank=5, seed=72, dtype="float64"), round_tucker=dict(rmax=4)),
     "tt_round_eps": dict(kind="tt", spec=dict(shape=(10,) * 5, rank=7, seed=24, dtype="float64"), round=dict(eps=0.3)),
 }
+# further reference cases of the same layer (their goldens in tucker.npz too), whose inputs also take the "cp" kind and the
+# Us / mode_rank / last_U_orthonormal fields of make_tucker_input; tests/test_gpu_tucker_paths.py runs every case of both
+TUCKER_PATH_CASES = {
+    # fp32 input, a capped rule on every mode
+    "dense_twin_f32_tucker4": dict(kind="dense", spec=dict(kind="tt_noise", shape=(12, 10, 8, 9, 7), rank=4, noise=1e-2, seed=5, dtype="float32"), ranks_tucker=4),
+    "dense_twin_f32_eps": dict(kind="dense", spec=dict(kind="tt_noise", shape=(12, 10, 8, 9, 7), rank=4, noise=1e-3, seed=7, dtype="float32"), eps=1e-2),
+    # Tensor(X, ranks_tucker=, ranks_tt=): round_tucker, then round_tt
+    "dense_twin_tucker_tt": dict(kind="dense", spec=dict(kind="tt_noise", shape=(12, 10, 8, 9, 7), rank=4, noise=1e-3, seed=73, dtype="float64"), ranks_tucker=5, ranks_tt=3),
+    # rmax lists with None entries, rmax with eps, dim as a subset and as an int
+    "tt_rmax_none_list": dict(kind="tt", spec=dict(shape=(12, 14, 10, 9), rank=5, seed=74, dtype="float64"), round_tucker=dict(rmax=[None, 3, None, 2])),
+    "tt_eps_rmax": dict(kind="tt", spec=dict(shape=(16,) * 4, rank=6, seed=75, dtype="float64"), round_tucker=dict(eps=0.2, rmax=[16, 5, 16, 16])),
+    "tt_dim_subset": dict(kind="tt", spec=dict(shape=(16,) * 4, rank=6, seed=76, dtype="float64"), round_tucker=dict(eps=0.2, dim=[0, 2])),
+    "tt_dim_int": dict(kind="tt", spec=dict(shape=(16,) * 4, rank=6, seed=77, dtype="float64"), round_tucker=dict(eps=0.2, dim=1)),
+    "tt_f32_eps": dict(kind="tt", spec=dict(shape=(16,) * 4, rank=6, seed=71, dtype="float32"), round_tucker=dict(eps=0.2)),
+    # one and two modes
+    "tt_N1": dict(kind="tt", spec=dict(shape=(30,), rank=1, seed=78, dtype="float64"), round_tucker=dict(eps=0.1)),
+    "tt_N2": dict(kind="tt", spec=dict(shape=(40, 30), rank=6, seed=79, dtype="float64"), round_tucker=dict(rmax=4)),
+    # TT-Tucker input (factors present, not orthonormal): rounded again
+    "tucker_round_again": dict(kind="tt", spec=dict(shape=(5, 6, 4, 5), rank=3, seed=80, dtype="float64", Us=(12, 14, 10, 9)), round_tucker=dict(rmax=[4, 3, 4, 3])),
+    # CP cores (first, middle and last) and CP cores under Tucker factors
+    "cp_round_tucker": dict(kind="cp", spec=dict(shape=(10, 9, 8, 7), R=5, seed=81, dtype="float64"), round_tucker=dict(rmax=3)),
+    "cp_tucker_round_tucker": dict(kind="cp", spec=dict(shape=(6, 5, 6), R=4, seed=82, dtype="float64", Us=(11, 12, 13)), round_tucker=dict(rmax=[4, 3, 4])),
+    # the eigensolver ladder of the factor split, by L = min(I, k): mixed Jacobi (the 10s), two-sided fp64 (72), one-sided
+    # in shared (100) and global memory (200), ChFSI (300 with rmax) and the adaptive solve (300, eps only, rank 30)
+    "tt_L72": dict(kind="tt", spec=dict(shape=(9, 72, 9), rank=9, seed=83, dtype="float64", mode_rank={1: 12}), round_tucker=dict(eps=1e-6)),
+    "tt_L100": dict(kind="tt", spec=dict(shape=(10, 100, 10), rank=10, seed=84, dtype="float64", mode_rank={1: 20}), round_tucker=dict(eps=1e-6)),
+    "tt_L200": dict(kind="tt", spec=dict(shape=(15, 200, 15), rank=15, seed=85, dtype="float64", mode_rank={1: 25}), round_tucker=dict(eps=1e-6)),
+    "tt_L300_chfsi": dict(kind="tt", spec=dict(shape=(18, 300, 18), rank=18, seed=86, dtype="float64", mode_rank={1: 30}), round_tucker=dict(rmax=[18, 20, 18])),
+    "tt_L300_adaptive": dict(kind="tt", spec=dict(shape=(18, 300, 18), rank=18, seed=87, dtype="float64", mode_rank={1: 30}), round_tucker=dict(eps=1e-4)),
+    # tn.round: the TT rounding reaches about 1e-8 (the dot formula's floor) of eps = 1e-4 on t + t and leaves the budget to round_tucker; with rmax = 2 it
+    # reaches far more than eps and round_tucker is skipped
+    "tt_round_leftover": dict(kind="tt", spec=dict(shape=(10, 11, 12, 13), rank=3, seed=88, dtype="float64", doubled=True), round=dict(eps=1e-4)),
+    # tn.round on a TT-Tucker input whose factors 0..N-2 are not orthonormal: round_tt must push them into the cores first
+    # (the reference pushes factors 0..N-2 only, tensor.py:2033, so the last one is drawn orthonormal)
+    "tucker_round": dict(kind="tt", spec=dict(shape=(5, 6, 4, 5), rank=4, seed=90, dtype="float64", Us=(12, 14, 10, 9), last_U_orthonormal=True), round=dict(eps=0.3)),
+    "tt_round_no_leftover": dict(kind="tt", spec=dict(shape=(10, 11, 12, 13), rank=6, seed=89, dtype="float64"), round=dict(eps=1e-3, rmax=2)),
+}
+
+
+def make_tucker_input(spec):
+    """(cores, Us) of a TUCKER_CASES entry of kind "tt" or "cp".  "tt": random TT cores (make_tt), optionally with mode
+    `mu`'s core projected onto a random `mode_rank[mu]`-dimensional subspace (its mode unfolding has that rank while
+    r0 r1 and I stay large), optionally under random (not orthonormal) factors Us[n] [I_n, S_n].  "cp": random CP
+    factors [S_n, R], optionally under factors.  Us is None where there is no factor."""
+    dtype = np.dtype(spec.get("dtype", "float64"))
+    rng = _rng(spec["seed"] + 1000)
+    if "R" in spec:
+        cores = [rng.standard_normal((S, spec["R"])).astype(dtype) for S in spec["shape"]]
+    else:
+        cores = make_tt(spec)
+        for mu, k in spec.get("mode_rank", {}).items():
+            c = cores[mu].astype(np.float64)
+            P = np.linalg.qr(rng.standard_normal((c.shape[1], k)))[0]
+            cores[mu] = np.einsum("aib,ij->ajb", c, P @ P.T).astype(dtype)
+    Us = [None] * len(cores)
+    if "Us" in spec:
+        Us = [rng.standard_normal((I, c.shape[-2])).astype(dtype) for I, c in zip(spec["Us"], cores)]
+        if spec.get("last_U_orthonormal"):
+            Us[-1] = np.linalg.qr(Us[-1].astype(np.float64))[0].astype(dtype)
+    return cores, Us
 
 
 # ---- full-size cases of BASELINE.json configs 2-4 (golden outputs: oracle/gen_golden_full.py -> tests/golden/full.npz) -----

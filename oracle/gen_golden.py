@@ -192,18 +192,25 @@ def gen_cpals():
 
 
 def gen_tucker():
+    """Regenerates tucker.npz; the keys of the cases already stored must come out bitwise as they were."""
+    from oracle import tt_oracle as orc
+
+    path = os.path.join(OUT, "tucker.npz")
+    old = dict(np.load(path)) if os.path.exists(path) else {}
     out = {}
-    torch.set_default_dtype(torch.float64)
-    for name, c in cases.TUCKER_CASES.items():
+    for name, c in {**cases.TUCKER_CASES, **cases.TUCKER_PATH_CASES}.items():
+        # the reference's CP -> TT conversion (tensor.py:1763) and identity factors (:1957) allocate in the default dtype
+        torch.set_default_dtype(torch.float32 if c["spec"].get("dtype") == "float32" else torch.float64)
         if c["kind"] == "dense":
             X = cases.make_dense(c["spec"])
-            kw = {k: c[k] for k in ("ranks_tucker", "eps") if k in c}
+            kw = {k: c[k] for k in ("ranks_tucker", "ranks_tt", "eps") if k in c}
             t = tn.Tensor(torch.as_tensor(X), **kw)
             dense = X
         else:
-            cores = cases.make_tt(c["spec"])
-            dense = cases.tt_full(cores)
-            t = tn.Tensor([torch.as_tensor(x.copy()) for x in cores])
+            cores, Us = cases.make_tucker_input(c["spec"])
+            dense = orc.tucker_full([x.copy() for x in cores], Us)
+            t = tn.Tensor([torch.as_tensor(x.copy()) for x in cores],
+                          Us=None if Us[0] is None else [torch.as_tensor(U.copy()) for U in Us])
             if "round_tucker" in c:
                 t.round_tucker(**c["round_tucker"])
             else:
@@ -213,7 +220,9 @@ def gen_tucker():
         out[f"{name}/relerr"] = np.float64(rel_err64(dense, t))
         print(name, list(t.ranks_tt), list(t.ranks_tucker), out[f"{name}/relerr"], flush=True)
     torch.set_default_dtype(torch.float32)
-    np.savez_compressed(os.path.join(OUT, "tucker.npz"), **out)
+    for k, v in old.items():
+        assert k in out and out[k].dtype == v.dtype and out[k].tobytes() == v.tobytes(), k
+    np.savez_compressed(path, **out)
 
 
 def gen_cross():

@@ -27,6 +27,16 @@ __all__ = [
     "relative_error",
     "py_maxvol",
     "py_rect_maxvol",
+    "cp_to_tt",
+    "factor_orthogonalize",
+    "orthogonalize",
+    "round_tt_tucker",
+    "round_tucker",
+    "round",
+    "tucker_from_dense",
+    "tucker_eps",
+    "tucker_core",
+    "tucker_full",
 ]
 
 
@@ -192,6 +202,170 @@ def relative_error(gt: np.ndarray, cores) -> float:
     """‖gt − T̂‖_F/‖gt‖_F with T̂ reconstructed and differenced in fp64."""
     gt64 = np.asarray(gt, dtype=np.float64)
     return float(np.linalg.norm(gt64 - tt_reconstruct(cores)) / np.linalg.norm(gt64))
+
+
+# --------------------------------------------------------------------------- #
+# Tucker factors, CP cores, Tucker rounding   (reference: tntorch/tensor.py:1717-2098)
+# A tensor is (cores, Us): cores [r0, S, r1] (TT) or [S, R] (CP), Us[n] [I, S] or None.
+# --------------------------------------------------------------------------- #
+def _cp_factor_to_core(factor):
+    """tensor.py:1741-1765, non-batch: a CP factor [I, R] -> the TT core [R, I, R] whose slices are diag(factor[i])."""
+    if factor.ndim == 3:  # already a TT core (:1741-1742)
+        return factor
+    I, R = factor.shape
+    core = np.zeros((R, I, R), dtype=factor.dtype)
+    core[np.arange(R), :, np.arange(R)] = factor.T
+    return core
+
+
+def cp_to_tt(cores):
+    """tensor.py:1728-1740 (factor=None): the first CP factor becomes [1, I, R], the middle ones diagonal [R, I, R]
+    cores, the last [R, I, 1].  In place on the list; returns it."""
+    if cores[0].ndim == 2:
+        cores[0] = cores[0][None, ...]
+    for mu in range(1, len(cores) - 1):
+        cores[mu] = _cp_factor_to_core(cores[mu])
+    if cores[-1].ndim == 2:
+        cores[-1] = cores[-1].T[..., None]
+    return cores
+
+
+def factor_orthogonalize(cores, Us, mu: int):
+    """tensor.py:1771-1798: U_mu = Q R, the core (TT or CP) absorbs R along its mode index."""
+    if Us[mu] is None:
+        return
+    Q, R = np.linalg.qr(Us[mu])  # :1783
+    Us[mu] = Q
+    if cores[mu].ndim == 2:
+        cores[mu] = np.einsum("jk,aj->ak", cores[mu], R)  # :1796
+    else:
+        cores[mu] = np.einsum("ijk,aj->iak", cores[mu], R)  # :1798
+
+
+def orthogonalize(cores, Us, mu: int):
+    """tensor.py:1881-1909 with the factor pushes of left_/right_orthogonalize (:1815, :1850): CP cores become TT
+    cores, then left QRs for 0..mu-1 and right QRs for N-1..mu+1.  Returns (R, L) as the reference does."""
+    N = len(cores)
+    if mu < 0:
+        mu += N
+    cp_to_tt(cores)
+    R = np.ones((1, 1))
+    L = np.ones((1, 1))
+    for i in range(mu):
+        factor_orthogonalize(cores, Us, i)
+        R = left_orthogonalize(cores, i)
+    for i in range(N - 1, mu, -1):
+        factor_orthogonalize(cores, Us, i)
+        L = right_orthogonalize(cores, i)
+    return R, L
+
+
+def round_tt_tucker(cores, Us, eps=1e-14, rmax=None, algorithm="svd"):
+    """tensor.py:2008-2083 on a tensor with Tucker factors: CP cores become TT cores (:2031), orthogonalize(N-1)
+    pushes the factors of modes 0..N-2 into their cores (:2033; the last factor stays as it is), then the TT
+    truncation sweep.  In place on the lists; returns them."""
+    N = len(cores)
+    cp_to_tt(cores)
+    for mu in range(N - 1):
+        factor_orthogonalize(cores, Us, mu)
+    round_tt(cores, eps=eps, rmax=rmax, algorithm=algorithm)
+    return cores, Us
+
+
+def round_tucker(cores, Us, eps=1e-14, rmax=None, dim="all", algorithm="svd"):
+    """tensor.py:1911-2006, non-batch.  In place on the lists `cores` and `Us`.  Returns, per mode in the order the
+    reference visits them (N-1 down to 0), what its factor split saw: the QR shape (r0 r1 x S), k, I, whether the mode
+    had a factor and a CP core before the call, the budget and rmax of its truncated_svd, the singular values of the
+    I x k matrix it split, and the rank it kept."""
+    N = len(cores)
+    if not hasattr(rmax, "__len__"):
+        rmax = [rmax] * N
+    assert len(rmax) == N
+    if dim == "all":
+        dim = range(N)
+    if not hasattr(dim, "__len__"):
+        dim = [dim] * N
+    had_U = [U is not None for U in Us]
+    was_cp = [c.ndim == 2 for c in cores]
+    for m in dim:  # :1942-1943: the CP factors of `dim` become diagonal cores, boundary ones included
+        cores[m] = _cp_factor_to_core(cores[m])
+    orthogonalize(cores, Us, -1)  # :1944
+    budget = eps / np.sqrt(len(dim))  # :1990
+    info = []
+    for mu in range(N - 1, -1, -1):
+        c = cores[mu]
+        r0, S, r1 = c.shape
+        if Us[mu] is None:
+            Us[mu] = np.eye(S, dtype=c.dtype)  # :1946-1957
+        Q, R = np.linalg.qr(c.transpose(0, 2, 1).reshape(-1, S))  # :1976-1983
+        cores[mu] = Q.reshape(r0, r1, -1).transpose(0, 2, 1)
+        Us[mu] = Us[mu] @ R.T  # :1985
+        sv = np.linalg.svd(Us[mu], compute_uv=False)
+        left, right = truncated_svd(Us[mu], eps=budget, rmax=rmax[mu], left_ortho=True, algorithm=algorithm)  # :1988
+        Us[mu] = left
+        cores[mu] = np.einsum("ijk,aj->iak", cores[mu], right)  # :2002
+        info.append(dict(mu=mu, rows=r0 * r1, S=S, k=Q.shape[1], I=Us[mu].shape[0], had_U=had_U[mu], cp=was_cp[mu],
+                         eps=budget, rmax=rmax[mu], sv=sv, rank=left.shape[1]))
+        if mu > 0:
+            factor_orthogonalize(cores, Us, mu)  # :2006 right_orthogonalize(mu)
+            right_orthogonalize(cores, mu)
+    return info
+
+
+def tucker_core(cores):
+    """tensor.py:1565-1574: the dense core tensor of the TT (or CP) cores, factors left out."""
+    return tt_reconstruct(cp_to_tt(list(cores)))
+
+
+def tucker_full(cores, Us):
+    """The dense tensor of (cores, Us): each factor absorbed into its core (tensor.py:1576-1627, 'ijk,aj->iak'), the
+    chain contracted with the boundary ranks summed (tensor.py:1639-1687)."""
+    cs = []
+    for c, U in zip(cp_to_tt(list(cores)), Us):
+        c = np.asarray(c, dtype=np.float64)
+        cs.append(c if U is None else np.einsum("ijk,aj->iak", c, np.asarray(U, dtype=np.float64)))
+    f = np.ones((1, cs[0].shape[0]))
+    for c in cs:
+        f = (f @ c.reshape(c.shape[0], -1)).reshape(-1, c.shape[2])
+    return f.sum(axis=-1).reshape([c.shape[1] for c in cs])
+
+
+def round(cores, Us, eps=1e-14, rmax=None, algorithm="svd"):
+    """tensor.py:2085-2098: TT rounding, then Tucker rounding with the budget left over, (1 + eps) / (1 + reached) - 1,
+    when the TT rounding reached less than eps.  In place on the lists; returns (reached, round_tucker's info or
+    None)."""
+    before = tucker_full(cores, Us)
+    round_tt_tucker(cores, Us, eps, rmax=rmax, algorithm=algorithm)
+    after = tucker_full(cores, Us)
+    reached = float(np.linalg.norm(before - after) / np.linalg.norm(before))  # metrics.relative_error (:2096)
+    info = None
+    if reached < eps:
+        info = round_tucker(cores, Us, (1 + eps) / (1 + reached) - 1, rmax=rmax, algorithm=algorithm)
+    return reached, info
+
+
+def tucker_from_dense(data, ranks_tucker, ranks_tt=None, algorithm="svd"):
+    """tn.Tensor(data, ranks_tucker=, ranks_tt=) (tensor.py:401-408): the exact TT (_full_rank_tt), round_tucker with
+    rmax = ranks_tucker, then round_tt with rmax = ranks_tt.  Returns (cores, Us, round_tucker's info)."""
+    cores = full_rank_tt(np.asarray(data))
+    Us = [None] * len(cores)
+    info = round_tucker(cores, Us, rmax=ranks_tucker, algorithm=algorithm)
+    if ranks_tt is not None:
+        round_tt_tucker(cores, Us, rmax=ranks_tt, algorithm=algorithm)
+    return cores, Us, info
+
+
+def tucker_eps(data, eps, algorithm="svd"):
+    """tn.Tensor(data, eps=) (tensor.py:436-439 -> round, :2085-2098): _full_rank_tt + round_tt(eps), which is
+    tt_svd(eps), then round_tucker with the budget left over.  Returns (cores, Us, reached, round_tucker's info or
+    None)."""
+    cores = tt_svd(np.asarray(data), eps=eps, algorithm=algorithm)
+    Us = [None] * len(cores)
+    reached = relative_error(data, cores) if len(cores) >= 2 else 0.0
+    info = None
+    if reached < eps:
+        info = round_tucker(cores, Us, (1 + eps) / (1 + reached) - 1, algorithm=algorithm)
+    return cores, Us, reached, info
 
 
 # --------------------------------------------------------------------------- #

@@ -7,6 +7,7 @@ Everything numerical runs in libtnb200.so on the GPU; there is no CPU path.
 """
 from __future__ import annotations
 
+import contextlib
 from typing import Any, Optional, Sequence, Union
 
 import numpy as np
@@ -427,6 +428,17 @@ class Tensor(object):
         return R, L
 
     # ------------------------------------------------------------------ rounding (tensor.py:2008-2098)
+    @contextlib.contextmanager
+    def _unchanged_on_error(self):
+        """A rounding that raises part way (a refused eigensolve) leaves the tensor as it was: the rounding steps only
+        rebind entries of `cores` / `Us`, never write into a tensor, so the lists of the start are put back."""
+        cores, Us = list(self.cores), list(self.Us)
+        try:
+            yield
+        except BaseException:
+            self.cores, self.Us = cores, Us
+            raise
+
     def round_tt(self, eps: float = 1e-14, rmax=None, algorithm: Optional[str] = "svd", verbose: Optional[bool] = False):
         """In place, by rebinding ``self.cores`` (same contract as the reference)."""
         assert algorithm in ("svd", "eig")
@@ -434,6 +446,11 @@ class Tensor(object):
         if not hasattr(rmax, "__len__"):
             rmax = [rmax] * (N - 1)
         assert len(rmax) == N - 1
+        with self._unchanged_on_error():
+            self._round_tt(eps, rmax)
+
+    def _round_tt(self, eps, rmax):
+        N = self.dim()
         self._cp_to_tt()  # tensor.py:2031: CP (or CP-Tucker) cores become TT (or TT-Tucker) ones
         for mu in range(N):  # orthogonalize() in the reference pushes the factors' non-orthogonal parts into the cores
             self.factor_orthogonalize(mu)
@@ -460,6 +477,11 @@ class Tensor(object):
             dim = range(N)
         if not hasattr(dim, "__len__"):
             dim = [dim] * N
+        with self._unchanged_on_error():
+            self._round_tucker(eps, rmax, dim)
+
+    def _round_tucker(self, eps, rmax, dim):
+        N = self.dim()
         self.orthogonalize(-1)
         for mu in range(N - 1, -1, -1):
             c = self.cores[mu]
@@ -503,11 +525,12 @@ class Tensor(object):
     def round(self, eps: float = 1e-14, **kwargs):
         """tensor.py:2085-2098: TT rounding, then Tucker rounding with the left-over error budget."""
         copy = self.clone()
-        self.round_tt(eps, **kwargs)
-        a, b = copy._tt_cores(), self._tt_cores()
-        aa, bb, ab = ops.tt_dot_batch([(a, a), (b, b), (a, b)])  # the three dots of metrics.relative_error, one call
-        d = (aa + bb - 2 * ab).clamp(min=0)
-        reached = float(torch.sqrt(d) / torch.sqrt(aa.clamp(min=0)))
-        if reached < eps:
-            kw = {k: v for k, v in kwargs.items() if k in ("rmax", "algorithm")}
-            self.round_tucker((1 + eps) / (1 + reached) - 1, **kw)
+        with self._unchanged_on_error():
+            self.round_tt(eps, **kwargs)
+            a, b = copy._tt_cores(), self._tt_cores()
+            aa, bb, ab = ops.tt_dot_batch([(a, a), (b, b), (a, b)])  # the three dots of metrics.relative_error, one call
+            d = (aa + bb - 2 * ab).clamp(min=0)
+            reached = float(torch.sqrt(d) / torch.sqrt(aa.clamp(min=0)))
+            if reached < eps:
+                kw = {k: v for k, v in kwargs.items() if k in ("rmax", "algorithm")}
+                self.round_tucker((1 + eps) / (1 + reached) - 1, **kw)
