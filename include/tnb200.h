@@ -492,6 +492,34 @@ int tnb_tt_dot(int dtype, const void* const* cores_a, const void* const* cores_b
                const int64_t* shape, const int32_t* ranks_a, const int32_t* ranks_b, double* out, void* workspace,
                size_t workspace_bytes, void* stream);
 
+/* Entries of ntrains tensor trains of one shape at npoints multi-indices, over the mode range [first, last):
+ *   out[t][a][p][b] = (G_first[:, i_p0, :] ... G_{last-1}[:, i_p(last-first-1), :])[a, b],
+ * out[t] row-major [r_first][npoints][r_last] of train t, the trains one after another, in the cores' dtype.  For the
+ * full range of a train with boundary ranks 1 this is the [1][P][1] core of tntorch's t[Xs]; an inner range is the fused
+ * core of t[:, idx, idx, :].  cores[t * ndim + k] is row-major [r_k][I_k][r_{k+1}] (only the range is read); each train
+ * has its own rank profile ranks[t * (ndim + 1) + k] (host).  idx is a device array, row-major [npoints][last - first]
+ * int64, shared by all trains.  dtype TNB_F32 or TNB_F64; any other returns TNB_ERR_UNSUPPORTED and sizes to 0.
+ * Null pointers, first >= last or outside [0, ndim], a mode size or rank below 1, or npoints < 1 are TNB_ERR_INVALID;
+ * ndim above 1024, a mode size at or above 2^31 - 1, a rank at or above 2^21, npoints * r_first at or above 2^31, or a
+ * core, state or output above 2^46 elements TNB_ERR_UNSUPPORTED; a workspace below tnb_tt_gather_workspace_bytes
+ * TNB_ERR_WORKSPACE; all before anything is launched.  Stream-ordered, no host synchronisation, no allocation.
+ * Index values are not checked: one outside [0, I_k) is never used to address a core and makes that point's outputs NaN.
+ * A point's value depends only on its own indices and the cores, so repeated calls are bitwise identical and shuffled
+ * points give shuffled outputs.
+ * Fused path (every train's npoints * r_first <= 4096, r_first * max r <= 2048, at most 64 modes): one launch per train,
+ * one CTA per point with its state in shared memory.  Grouped path otherwise: one launch narrowing the indices, then per
+ * train one launch for the first mode and four per later mode (histogram, scan, scatter of the rows by the mode's index,
+ * then one step that stages each core slice once per tile of rows sharing it); a step runs on the tensor cores (fp64
+ * mma.sync .f64, fp32 3xTF32) when r_k and r_{k+1} are in [16, 256], on CUDA-core tiles otherwise.  The workspace holds
+ * the narrowed indices, one permutation and tile list, and two state buffers of npoints * r_first * max r_k; never a
+ * copy of a core.
+ * Replaces: tntorch.Tensor.__getitem__ with index arrays (tensor.py:1019-1434), which forms core[:, idx, :] per mode. */
+size_t tnb_tt_gather_workspace_bytes(int dtype, int ntrains, int ndim, const int64_t* shape, const int32_t* ranks,
+                                     int first, int last, int64_t npoints);
+int tnb_tt_gather(int dtype, const void* const* cores, int ntrains, int ndim, const int64_t* shape,
+                  const int32_t* ranks, int first, int last, const int64_t* idx, int64_t npoints, void* out,
+                  void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

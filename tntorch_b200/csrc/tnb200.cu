@@ -16,6 +16,7 @@
 #include "expand_tc.cuh"
 #include "tt_multiply.cuh"
 #include "tt_dot.cuh"
+#include "tt_gather.cuh"
 
 using namespace tnb;
 
@@ -1068,6 +1069,43 @@ int tnb_tt_dot(int dtype, const void* const* cores_a, const void* const* cores_b
   return tt_dot_impl<float>(ar, false, reinterpret_cast<const float* const*>(cores_a),
                             reinterpret_cast<const float* const*>(cores_b), npairs, ndim, shape, ranks_a, ranks_b, out,
                             as_stream(stream));
+}
+
+// ------------------------------------------------------------------ entries of tensor trains at many multi-indices
+size_t tnb_tt_gather_workspace_bytes(int dtype, int ntrains, int ndim, const int64_t* shape, const int32_t* ranks,
+                                     int first, int last, int64_t npoints) {
+  if ((dtype != TNB_F32 && dtype != TNB_F64) || !shape || !ranks ||
+      ttg_check_dims(ntrains, ndim, shape, ranks, first, last, npoints) != TNB_OK)
+    return 0;
+  ArenaSizer ar;
+  int rc = dtype == TNB_F64 ? tt_gather_impl<double>(ar, true, nullptr, ntrains, ndim, shape, ranks, first, last,
+                                                     nullptr, npoints, nullptr, 0)
+                            : tt_gather_impl<float>(ar, true, nullptr, ntrains, ndim, shape, ranks, first, last, nullptr,
+                                                    npoints, nullptr, 0);
+  if (rc != TNB_OK) return 0;
+  return ar.off > 256 ? ar.off : 256;  // never 0 for a supported call: 0 is the refusal
+}
+
+int tnb_tt_gather(int dtype, const void* const* cores, int ntrains, int ndim, const int64_t* shape,
+                  const int32_t* ranks, int first, int last, const int64_t* idx, int64_t npoints, void* out,
+                  void* workspace, size_t workspace_bytes, void* stream) {
+  if (dtype != TNB_F32 && dtype != TNB_F64)
+    return fail(TNB_ERR_UNSUPPORTED, "tnb_tt_gather: dtype %d is not built (TNB_F32, TNB_F64)", dtype);
+  if (!cores || !shape || !ranks || !idx || !out || !workspace)
+    return fail(TNB_ERR_INVALID, "tnb_tt_gather: null argument");
+  TNB_TRY(ttg_check_dims(ntrains, ndim, shape, ranks, first, last, npoints));
+  for (int t = 0; t < ntrains; ++t)
+    for (int k = first; k < last; ++k)
+      if (!cores[(int64_t)t * ndim + k]) return fail(TNB_ERR_INVALID, "tnb_tt_gather: train %d core %d is null", t, k);
+  TNB_TRY(require_device());
+  if (workspace_bytes < tnb_tt_gather_workspace_bytes(dtype, ntrains, ndim, shape, ranks, first, last, npoints))
+    return fail(TNB_ERR_WORKSPACE, "tnb_tt_gather: workspace too small");
+  Arena ar(workspace, workspace_bytes);
+  if (dtype == TNB_F64)
+    return tt_gather_impl<double>(ar, false, reinterpret_cast<const double* const*>(cores), ntrains, ndim, shape, ranks,
+                                  first, last, idx, npoints, static_cast<double*>(out), as_stream(stream));
+  return tt_gather_impl<float>(ar, false, reinterpret_cast<const float* const*>(cores), ntrains, ndim, shape, ranks,
+                               first, last, idx, npoints, static_cast<float*>(out), as_stream(stream));
 }
 
 }  // extern "C"

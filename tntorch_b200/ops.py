@@ -8,6 +8,7 @@ from __future__ import annotations
 import ctypes as C
 from typing import List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -1139,6 +1140,103 @@ def tt_decompress(cores: Sequence[torch.Tensor], dtype: Optional[torch.dtype] = 
     return out
 
 
+def _gather_key(idx, shape, first: int, last: int, device, check: bool) -> torch.Tensor:
+    """idx as a contiguous int64 [P, last - first] tensor on `device`.  With `check`, an index outside [0, I_k) raises
+    IndexError before anything is launched: a host key is checked on the host, a device key by one reduction and one
+    host synchronisation."""
+    M = last - first
+    on_device = isinstance(idx, torch.Tensor) and idx.is_cuda
+    if isinstance(idx, torch.Tensor):
+        if idx.dtype not in (torch.int32, torch.int64):
+            raise ValueError(f"tt_gather: indices must be int32 or int64, got {idx.dtype}")
+        key = idx
+    else:
+        key = torch.as_tensor(np.asarray(idx))
+        if key.dtype not in (torch.int32, torch.int64):
+            raise ValueError(f"tt_gather: indices must be int32 or int64, got {key.dtype}")
+    if key.dim() == 1 and M == 1:
+        key = key[:, None]
+    if key.dim() != 2 or key.shape[1] != M or key.shape[0] < 1:
+        raise ValueError(f"tt_gather: indices must be [P >= 1, {M}], got {list(key.shape)}")
+    if check:
+        hi = torch.tensor(list(shape[first:last]), dtype=torch.int64, device=key.device)
+        bad = (key < 0) | (key >= hi)
+        if bad.any().item() if on_device else bool(bad.any()):
+            p, m = (int(v) for v in bad.nonzero()[0])
+            raise IndexError(f"index {int(key[p, m])} is out of bounds for mode {first + m} of size {shape[first + m]}")
+    if on_device and key.device != device:
+        raise ValueError("tt_gather: indices must be on the host or on the cores' device")
+    return key.to(device=device, dtype=torch.int64).contiguous()
+
+
+def tt_gather_batch(trains, idx, first: int = 0, last: Optional[int] = None, check: bool = True) -> torch.Tensor:
+    """Entries of B tensor trains of one shape at P multi-indices over the modes [first, last), from one library call
+    (tnb_tt_gather) that forms nothing but each point's running state: out[t, a, p, b] =
+    (G_first[:, i_p0, :] ... G_{last-1}[:, i_p(M-1), :])[a, b], as a [B, r_first, P, r_last] tensor in the cores' dtype
+    (float32 or float64).  The trains may differ in their inner ranks but not in r_first and r_last.  `idx` is
+    [P, last - first] int32 or int64, on the host (uploaded) or on the cores' device.  With `check=True` an index outside
+    [0, I_k) raises IndexError before anything launches; for a device key that costs one reduction and one host
+    synchronisation (the reference moves every key to the host).  With `check=False` the call has no host
+    synchronisation, and an out-of-range index gives NaN for its point."""
+    trains = [list(t) for t in trains]
+    if not trains or not trains[0]:
+        raise ValueError("tt_gather: no trains")
+    N = len(trains[0])
+    last = N if last is None else int(last)
+    first = int(first)
+    if not 0 <= first < last <= N:
+        raise ValueError(f"tt_gather: mode range [{first}, {last}) is not inside [0, {N})")
+    shape, ranks = None, []
+    for cores in trains:
+        if len(cores) != N or any(c.dim() != 3 for c in cores):
+            raise ValueError(f"tt_gather: every train must be {N} 3-D cores [r, I, r']")
+        if any(a.shape[2] != b.shape[0] for a, b in zip(cores[:-1], cores[1:])):
+            raise ValueError("tt_gather: core ranks do not match")
+        sh = [c.shape[1] for c in cores]
+        if shape is None:
+            shape = sh
+        elif sh != shape:
+            raise ValueError(f"tt_gather: every train must have the shape {shape}, got {sh}")
+        ranks += [cores[0].shape[0]] + [c.shape[2] for c in cores]
+    R = N + 1
+    ra, rl = ranks[first], ranks[last]
+    if any(ranks[t * R + first] != ra or ranks[t * R + last] != rl for t in range(len(trains))):
+        raise ValueError("tt_gather: every train must have the same ranks at the ends of the range")
+    c0 = trains[0][first]
+    _require_cuda(c0, "tt_gather")
+    allc = [c for cores in trains for c in cores[first:last]]
+    if any(c.device != c0.device for c in allc):
+        raise ValueError("tt_gather: cores must share one CUDA device")
+    if any(c.dtype != c0.dtype for c in allc) or c0.dtype not in _DT:
+        raise ValueError("tt_gather: cores must all be float32 or all float64")
+    if any(c.requires_grad for c in allc):
+        raise ValueError("tt_gather: cores that require grad are not supported")
+    key = _gather_key(idx, shape, first, last, c0.device, check)
+    P, B = key.shape[0], len(trains)
+    cs = [c.contiguous() if first <= k < last else c for cores in trains for k, c in enumerate(cores)]
+    code = _DT[c0.dtype]
+    L = lib()
+    sh, rk = i64(shape), i32(ranks)
+    wsb = L.tnb_tt_gather_workspace_bytes(code, B, N, sh, rk, first, last, P)
+    if wsb == 0:
+        _lib.check(_lib.ERR_UNSUPPORTED)
+    ws = _ws(wsb, c0.device)
+    out = torch.empty(B, ra, P, rl, dtype=c0.dtype, device=c0.device)
+    ptrs = (C.c_void_p * (B * N))(*[c.data_ptr() for c in cs])
+    with torch.cuda.device(c0.device):
+        _lib.check(L.tnb_tt_gather(code, ptrs, B, N, sh, rk, first, last, _ptr(key), P, _ptr(out), _ptr(ws), wsb,
+                              _stream()))
+    return out
+
+
+def tt_gather(cores: Sequence[torch.Tensor], idx, first: int = 0, last: Optional[int] = None,
+              check: bool = True) -> torch.Tensor:
+    """Entries of one tensor train at P multi-indices over the modes [first, last) as [r_first, P, r_last]
+    (tt_gather_batch with one train).  For the full range of a train with boundary ranks 1, out[0, :, 0] are the values
+    tntorch's t[Xs].torch() returns."""
+    return tt_gather_batch([cores], idx, first, last, check)[0]
+
+
 def tt_multiply(cores: Sequence[torch.Tensor], X: torch.Tensor) -> torch.Tensor:
     """Y = X.reshape(-1, I) @ M for the TT-matrix M of cores [r_k, i_k, o_k, r_{k+1}] (one dtype, one CUDA device,
     boundary ranks 1), in one library call (tnb_tt_multiply) that never forms M: stream-ordered, no host
@@ -1258,3 +1356,4 @@ def tt_dot_batch(pairs) -> torch.Tensor:
 def tt_dot(a_cores: Sequence[torch.Tensor], b_cores: Sequence[torch.Tensor]) -> torch.Tensor:
     """<a, b> of two tensor trains of one shape as a 0-d float64 tensor on their device (tt_dot_batch with one pair)."""
     return tt_dot_batch([(a_cores, b_cores)])[0]
+

@@ -499,6 +499,13 @@ class Tensor(object):
             if mu > 0:
                 self.right_orthogonalize(mu)
 
+    def __getitem__(self, key):
+        """tensor.py:1019-1434: NumPy-style indexing (see getitem.py); index arrays and integers are read by
+        ops.tt_gather without forming core[:, idx, :]."""
+        from .getitem import getitem
+
+        return getitem(self, key)
+
     def _tt_dot(self, other):
         """<self, other> for two TT(-Tucker, -CP) tensors (metrics.dot) as a 0-d float64 tensor: one library call
         (ops.tt_dot) on the cores `_tt_cores()` gives."""
