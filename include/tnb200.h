@@ -520,6 +520,37 @@ int tnb_tt_gather(int dtype, const void* const* cores, int ntrains, int ndim, co
                   const int32_t* ranks, int first, int last, const int64_t* idx, int64_t npoints, void* out,
                   void* workspace, size_t workspace_bytes, void* stream);
 
+/* The gradient of tnb_tt_gather with respect to the cores of the range, for the same arguments and limits, given
+ * grad_out (the layout of tnb_tt_gather's out, in the cores' dtype): grad_cores[t * ndim + k], for k in [first, last),
+ * row-major [r_k][I_k][r_{k+1}], is fully overwritten with dG_k[:, i, :] = sum over the points with index i at mode k of
+ * L_k^T W_k (L_k the product of the slices before mode k, W_k grad_out times the transposed slices after it); slices no
+ * point reaches are zero.  Entries outside the range are not read and may be null.  dtype TNB_F32 or TNB_F64; any other
+ * returns TNB_ERR_UNSUPPORTED and sizes to 0.  Malformed arguments get tnb_tt_gather's codes, a null grad_out,
+ * grad_cores or range entry of it TNB_ERR_INVALID, all before anything is launched.  Stream-ordered, no host
+ * synchronisation, no allocation, bitwise reproducible: the points are put in a stable order by each mode's index (a
+ * radix sort that depends on idx only) and every sum runs in a fixed order, with no atomics on a value.  A point with
+ * any index outside its mode takes no part in any gradient and never addresses a core.
+ * Launches per call: one narrowing the indices; per mode one bucket count and, per 8-bit digit of I_k (one for
+ * I_k < 256), three sort launches (digit histogram, scan, stable scatter); then per train: one tile-list launch per
+ * mode after the first and one chunk-list launch per mode, one for the first mode's state and one forward step per
+ * later mode but the last (recomputing each L_k), one loading grad_out, and per mode, from the last, one reduction
+ * (a segmented L_k^T W_k GEMM over the rows of each index value, in chunks sized from the shapes and P) and one
+ * combination of multi-chunk partials (summed in chunk order, in fp64), and above the first mode one reverse step
+ * W_{k-1} = W_k G_k[:, i, :]^T.  Steps and reductions run on the tensor cores (fp64 mma.sync .f64, fp32 3xTF32) when
+ * r_k and r_{k+1} are in [16, 256], on CUDA-core tiles otherwise.  The grad_cores are zeroed with cudaMemsetAsync.
+ * The workspace holds the narrowed indices, the per-mode bucket counts and stable orders (M * npoints int32), a sort
+ * buffer and its digit histograms, one train's tile and chunk lists, the kept L_k (npoints * r_first * sum r_k over the
+ * modes after the first), two W buffers of npoints * r_first * max r_{k+1} and one mode's chunk partials (below
+ * 2 * npoints * r_first / chunk slices); never a copy of a core.
+ * Replaces: autograd through tntorch's t[Xs] chain of core[:, idx, :] products (tensor.py:1286-1330), which keeps every
+ * mode's [r, P, r] slice tensor until backward. */
+size_t tnb_tt_gather_grad_workspace_bytes(int dtype, int ntrains, int ndim, const int64_t* shape, const int32_t* ranks,
+                                          int first, int last, int64_t npoints);
+int tnb_tt_gather_grad(int dtype, const void* const* cores, int ntrains, int ndim, const int64_t* shape,
+                       const int32_t* ranks, int first, int last, const int64_t* idx, int64_t npoints,
+                       const void* grad_out, void* const* grad_cores, void* workspace, size_t workspace_bytes,
+                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -137,6 +137,10 @@ SIGNATURES = {
     "tnb_tt_gather_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, _i64p, _i32p, C.c_int, C.c_int, C.c_int64]),
     "tnb_tt_gather": (C.c_int, [C.c_int, C.POINTER(_vp), C.c_int, C.c_int, _i64p, _i32p, C.c_int, C.c_int, _vp,
                                 C.c_int64, _vp, _vp, C.c_size_t, _vp]),
+    "tnb_tt_gather_grad_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, _i64p, _i32p, C.c_int, C.c_int,
+                                                        C.c_int64]),
+    "tnb_tt_gather_grad": (C.c_int, [C.c_int, C.POINTER(_vp), C.c_int, C.c_int, _i64p, _i32p, C.c_int, C.c_int, _vp,
+                                     C.c_int64, _vp, C.POINTER(_vp), _vp, C.c_size_t, _vp]),
 }
 
 

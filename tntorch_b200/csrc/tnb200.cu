@@ -17,6 +17,7 @@
 #include "tt_multiply.cuh"
 #include "tt_dot.cuh"
 #include "tt_gather.cuh"
+#include "tt_gather_grad.cuh"
 
 using namespace tnb;
 
@@ -1106,6 +1107,47 @@ int tnb_tt_gather(int dtype, const void* const* cores, int ntrains, int ndim, co
                                   first, last, idx, npoints, static_cast<double*>(out), as_stream(stream));
   return tt_gather_impl<float>(ar, false, reinterpret_cast<const float* const*>(cores), ntrains, ndim, shape, ranks,
                                first, last, idx, npoints, static_cast<float*>(out), as_stream(stream));
+}
+
+// ------------------------------------------------------------------ the gradient of tnb_tt_gather
+size_t tnb_tt_gather_grad_workspace_bytes(int dtype, int ntrains, int ndim, const int64_t* shape, const int32_t* ranks,
+                                          int first, int last, int64_t npoints) {
+  if ((dtype != TNB_F32 && dtype != TNB_F64) || !shape || !ranks ||
+      ttg_check_dims(ntrains, ndim, shape, ranks, first, last, npoints) != TNB_OK)
+    return 0;
+  ArenaSizer ar;
+  int rc = dtype == TNB_F64 ? tt_gather_grad_impl<double>(ar, true, nullptr, ntrains, ndim, shape, ranks, first, last,
+                                                          nullptr, npoints, nullptr, nullptr, 0)
+                            : tt_gather_grad_impl<float>(ar, true, nullptr, ntrains, ndim, shape, ranks, first, last,
+                                                         nullptr, npoints, nullptr, nullptr, 0);
+  if (rc != TNB_OK) return 0;
+  return ar.off > 256 ? ar.off : 256;
+}
+
+int tnb_tt_gather_grad(int dtype, const void* const* cores, int ntrains, int ndim, const int64_t* shape,
+                       const int32_t* ranks, int first, int last, const int64_t* idx, int64_t npoints,
+                       const void* grad_out, void* const* grad_cores, void* workspace, size_t workspace_bytes,
+                       void* stream) {
+  if (dtype != TNB_F32 && dtype != TNB_F64)
+    return fail(TNB_ERR_UNSUPPORTED, "tnb_tt_gather_grad: dtype %d is not built (TNB_F32, TNB_F64)", dtype);
+  if (!cores || !shape || !ranks || !idx || !grad_out || !grad_cores || !workspace)
+    return fail(TNB_ERR_INVALID, "tnb_tt_gather_grad: null argument");
+  TNB_TRY(ttg_check_dims(ntrains, ndim, shape, ranks, first, last, npoints));
+  for (int t = 0; t < ntrains; ++t)
+    for (int k = first; k < last; ++k)
+      if (!cores[(int64_t)t * ndim + k] || !grad_cores[(int64_t)t * ndim + k])
+        return fail(TNB_ERR_INVALID, "tnb_tt_gather_grad: train %d core %d or its gradient is null", t, k);
+  TNB_TRY(require_device());
+  if (workspace_bytes < tnb_tt_gather_grad_workspace_bytes(dtype, ntrains, ndim, shape, ranks, first, last, npoints))
+    return fail(TNB_ERR_WORKSPACE, "tnb_tt_gather_grad: workspace too small");
+  Arena ar(workspace, workspace_bytes);
+  if (dtype == TNB_F64)
+    return tt_gather_grad_impl<double>(ar, false, reinterpret_cast<const double* const*>(cores), ntrains, ndim, shape,
+                                       ranks, first, last, idx, npoints, static_cast<const double*>(grad_out),
+                                       reinterpret_cast<double* const*>(grad_cores), as_stream(stream));
+  return tt_gather_grad_impl<float>(ar, false, reinterpret_cast<const float* const*>(cores), ntrains, ndim, shape, ranks,
+                                    first, last, idx, npoints, static_cast<const float*>(grad_out),
+                                    reinterpret_cast<float* const*>(grad_cores), as_stream(stream));
 }
 
 }  // extern "C"

@@ -262,8 +262,24 @@ __device__ __forceinline__ T* ttg_dst(const TtgStep& s, T* nxt, T* out, int rid,
   return nxt + (int64_t)rid * s.rk1 + c;
 }
 
+// Row `j` of a step's bucket order: perm holds row ids, or with PPERM point ids (the backward's stable order), row j
+// being row j % r_first of the point at j / r_first.
+template <bool PPERM>
+__device__ __forceinline__ int ttg_rid(const TtgStep& s, int j) {
+  if constexpr (PPERM) return s.perm[j / s.ra] * s.ra + j % s.ra;
+  return s.perm[j];
+}
+
+// Slice entry (k, c) of the step's right operand: G[k, i, c], or with TRANS (the backward's reverse step, whose rk
+// columns are r_{k+1} and rk1 columns r_k) G[c, i, k], the slice transposed.
+template <bool TRANS, typename T>
+__device__ __forceinline__ T ttg_slice(const TtgStep& s, const T* G, int i, int k, int c) {
+  if constexpr (TRANS) return G[((int64_t)c * s.n + i) * s.rk + k];
+  return G[((int64_t)k * s.n + i) * s.rk1 + c];
+}
+
 // The step on CUDA cores: each thread 4 rows x 4 columns (rows ty + 16 u, columns tx + 16 v).
-template <typename T>
+template <typename T, bool PPERM = false, bool TRANS = false>
 __global__ void __launch_bounds__(TTG_THREADS) ttg_step_generic_kernel(const TtgStep s, const T* __restrict__ G,
                                                                        const T* __restrict__ cur, T* nxt, T* out) {
   __shared__ T Ss[TTG_T][TTG_BK + 1];
@@ -274,7 +290,7 @@ __global__ void __launch_bounds__(TTG_THREADS) ttg_step_generic_kernel(const Ttg
   const int* te = s.tiles + 3 * (int64_t)tile;
   const int i = te[0], row0 = te[1], cnt = te[2];
   const int c0 = blockIdx.y * TTG_BN, tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
-  if (tid < TTG_T) rids[tid] = tid < cnt ? s.perm[row0 + tid] : 0;
+  if (tid < TTG_T) rids[tid] = tid < cnt ? ttg_rid<PPERM>(s, row0 + tid) : 0;
   __syncthreads();
   if (i >= s.n) {  // out-of-range index: NaN
     for (int e = tid; e < cnt * TTG_BN; e += TTG_THREADS) {
@@ -294,8 +310,9 @@ __global__ void __launch_bounds__(TTG_THREADS) ttg_step_generic_kernel(const Ttg
       Ss[r][kk] = (r < cnt && k < s.rk) ? cur[(int64_t)rids[r] * s.rk + k] : (T)0;
     }
     for (int e = tid; e < TTG_BK * TTG_BN; e += TTG_THREADS) {
-      const int kk = e / TTG_BN, cc = e % TTG_BN, k = k0 + kk, c = c0 + cc;
-      Gs[kk][cc] = (k < s.rk && c < s.rk1) ? G[((int64_t)k * s.n + i) * s.rk1 + c] : (T)0;
+      // transposed, consecutive threads walk k, the slice's contiguous index
+      const int kk = TRANS ? e % TTG_BK : e / TTG_BN, cc = TRANS ? e / TTG_BK : e % TTG_BN, k = k0 + kk, c = c0 + cc;
+      Gs[kk][cc] = (k < s.rk && c < s.rk1) ? ttg_slice<TRANS>(s, G, i, k, c) : (T)0;
     }
     __syncthreads();
     const int kl = min(TTG_BK, s.rk - k0);
@@ -324,10 +341,52 @@ __global__ void __launch_bounds__(TTG_THREADS) ttg_step_generic_kernel(const Ttg
   }
 }
 
+// One staged 64 x 32 by 32 x 64 block product on the tensor cores, accumulated into a warp's 16 x 32 share of the
+// 64 x 64 block: rows mrow .. + 16, n8 tiles at ncol .. + 32 (fp64 k16 DMMA steps; fp32 k8 3xTF32 steps on hi / lo).
+template <typename T, typename Acc>
+__device__ __forceinline__ void ttg_mma_block(Acc (&acc)[4][4], const T (*Ss)[TTG_T][TTG_SS], const T (*Gs)[TTG_BK][TTG_SG],
+                                              int mrow, int ncol, int g, int t) {
+  constexpr bool F64 = sizeof(T) == 8;
+  if constexpr (F64) {
+#pragma unroll
+    for (int ks = 0; ks < TTG_BK; ks += 16) {
+      double a[8];
+#pragma unroll
+      for (int q = 0; q < 8; ++q) a[q] = Ss[0][mrow + g + 8 * (q & 1)][ks + t + 4 * (q >> 1)];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        double b[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) b[q] = Gs[0][ks + t + 4 * q][ncol + 8 * j + g];
+        dmma_16816(acc[j], a, b);
+      }
+    }
+  } else {
+#pragma unroll
+    for (int ks = 0; ks < TTG_BK; ks += 8) {
+      uint32_t ah[4], al[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const int r = mrow + g + 8 * (q & 1), k = ks + t + 4 * (q >> 1);
+        ah[q] = __float_as_uint(Ss[0][r][k]), al[q] = __float_as_uint(Ss[1][r][k]);
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const int c = ncol + 8 * j + g;
+        const uint32_t bh0 = __float_as_uint(Gs[0][ks + t][c]), bh1 = __float_as_uint(Gs[0][ks + t + 4][c]);
+        const uint32_t bl0 = __float_as_uint(Gs[1][ks + t][c]), bl1 = __float_as_uint(Gs[1][ks + t + 4][c]);
+        mma_tf32(acc[j], ah[0], ah[1], ah[2], ah[3], bl0, bl1);  // S_hi G_lo
+        mma_tf32(acc[j], al[0], al[1], al[2], al[3], bh0, bh1);  // S_lo G_hi
+        mma_tf32(acc[j], ah[0], ah[1], ah[2], ah[3], bh0, bh1);  // S_hi G_hi
+      }
+    }
+  }
+}
+
 // The step on the tensor cores.  Eight warps over the 64 x 64 output block: warp w takes rows 16 (w & 3) .. + 16 and
 // n8 tiles 4 (w >> 2) .. + 4.  fp64: k16 DMMA steps on the staged operands.  fp32: k8 3xTF32 steps, each operand
 // stored hi / lo (rounded to nearest) as it is staged.
-template <typename T>
+template <typename T, bool PPERM = false, bool TRANS = false>
 __global__ void __launch_bounds__(TTG_THREADS) ttg_step_tc_kernel(const TtgStep s, const T* __restrict__ G,
                                                                   const T* __restrict__ cur, T* nxt, T* out) {
   constexpr bool F64 = sizeof(T) == 8;
@@ -342,7 +401,7 @@ __global__ void __launch_bounds__(TTG_THREADS) ttg_step_tc_kernel(const TtgStep 
   const int c0 = blockIdx.y * TTG_BN, tid = threadIdx.x;
   const int w = tid >> 5, lane = tid & 31, g = lane >> 2, t = lane & 3;
   const int mrow = 16 * (w & 3), ncol = 32 * (w >> 2);
-  if (tid < TTG_T) rids[tid] = tid < cnt ? s.perm[row0 + tid] : 0;
+  if (tid < TTG_T) rids[tid] = tid < cnt ? ttg_rid<PPERM>(s, row0 + tid) : 0;
   __syncthreads();
   if (i >= s.n) {
     for (int e = tid; e < cnt * TTG_BN; e += TTG_THREADS) {
@@ -369,8 +428,8 @@ __global__ void __launch_bounds__(TTG_THREADS) ttg_step_tc_kernel(const TtgStep 
       }
     }
     for (int e = tid; e < TTG_BK * TTG_BN; e += TTG_THREADS) {
-      const int kk = e / TTG_BN, cc = e % TTG_BN, k = k0 + kk, c = c0 + cc;
-      const T v = (k < s.rk && c < s.rk1) ? G[((int64_t)k * s.n + i) * s.rk1 + c] : (T)0;
+      const int kk = TRANS ? e % TTG_BK : e / TTG_BN, cc = TRANS ? e / TTG_BK : e % TTG_BN, k = k0 + kk, c = c0 + cc;
+      const T v = (k < s.rk && c < s.rk1) ? ttg_slice<TRANS>(s, G, i, k, c) : (T)0;
       if constexpr (F64) {
         Gs[0][kk][cc] = v;
       } else {
@@ -379,40 +438,7 @@ __global__ void __launch_bounds__(TTG_THREADS) ttg_step_tc_kernel(const TtgStep 
       }
     }
     __syncthreads();
-    if constexpr (F64) {
-#pragma unroll
-      for (int ks = 0; ks < TTG_BK; ks += 16) {
-        double a[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) a[q] = Ss[0][mrow + g + 8 * (q & 1)][ks + t + 4 * (q >> 1)];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          double b[4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) b[q] = Gs[0][ks + t + 4 * q][ncol + 8 * j + g];
-          dmma_16816(acc[j], a, b);
-        }
-      }
-    } else {
-#pragma unroll
-      for (int ks = 0; ks < TTG_BK; ks += 8) {
-        uint32_t ah[4], al[4];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const int r = mrow + g + 8 * (q & 1), k = ks + t + 4 * (q >> 1);
-          ah[q] = __float_as_uint(Ss[0][r][k]), al[q] = __float_as_uint(Ss[1][r][k]);
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const int c = ncol + 8 * j + g;
-          const uint32_t bh0 = __float_as_uint(Gs[0][ks + t][c]), bh1 = __float_as_uint(Gs[0][ks + t + 4][c]);
-          const uint32_t bl0 = __float_as_uint(Gs[1][ks + t][c]), bl1 = __float_as_uint(Gs[1][ks + t + 4][c]);
-          mma_tf32(acc[j], ah[0], ah[1], ah[2], ah[3], bl0, bl1);  // S_hi G_lo
-          mma_tf32(acc[j], al[0], al[1], al[2], al[3], bh0, bh1);  // S_lo G_hi
-          mma_tf32(acc[j], ah[0], ah[1], ah[2], ah[3], bh0, bh1);  // S_hi G_hi
-        }
-      }
-    }
+    ttg_mma_block<T>(acc, Ss, Gs, mrow, ncol, g, t);
     __syncthreads();
   }
   // c fragment: e at row g + 8 (e >> 1), column 2 t + (e & 1) of each n8 tile

@@ -13,7 +13,9 @@ Results have the reference's type and core shapes (for TT and Tucker tensors):
 Tucker factors of integer and index modes are absorbed into their cores first; CP cores are turned into TT cores, so a
 CP tensor gives the reference's values in TT cores.  On a batch tensor the first key entry indexes the batch: an integer
 gives a non-batch result, a slice a batch one whose gathers are one ops.tt_gather_batch call each.  When a core or a
-factor requires grad, the gathers and joins are the reference's torch formulation, so that autograd sees them.
+factor requires grad, the gathers of fp32 and fp64 cores stay library calls, differentiated by one tnb_tt_gather_grad
+call each; Tucker absorption and the joins of integer runs are torch products then, so autograd reaches the factors
+(and CP factors through _cp_to_tt).  Cores of any other dtype take the reference's torch chain under grad.
 """
 from __future__ import annotations
 
@@ -116,7 +118,8 @@ class _View:
         """[.., r_f, P, r_l]: the product of the slices of modes f..l-1 at the P points `cols` (one index tensor per
         mode)."""
         cores = [self.absorbed(k) for k in range(f, l)]
-        if self.grad:  # the reference's chain of core[:, idx, :] products (tensor.py:1286-1330)
+        if self.grad and cores[0].dtype not in (torch.float32, torch.float64):
+            # a dtype the library does not take: the reference's chain of core[:, idx, :] products (tensor.py:1286-1330)
             dev = cores[0].device
             s = cores[0][..., cols[0].to(dev), :]
             for c, ix in zip(cores[1:], cols[1:]):

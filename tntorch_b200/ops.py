@@ -1177,7 +1177,11 @@ def tt_gather_batch(trains, idx, first: int = 0, last: Optional[int] = None, che
     [P, last - first] int32 or int64, on the host (uploaded) or on the cores' device.  With `check=True` an index outside
     [0, I_k) raises IndexError before anything launches; for a device key that costs one reduction and one host
     synchronisation (the reference moves every key to the host).  With `check=False` the call has no host
-    synchronisation, and an out-of-range index gives NaN for its point."""
+    synchronisation, and an out-of-range index gives NaN for its point.
+    When grad mode is on and a core of the range requires grad, the result is differentiable with respect to the
+    range's cores: the backward is one library call (tnb_tt_gather_grad) on the key the forward validated, without a
+    second check or a host synchronisation; a point with an out-of-range index (check=False) adds nothing to any
+    gradient.  It is differentiable once: a double backward raises."""
     trains = [list(t) for t in trains]
     if not trains or not trains[0]:
         raise ValueError("tt_gather: no trains")
@@ -1209,24 +1213,80 @@ def tt_gather_batch(trains, idx, first: int = 0, last: Optional[int] = None, che
         raise ValueError("tt_gather: cores must share one CUDA device")
     if any(c.dtype != c0.dtype for c in allc) or c0.dtype not in _DT:
         raise ValueError("tt_gather: cores must all be float32 or all float64")
-    if any(c.requires_grad for c in allc):
-        raise ValueError("tt_gather: cores that require grad are not supported")
     key = _gather_key(idx, shape, first, last, c0.device, check)
-    P, B = key.shape[0], len(trains)
-    cs = [c.contiguous() if first <= k < last else c for cores in trains for k, c in enumerate(cores)]
-    code = _DT[c0.dtype]
-    L = lib()
-    sh, rk = i64(shape), i32(ranks)
-    wsb = L.tnb_tt_gather_workspace_bytes(code, B, N, sh, rk, first, last, P)
-    if wsb == 0:
-        _lib.check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, c0.device)
-    out = torch.empty(B, ra, P, rl, dtype=c0.dtype, device=c0.device)
-    ptrs = (C.c_void_p * (B * N))(*[c.data_ptr() for c in cs])
-    with torch.cuda.device(c0.device):
-        _lib.check(L.tnb_tt_gather(code, ptrs, B, N, sh, rk, first, last, _ptr(key), P, _ptr(out), _ptr(ws), wsb,
-                              _stream()))
-    return out
+    plan = _GatherPlan(len(trains), N, shape, ranks, first, last, key)
+    if torch.is_grad_enabled() and any(c.requires_grad for c in allc):
+        return _TtGather.apply(plan, *allc)
+    return plan.forward([c for cores in trains for c in cores[first:last]])
+
+
+class _GatherPlan:
+    """One tt_gather call's shapes and validated device key, shared by its forward and its backward."""
+
+    def __init__(self, B, N, shape, ranks, first, last, key):
+        self.B, self.N, self.shape, self.ranks, self.first, self.last, self.key = B, N, shape, ranks, first, last, key
+        self.P = key.shape[0]
+
+    def _ptrs(self, range_tensors):
+        """The B x N pointer table of the range's tensors (B x (last - first), train-major); null outside the range."""
+        M = self.last - self.first
+        table = [None] * (self.B * self.N)
+        for t in range(self.B):
+            for m in range(M):
+                table[t * self.N + self.first + m] = range_tensors[t * M + m].data_ptr()
+        return (C.c_void_p * len(table))(*table)
+
+    def forward(self, cores):
+        c0 = cores[0]
+        cs = [c.contiguous() for c in cores]
+        code, L = _DT[c0.dtype], lib()
+        sh, rk = i64(self.shape), i32(self.ranks)
+        B, N, first, last, P = self.B, self.N, self.first, self.last, self.P
+        wsb = L.tnb_tt_gather_workspace_bytes(code, B, N, sh, rk, first, last, P)
+        if wsb == 0:
+            _lib.check(_lib.ERR_UNSUPPORTED)
+        ws = _ws(wsb, c0.device)
+        out = torch.empty(B, self.ranks[first], P, self.ranks[last], dtype=c0.dtype, device=c0.device)
+        with torch.cuda.device(c0.device):
+            _lib.check(L.tnb_tt_gather(code, self._ptrs(cs), B, N, sh, rk, first, last, _ptr(self.key), P, _ptr(out),
+                                       _ptr(ws), wsb, _stream()))
+        return out
+
+    def backward(self, cores, grad_out):
+        """The gradients of the range's cores (tnb_tt_gather_grad), in the order of `cores`."""
+        c0 = cores[0]
+        cs = [c.contiguous() for c in cores]
+        gout = grad_out.to(c0.dtype).contiguous()
+        grads = [torch.empty(c.shape, dtype=c.dtype, device=c.device) for c in cs]
+        code, L = _DT[c0.dtype], lib()
+        sh, rk = i64(self.shape), i32(self.ranks)
+        B, N, first, last, P = self.B, self.N, self.first, self.last, self.P
+        wsb = L.tnb_tt_gather_grad_workspace_bytes(code, B, N, sh, rk, first, last, P)
+        if wsb == 0:
+            _lib.check(_lib.ERR_UNSUPPORTED)
+        ws = _ws(wsb, c0.device)
+        with torch.cuda.device(c0.device):
+            _lib.check(L.tnb_tt_gather_grad(code, self._ptrs(cs), B, N, sh, rk, first, last, _ptr(self.key), P,
+                                            _ptr(gout), self._ptrs(grads), _ptr(ws), wsb, _stream()))
+        return grads
+
+
+class _TtGather(torch.autograd.Function):
+    """tt_gather_batch under autograd: the forward is one tnb_tt_gather call, the backward one tnb_tt_gather_grad
+    call on the key the forward validated (no second check, no host synchronisation)."""
+
+    @staticmethod
+    def forward(ctx, plan, *cores):
+        ctx.plan = plan
+        ctx.save_for_backward(*cores)
+        return plan.forward(list(cores))
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_out):
+        cores = ctx.saved_tensors
+        grads = ctx.plan.backward(list(cores), grad_out)
+        return (None,) + tuple(g if need else None for g, need in zip(grads, ctx.needs_input_grad[1:]))
 
 
 def tt_gather(cores: Sequence[torch.Tensor], idx, first: int = 0, last: Optional[int] = None,
