@@ -551,6 +551,42 @@ int tnb_tt_gather_grad(int dtype, const void* const* cores, int ntrains, int ndi
                        const void* grad_out, void* const* grad_cores, void* workspace, size_t workspace_bytes,
                        void* stream);
 
+/* round_tt(a * b) for two tensor trains a, b of one shape: the rounded elementwise product, without forming its
+ * Kronecker cores C_k[:, i, :] = A_k[:, i, :] (x) B_k[:, i, :] of bond rank R_k = ranks_a[k] * ranks_b[k].
+ * cores_a[k] is row-major [ranks_a[k]][shape[k]][ranks_a[k + 1]], likewise b; boundary ranks 1; dtype TNB_F32 or TNB_F64
+ * for both (the arithmetic is fp64 in both: fp32 cores are widened exactly; the output cores take the input dtype).
+ * rmax: ndim - 1 caps (<= 0: none) or null; eps: the relative error budget of tnb_tt_round (delta = eps / sqrt(N - 1)
+ * ||C||).  The output layout is that of tnb_tt_round: core k at core_offsets[k] of cores_out, row-major
+ * [ranks_host[k]][shape[k]][ranks_host[k + 1]]; core 0 carries the norm, cores 1 .. N-1 have orthonormal rows.  The slots
+ * are sized for the truncated ranks (tnb_tt_hadamard_round_cores_capacity), never for R_k.  energies_host (or null)
+ * receives ||C||^2 and the discarded energy ||C - result||^2 (the sum of the discarded eigenvalues of every bond), so
+ * sqrt(energies[1] / energies[0]) is the rounding's relative error.
+ * The method is a Gram form of tnb_tt_round's two sweeps: the left Grams GL_k = C_{<k}^T C_{<k} (R_k x R_k, all kept) by
+ * GL_{k+1} = sum_i C_i^T GL_k C_i, four one-index contractions per mode value on the fp64 tensor cores (mma.sync m16n8k16
+ * .f64) when the mode's four ranks are in [16, 256], on fp64 CUDA-core tiles otherwise or under TNB_FLAG_NO_TENSORCORE;
+ * then from the right, at each bond, Y = C_mu W_{mu+1}, H = Y^T GL_mu Y (the Gram of the carry tnb_tt_round truncates),
+ * the eigen stage and rank rule of tnb_tt_round (Jacobi up to 256, the subspace solver above), core mu = V_r^T and
+ * W_mu = Y V_r.  The rounding is Gram-class: where the rank rule decides at the Gram's noise floor the rank may lie
+ * between the numerical rank and the cap.  Its envelope is the eigen stage's: a Gram size I_mu r_{mu+1} up to 46000 and a
+ * kept rank of at most 240 where that Gram is wider than 256; outside it the call returns TNB_ERR_UNSUPPORTED, so an
+ * eps-only call at large ranks (128^10 at rank 64 squared) needs rmax.
+ * Null pointers, ndim outside [1, 62], a mode size or rank below 1 or boundary ranks other than 1 are TNB_ERR_INVALID; a
+ * rank above 4096 or R_k above 65536 TNB_ERR_UNSUPPORTED; a short cores buffer or workspace TNB_ERR_WORKSPACE; all
+ * before anything is launched.  Stream-ordered; one host synchronisation per bond (an eps-only subspace solve may take
+ * a few) and one at the end; no allocation beyond the workspace and the library's pinned scratch; bitwise reproducible
+ * (fixed-order sums, no atomics, chunks that depend on the shapes only).  The workspace holds every GL_k (sum R_k^2
+ * doubles), then either the recurrence's two chunk buffers (at most 2^26 doubles together unless one mode value needs
+ * more) or one bond's W, Y, GL Y, H and eigen scratch.
+ * Replaces: tntorch's round_tt(t1 * t2) (tensor.py:560-640 then 2008-2083), which forms the Kronecker cores. */
+int64_t tnb_tt_hadamard_round_cores_capacity(int ndim, const int64_t* shape, const int32_t* ranks_a,
+                                             const int32_t* ranks_b, const int32_t* rmax, int64_t* core_offsets_host);
+size_t tnb_tt_hadamard_round_workspace_bytes(int dtype, int ndim, const int64_t* shape, const int32_t* ranks_a,
+                                             const int32_t* ranks_b, const int32_t* rmax);
+int tnb_tt_hadamard_round(int dtype, const void* const* cores_a, const void* const* cores_b, int ndim,
+                          const int64_t* shape, const int32_t* ranks_a, const int32_t* ranks_b, const int32_t* rmax,
+                          double eps, uint32_t flags, void* workspace, size_t workspace_bytes, void* cores_out,
+                          int64_t cores_capacity, int32_t* ranks_host, double* energies_host, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

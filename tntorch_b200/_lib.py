@@ -66,7 +66,11 @@ SIGNATURES = {
     "tnb_tt_sum_round": (C.c_int, [C.c_int, C.POINTER(_vp), C.c_int, _f64p, C.c_int, _i64p, _i32p, _i32p, C.c_double,
                                    C.c_uint32, _vp, C.c_size_t, _vp, C.c_int64, _i32p, _vp]),
     "tnb_tt_hadamard": (C.c_int, [C.c_int, C.POINTER(_vp), C.POINTER(_vp), C.c_int, _i64p, _i32p, _i32p, C.POINTER(_vp), _vp]),
-    "tnb_truncated_svd_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int64, C.c_int64]),
+    "tnb_tt_hadamard_round_cores_capacity": (C.c_int64, [C.c_int, _i64p, _i32p, _i32p, _i32p, _i64p]),
+    "tnb_tt_hadamard_round_workspace_bytes": (C.c_size_t, [C.c_int, C.c_int, _i64p, _i32p, _i32p, _i32p]),
+    "tnb_tt_hadamard_round": (C.c_int, [C.c_int, C.POINTER(_vp), C.POINTER(_vp), C.c_int, _i64p, _i32p, _i32p, _i32p,
+                                        C.c_double, C.c_uint32, _vp, C.c_size_t, _vp, C.c_int64, _i32p, _f64p, _vp]),
+    "tnb_truncated_svd_workspace_bytes":(C.c_size_t, [C.c_int, C.c_int64, C.c_int64]),
     "tnb_truncated_svd": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_int64, C.c_double, C.c_double, C.c_int32, C.c_int,
                                     _vp, C.c_size_t, _vp, _vp, _i32p, _vp]),
     "tnb_cp_als_factors_capacity": (C.c_int64, [C.c_int, _i64p, C.c_int32, _i64p]),

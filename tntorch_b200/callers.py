@@ -116,7 +116,8 @@ def hadamard_sum(ts: Sequence[Tensor], algorithm: str = "exact", eps: float = No
 
     'exact' contracts the K trains directly (cost grows with the product of the ranks).  'svd' / 'eig' keep a running
     product P <- round_tt(P * t_k, eps/sqrt(K-1)): Kronecker cores (tnb_tt_hadamard) followed by the rounding sweeps
-    (tnb_tt_round), so the interface never exceeds the rounded rank times r_k; the result is within eps * ||prod|| *
+    (tnb_tt_round), or one fused tnb_tt_hadamard_round call where those cannot run (a product rank above 256, or not
+    enough device memory), so the interface never exceeds the rounded rank times r_k; the result is within eps * ||prod|| *
     sqrt(numel) of the exact sum (the reference re-rounds the same intermediate quantities mode by mode)."""
     assert algorithm in ("svd", "eig", "exact")
     assert all(list(ts[0].shape) == list(t.shape) for t in ts[1:])
@@ -128,8 +129,21 @@ def hadamard_sum(ts: Sequence[Tensor], algorithm: str = "exact", eps: float = No
     step_eps = (1e-14 if eps is None else eps) / math.sqrt(len(ts) - 1)
     P = cs[0]
     for k in range(1, len(cs)):
-        P = ops.tt_round(ops.tt_hadamard(P, cs[k]), eps=step_eps)
+        P = _round_product(P, cs[k], step_eps)
     return float(_sum_all(P))
+
+
+def _round_product(a, b, eps):
+    """round_tt(a * b, eps) of two lists of TT cores: Kronecker cores and tt_round where they can run, else one fused
+    tt_hadamard_round call (ops.hadamard_round_instead_of_kronecker)."""
+    if a[0].dtype == b[0].dtype:
+        shape = [c.shape[1] for c in a]
+        ra = [a[0].shape[0]] + [c.shape[2] for c in a]
+        rb = [b[0].shape[0]] + [c.shape[2] for c in b]
+        free, _ = torch.cuda.mem_get_info(a[0].device)
+        if ops.hadamard_round_instead_of_kronecker(shape, ra, rb, a[0].element_size(), int(free)):
+            return ops.tt_hadamard_round(a, b, eps=eps)
+    return ops.tt_round(ops.tt_hadamard(a, b), eps=eps)
 
 
 def shift_mode(t: Tensor, n: int, shift: int, eps: Union[float, str] = 1e-3):

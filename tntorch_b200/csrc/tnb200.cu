@@ -18,6 +18,7 @@
 #include "tt_dot.cuh"
 #include "tt_gather.cuh"
 #include "tt_gather_grad.cuh"
+#include "tt_hadamard_round.cuh"
 
 using namespace tnb;
 
@@ -1070,6 +1071,59 @@ int tnb_tt_dot(int dtype, const void* const* cores_a, const void* const* cores_b
   return tt_dot_impl<float>(ar, false, reinterpret_cast<const float* const*>(cores_a),
                             reinterpret_cast<const float* const*>(cores_b), npairs, ndim, shape, ranks_a, ranks_b, out,
                             as_stream(stream));
+}
+
+// ------------------------------------------------------------------ rounded elementwise product of two tensor trains
+int64_t tnb_tt_hadamard_round_cores_capacity(int ndim, const int64_t* shape, const int32_t* ranks_a,
+                                             const int32_t* ranks_b, const int32_t* rmax, int64_t* core_offsets_host) {
+  HrDims d;
+  if (make_hr_dims(ndim, shape, ranks_a, ranks_b, rmax, d) != TNB_OK) return -1;
+  if (core_offsets_host)
+    for (int k = 0; k < ndim; ++k) core_offsets_host[k] = d.slot[k];
+  return d.capacity;
+}
+
+size_t tnb_tt_hadamard_round_workspace_bytes(int dtype, int ndim, const int64_t* shape, const int32_t* ranks_a,
+                                             const int32_t* ranks_b, const int32_t* rmax) {
+  HrDims d;
+  if ((dtype != TNB_F32 && dtype != TNB_F64) || make_hr_dims(ndim, shape, ranks_a, ranks_b, rmax, d) != TNB_OK) return 0;
+  ArenaSizer ar;
+  const int rc = dtype == TNB_F32
+                     ? tt_hadamard_round_impl<float>(ar, true, nullptr, nullptr, d, rmax, 0.0, 0, nullptr, nullptr, nullptr, 0)
+                     : tt_hadamard_round_impl<double>(ar, true, nullptr, nullptr, d, rmax, 0.0, 0, nullptr, nullptr, nullptr, 0);
+  if (rc != TNB_OK) return 0;
+  return with_slack(ar.off);
+}
+
+int tnb_tt_hadamard_round(int dtype, const void* const* cores_a, const void* const* cores_b, int ndim,
+                          const int64_t* shape, const int32_t* ranks_a, const int32_t* ranks_b, const int32_t* rmax,
+                          double eps, uint32_t flags, void* workspace, size_t workspace_bytes, void* cores_out,
+                          int64_t cores_capacity, int32_t* ranks_host, double* energies_host, void* stream) {
+  if (dtype != TNB_F32 && dtype != TNB_F64)
+    return fail(TNB_ERR_UNSUPPORTED, "tnb_tt_hadamard_round: dtype %d is not built (TNB_F32, TNB_F64)", dtype);
+  if (!cores_a || !cores_b || !shape || !ranks_a || !ranks_b || !cores_out || !ranks_host || !workspace)
+    return fail(TNB_ERR_INVALID, "tnb_tt_hadamard_round: null argument");
+  HrDims d;
+  TNB_TRY(make_hr_dims(ndim, shape, ranks_a, ranks_b, rmax, d));
+  for (int k = 0; k < ndim; ++k)
+    if (!cores_a[k] || !cores_b[k]) return fail(TNB_ERR_INVALID, "tnb_tt_hadamard_round: core %d is null", k);
+  if (cores_capacity < d.capacity)
+    return fail(TNB_ERR_WORKSPACE, "tnb_tt_hadamard_round: cores buffer holds %lld elements, need %lld",
+                (long long)cores_capacity, (long long)d.capacity);
+  const size_t need = tnb_tt_hadamard_round_workspace_bytes(dtype, ndim, shape, ranks_a, ranks_b, rmax);
+  if (need == 0) return TNB_ERR_UNSUPPORTED;  // the sizing pass's refusal is the last error
+  if (workspace_bytes < need)
+    return fail(TNB_ERR_WORKSPACE, "tnb_tt_hadamard_round: workspace too small (need %zu bytes, got %zu)", need,
+                workspace_bytes);
+  TNB_TRY(require_device());
+  Arena ar(workspace, workspace_bytes);
+  if (dtype == TNB_F32)
+    return tt_hadamard_round_impl<float>(ar, false, reinterpret_cast<const float* const*>(cores_a),
+                                         reinterpret_cast<const float* const*>(cores_b), d, rmax, eps, flags,
+                                         static_cast<float*>(cores_out), ranks_host, energies_host, as_stream(stream));
+  return tt_hadamard_round_impl<double>(ar, false, reinterpret_cast<const double* const*>(cores_a),
+                                        reinterpret_cast<const double* const*>(cores_b), d, rmax, eps, flags,
+                                        static_cast<double*>(cores_out), ranks_host, energies_host, as_stream(stream));
 }
 
 // ------------------------------------------------------------------ entries of tensor trains at many multi-indices

@@ -549,6 +549,69 @@ def tt_hadamard(a_cores, b_cores):
     return outs
 
 
+def tt_hadamard_round(a_cores, b_cores, eps: float = 1e-14, rmax=None, return_info: bool = False,
+                      use_tensorcore: bool = True):
+    """round_tt(a * b) of two tensor trains in ONE library call (tnb_tt_hadamard_round) that never forms the Kronecker
+    cores of the product: left Grams of the product by a structured recurrence, then the truncation sweep of tt_round on
+    the Gram of each bond's carry.  Ranks and tolerance follow tt_round (delta = eps / sqrt(N - 1) ||a * b||, rmax a
+    scalar or N - 1 caps).  fp32 or fp64 cores of one dtype (ValueError otherwise), computed in fp64, returned in the
+    input dtype.  return_info adds dict(norm_sq=||a*b||^2, discarded_sq=||a*b - result||^2).  Envelope: a bond Gram of
+    I_mu r_{mu+1} up to 46000 and, where it is wider than 256, a kept rank up to 240 (NotImplementedError otherwise):
+    eps-only calls at large ranks need rmax.  use_tensorcore=False runs every GEMM on CUDA-core tiles."""
+    ops_c, K, N, shape, ranks, ptrs, dt, dev = _tt_operands([a_cores, b_cores])
+    ra, rb = ranks[: N + 1], ranks[N + 1:]
+    if ra[0] != 1 or ra[N] != 1 or rb[0] != 1 or rb[N] != 1:
+        raise ValueError("tt_hadamard_round: boundary ranks must be 1")
+    if any(c.requires_grad for cores in ops_c for c in cores):
+        raise ValueError("tt_hadamard_round: cores that require grad are not supported")
+    code = _dtype_code(ops_c[0][0])
+    rm = _rmax_list(rmax, max(N - 1, 0))
+    L = lib()
+    sh, rac, rbc = i64(shape), i32(ra), i32(rb)
+    rmc = i32(rm) if N > 1 else i32([0])
+    offs = (C.c_int64 * N)()
+    cap = L.tnb_tt_hadamard_round_cores_capacity(N, sh, rac, rbc, rmc, offs)
+    if cap < 0:
+        check(_lib.ERR_INVALID)
+    wsb = L.tnb_tt_hadamard_round_workspace_bytes(code, N, sh, rac, rbc, rmc)
+    if wsb == 0:
+        check(_lib.ERR_UNSUPPORTED)
+    ws = _ws(wsb, dev)
+    out = torch.empty(int(cap), dtype=dt, device=dev)
+    rk = (C.c_int32 * (N + 1))()
+    en = (C.c_double * 2)()
+    pa = (C.c_void_p * N)(*[c.data_ptr() for c in ops_c[0]])
+    pb = (C.c_void_p * N)(*[c.data_ptr() for c in ops_c[1]])
+    flags = 0 if use_tensorcore else _lib.FLAG_NO_TENSORCORE
+    with torch.cuda.device(dev):
+        check(L.tnb_tt_hadamard_round(code, pa, pb, N, sh, rac, rbc, rmc, float(eps), flags, _ptr(ws), ws.numel(), _ptr(out),
+                                      cap, rk, en, _stream()))
+    res = [out[offs[n]: offs[n] + rk[n] * shape[n] * rk[n + 1]].view(rk[n], shape[n], rk[n + 1]) for n in range(N)]
+    if return_info:
+        return res, dict(norm_sq=float(en[0]), discarded_sq=float(en[1]))
+    return res
+
+
+def hadamard_round_instead_of_kronecker(shape: Sequence[int], ranks_a: Sequence[int], ranks_b: Sequence[int],
+                                        itemsize: int, free_bytes: int) -> bool:
+    """The rule `round_tt(a * b)` inside `tn.reduce(..., operator.mul)` and `tn.hadamard_sum(..., 'svd' | 'eig')` is
+    computed by: the fused `tt_hadamard_round` when the Kronecker path cannot run, i.e. some product rank
+    ra_k rb_k is above 256 (tt_round's direct eigensolver limit), or the Kronecker cores plus tt_round's workspace
+    exceed free device memory; the Kronecker cores (`tt_hadamard`) and `tt_round` otherwise."""
+    N = len(shape)
+    R = [int(a) * int(b) for a, b in zip(ranks_a, ranks_b)]
+    if any(r > 256 for r in R):
+        return True
+    kron = sum(R[k] * int(shape[k]) * R[k + 1] for k in range(N)) * int(itemsize)
+    code = _lib.TNB_F32 if int(itemsize) == 4 else _lib.TNB_F64
+    rm = i32([0] * max(N - 1, 1))
+    wsb = lib().tnb_tt_round_workspace_bytes(code, N, i64(shape), i32(R), rm)
+    if wsb == 0:
+        return True
+    cap = lib().tnb_tt_round_cores_capacity(N, i64(shape), i32(R), rm, None)
+    return kron + int(wsb) + max(int(cap), 0) * int(itemsize) > int(free_bytes)
+
+
 def truncated_svd(M: torch.Tensor, delta=None, eps=None, rmax=None, left_ortho=True, batch_mode: bool = False,
                   return_zero_flag: bool = False):
     """tn.truncated_svd (round.py:52-187) of one matrix.  batch_mode = the reference's rank rule for one sample of a

@@ -60,18 +60,25 @@ def truncated_svd(
 def reduce(ts, function, eps=0, rmax=None, algorithm="svd", verbose=False, **kwargs):
     """tools.py:460-512: a function of all tensors of a sequence, climbing a binary tree and rounding every intermediate.
     For `operator.add` (and `operator.sub`'s accumulate form) the node `tn.round(a + b)` is ONE library call
-    (tnb_tt_sum_round: block cores assembled in the workspace, then the rounding sweeps); any other function is applied
-    as given and rounded with `round`."""
+    (tnb_tt_sum_round: block cores assembled in the workspace, then the rounding sweeps).  For `operator.mul` the node
+    `tn.round(a * b)` is one tnb_tt_hadamard_round call when the Kronecker cores cannot be rounded (a product rank above
+    256, or not enough device memory: ops.hadamard_round_instead_of_kronecker), and runs as before otherwise.  Any other
+    function is applied as given and rounded with `round`."""
     import operator
 
     from .tensor import Tensor
 
     assert algorithm in ("svd", "eig")
     fused = function is operator.add and not kwargs
+    product = function is operator.mul and not kwargs
 
     def node(a, b):
         if fused and not a.batch and not b.batch:
             return Tensor(ops.tt_sum_round([a._tt_cores(), b._tt_cores()], eps=eps, rmax=rmax))
+        if product and isinstance(a, Tensor) and isinstance(b, Tensor) and not a.batch and not b.batch:
+            out = _hadamard_round_node(a, b, eps, rmax, algorithm)
+            if out is not None:
+                return out
         out = function(a, b, **kwargs)
         out.round(eps=eps, rmax=rmax, algorithm=algorithm)
         return out
@@ -89,6 +96,31 @@ def reduce(ts, function, eps=0, rmax=None, algorithm="svd", verbose=False, **kwa
     for key in keys[1:]:
         result = node(result, d[key])
     return result
+
+
+def _hadamard_round_node(a, b, eps, rmax, algorithm):
+    """`round(a * b, eps, rmax)` as reduce's `operator.mul` node takes it when the Kronecker path cannot run
+    (ops.hadamard_round_instead_of_kronecker): one fused tt_hadamard_round call, then Tensor.round's Tucker step with the
+    left-over budget, the error reached taken from the returned energies.  None: the Kronecker path runs as before."""
+    from .tensor import Tensor
+
+    c0 = a.cores[0]
+    if c0.dtype != b.cores[0].dtype or list(a.shape) != list(b.shape):
+        return None
+    # the TT ranks _tt_cores() would give (a CP tensor's boundary ranks are 1), read without converting anything
+    ra, rb = [int(r) for r in a.ranks_tt], [int(r) for r in b.ranks_tt]
+    ra[0] = ra[-1] = rb[0] = rb[-1] = 1
+    free, _ = torch.cuda.mem_get_info(c0.device)
+    if not ops.hadamard_round_instead_of_kronecker(list(a.shape), ra, rb, c0.element_size(), int(free)):
+        return None
+    ca, cb = a._tt_cores(), b._tt_cores()
+    cores, info = ops.tt_hadamard_round(ca, cb, eps=eps, rmax=rmax, return_info=True)
+    out = Tensor(cores)
+    nn = info["norm_sq"]
+    reached = math.sqrt(info["discarded_sq"] / nn) if nn > 0 else 0.0
+    if reached < eps:
+        out.round_tucker((1 + eps) / (1 + reached) - 1, rmax=rmax, algorithm=algorithm)
+    return out
 
 
 def relative_error(gt, approx):
