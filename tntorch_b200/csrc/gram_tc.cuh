@@ -1007,47 +1007,71 @@ gram_tc_kernel(const __grid_constant__ CUtensorMap tmap, const __grid_constant__
   }
 }
 
-// Sum the split-K partial tiles in fp64 (fixed order), mirror to the lower triangle.
-__global__ void gram_tc_finalize_kernel(const GramTcParams p, double* __restrict__ G, float* __restrict__ Gf) {
-  if (p.fold > 1) {  // single 128 x 128 tile; fold the diagonal n_orig x n_orig blocks
-    // one WARP per output element: the ksplit * fold terms (hundreds, strided) are dealt to the lanes and combined by a
-    // shuffle tree in a fixed order — deterministic like the serial sum, without its 300-deep dependent chain per thread
-    const int no = p.n_orig;
-    const size_t split_stride = (size_t)p.num_tiles * 128 * p.tn;
-    const int lane = threadIdx.x & 31;
-    const int warps = (gridDim.x * blockDim.x) >> 5;
-    const int nterms = p.ksplit * p.fold;
-    for (int idx = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; idx < no * no; idx += warps) {
-      const int i = idx / no, j = idx % no;
-      double s = 0.0;
-      for (int t = lane; t < nterms; t += 32) {
-        const int z = t / p.fold, a = t - z * p.fold;
-        s += (double)p.partial[(size_t)z * split_stride + (size_t)(a * no + i) * p.tn + (a * no + j)];
-      }
-      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      if (lane == 0) {
-        G[idx] = s;
-        if (Gf) Gf[idx] = (float)s;
-      }
-    }
-    return;
-  }
-  const int64_t total = (int64_t)p.n * p.n;
-  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
-       idx += (int64_t)gridDim.x * blockDim.x) {
-    const int i = (int)(idx / p.n), j = (int)(idx % p.n);
-    const int ii = i <= j ? i : j, jj = i <= j ? j : i;
-    const int bm = ii / 128, bn = jj / p.tn;
-    // flat index of (bm, bn) among kept tiles: row a keeps the column tiles b >= first(a) = floor(a*128 / tn)
-    int tile = 0;
-    for (int a = 0; a < bm; ++a) tile += p.num_bn - (a * 128) / p.tn;
-    tile += bn - (bm * 128) / p.tn;
-    const size_t off = ((size_t)tile * 128 + (ii - bm * 128)) * (size_t)p.tn + (jj - bn * p.tn);
-    const size_t split_stride = (size_t)p.num_tiles * 128 * p.tn;
+// Folded form (p.fold > 1): a single 128 x 128 tile; sum the split-K partials of the diagonal n_orig x n_orig blocks in
+// fp64.  One WARP per output element: the ksplit * fold terms (hundreds, strided) are dealt to the lanes and combined by
+// a shuffle tree in a fixed order — deterministic like the serial sum, without its 300-deep dependent chain per thread.
+__global__ void gram_tc_fold_finalize_kernel(const GramTcParams p, double* __restrict__ G, float* __restrict__ Gf) {
+  const int no = p.n_orig;
+  const size_t split_stride = (size_t)p.num_tiles * 128 * p.tn;
+  const int lane = threadIdx.x & 31;
+  const int warps = (gridDim.x * blockDim.x) >> 5;
+  const int nterms = p.ksplit * p.fold;
+  for (int idx = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; idx < no * no; idx += warps) {
+    const int i = idx / no, j = idx % no;
     double s = 0.0;
-    for (int z = 0; z < p.ksplit; ++z) s += (double)p.partial[(size_t)z * split_stride + off];
-    G[idx] = s;
-    if (Gf) Gf[idx] = (float)s;
+    for (int t = lane; t < nterms; t += 32) {
+      const int z = t / p.fold, a = t - z * p.fold;
+      s += (double)p.partial[(size_t)z * split_stride + (size_t)(a * no + i) * p.tn + (a * no + j)];
+    }
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) {
+      G[idx] = s;
+      if (Gf) Gf[idx] = (float)s;
+    }
+  }
+}
+
+// Sum the split-K partial tiles in fp64 (fixed order z = 0 .. ksplit - 1), mirror to the lower triangle.  One CTA of
+// 32 x 8 threads per 32 x 32 block (bi, bj), bi <= bj, of the upper triangle (grid: bj = blockIdx.x, bi = blockIdx.y):
+// it reads the partials along their rows and writes the block, then its transpose through shared memory to the mirror
+// block (bj, bi), so every read and write is along a row.  Reading the lower triangle's sums straight from the partial
+// tiles (one thread per element of G) would walk down their columns, 4 useful bytes per 32-byte sector, and this kernel
+// runs inside the chain of whole-GPU kernels of a batch (BigKernelGate), where the next tensor's Gram waits for it.
+constexpr int GF_BLOCK = 32;
+__global__ void __launch_bounds__(256) gram_tc_finalize_kernel(const GramTcParams p, double* __restrict__ G,
+                                                               float* __restrict__ Gf) {
+  const int bi = blockIdx.y, bj = blockIdx.x;
+  if (bi > bj) return;
+  __shared__ double blk[GF_BLOCK][GF_BLOCK + 1];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  const int n = p.n, i0 = bi * GF_BLOCK, j0 = bj * GF_BLOCK;
+  // the kept 128 x tn partial tile (bm, bn) holding this block (32 divides 128 and tn); its flat index among the kept
+  // tiles: row a keeps the column tiles b >= first(a) = floor(a*128 / tn)
+  const int bm = i0 / 128, bn = j0 / p.tn;
+  int tile = 0;
+  for (int a = 0; a < bm; ++a) tile += p.num_bn - (a * 128) / p.tn;
+  tile += bn - (bm * 128) / p.tn;
+  const size_t split_stride = (size_t)p.num_tiles * 128 * p.tn;
+  const float* src = p.partial + ((size_t)tile * 128 + (i0 - bm * 128)) * (size_t)p.tn + (j0 - bn * p.tn) + tx;
+  for (int r = ty; r < GF_BLOCK; r += 8) {
+    const int i = i0 + r, j = j0 + tx;
+    if (i < n && j < n && i <= j) {
+      const float* s0 = src + (size_t)r * p.tn;
+      double s = 0.0;
+      for (int z = 0; z < p.ksplit; ++z) s += (double)s0[(size_t)z * split_stride];
+      G[(size_t)i * n + j] = s;
+      if (Gf) Gf[(size_t)i * n + j] = (float)s;
+      blk[r][tx] = s;
+    }
+  }
+  __syncthreads();
+  for (int r = ty; r < GF_BLOCK; r += 8) {
+    const int i = j0 + r, j = i0 + tx;  // (i, j) of the lower triangle mirrors (j, i) = blk[tx][r]
+    if (i < n && j < i) {
+      const double s = blk[tx][r];
+      G[(size_t)i * n + j] = s;
+      if (Gf) Gf[(size_t)i * n + j] = (float)s;
+    }
   }
 }
 
@@ -1306,8 +1330,13 @@ inline int gram_tc(const T* A, int64_t rows, int64_t n, double* G, float* Gf, vo
     gram_tc_kernel<TC_ROWMAJOR><<<grid, TC_THREADS, TC_SMEM_BYTES, st>>>(tmap, tmap, p);
   }
   TNB_LAUNCH_CHECK();
-  const int64_t total = n_in * n_in * (p.fold > 1 ? 32 : 1);  // folded form: one warp per element
-  gram_tc_finalize_kernel<<<(unsigned)std::min<int64_t>((total + 255) / 256, 4096), 256, 0, st>>>(p, G, Gf);
+  if (p.fold > 1) {
+    const int64_t total = n_in * n_in * 32;  // one warp per element
+    gram_tc_fold_finalize_kernel<<<(unsigned)std::min<int64_t>((total + 255) / 256, 4096), 256, 0, st>>>(p, G, Gf);
+  } else {
+    const unsigned nb = (unsigned)ceil_div<int64_t>(n, GF_BLOCK);
+    gram_tc_finalize_kernel<<<dim3(nb, nb), 256, 0, st>>>(p, G, Gf);
+  }
   TNB_LAUNCH_CHECK();
   return TNB_OK;
 }
