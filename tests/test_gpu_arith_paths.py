@@ -527,6 +527,31 @@ def test_tt_sum_refuses_17_operands():
         ops.tt_sum(ops_d)
 
 
+# The library takes a train's ranks as one list r_0..r_N and reads core k as r_k x I_k x r_{k+1}.  A train whose core 0
+# ends in rank 3 while core 1 starts with rank 2 has no such list: it is refused before anything launches.
+UNCHAINED = {
+    "tt_sum": lambda ops, a, bad: ops.tt_sum([a, bad]),
+    "tt_sum_round": lambda ops, a, bad: ops.tt_sum_round([a, bad], rmax=2),
+    "tt_hadamard": lambda ops, a, bad: ops.tt_hadamard(a, bad),
+    "tt_hadamard_round": lambda ops, a, bad: ops.tt_hadamard_round(a, bad, rmax=2),
+    "tt_round_batch": lambda ops, a, bad: ops.tt_round_batch([bad, bad], rmax=2),
+}
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", list(UNCHAINED))
+def test_unchained_core_ranks_are_refused_before_any_launch(name):
+    from tntorch_b200 import ops
+
+    a = _rand_tt((4, 5, 6), [2, 3], 1, F64)
+    bad = [torch.randn(1, 4, 3, dtype=F64, device="cuda"), torch.randn(2, 5, 3, dtype=F64, device="cuda"),
+           torch.randn(3, 6, 1, dtype=F64, device="cuda")]
+    before = ops.launch_count()
+    with pytest.raises(ValueError, match="ranks"):
+        UNCHAINED[name](ops, a, bad)
+    assert ops.launch_count() == before
+
+
 HAD_CASES = {
     "N1": ((13,), [], []),
     "N2_1xr_rx1": ((6, 9), [1], [4]),

@@ -54,6 +54,14 @@ def _ws(nbytes: int, device) -> torch.Tensor:
     return torch.empty(max(int(nbytes), 256), dtype=torch.uint8, device=device)
 
 
+def _workspace(nbytes: int, device) -> torch.Tensor:
+    """The workspace of a size a *_workspace_bytes query returned.  A size of 0 is the library refusing the call
+    (NotImplementedError)."""
+    if nbytes == 0:
+        check(_lib.ERR_UNSUPPORTED)
+    return _ws(nbytes, device)
+
+
 def _ptr(t: Optional[torch.Tensor]) -> C.c_void_p:
     return C.c_void_p(0 if t is None else t.data_ptr())
 
@@ -72,6 +80,52 @@ def _rmax_list(rmax, nbonds: int) -> List[int]:
             assert r >= 1
             out.append(min(r, 2**31 - 1))
     return out
+
+
+def _tt_ranks(cores, what: str, boundary: bool = False, one_dtype: bool = True) -> List[int]:
+    """The rank list [r_0, ..., r_N] of TT cores [r_k, I_k, r_{k+1}], the form the C-ABI takes them in.  The library
+    reads core k as r_k x I_k x r_{k+1} from that list, so the cores must be CUDA tensors (RuntimeError), 3-D, on one
+    device and, unless one_dtype=False, of one dtype, and their ranks must chain (ValueError).  With boundary=True,
+    r_0 and r_N must be 1."""
+    for c in cores:
+        _require_cuda(c, what)
+    if not cores or any(c.dim() != 3 for c in cores):
+        raise ValueError(f"{what}: cores must be 3-D tensors [r, I, r']")
+    c0 = cores[0]
+    if any(c.device != c0.device for c in cores):
+        raise ValueError(f"{what}: cores must share one CUDA device")
+    if one_dtype and any(c.dtype != c0.dtype for c in cores):
+        raise ValueError(f"{what}: cores must share one dtype")
+    if any(cores[k].shape[2] != cores[k + 1].shape[0] for k in range(len(cores) - 1)):
+        raise ValueError(f"{what}: core ranks do not match")
+    ranks = [c0.shape[0]] + [c.shape[2] for c in cores]
+    if boundary and (ranks[0] != 1 or ranks[-1] != 1):
+        raise ValueError(f"{what}: boundary ranks must be 1, got {ranks[0]} and {ranks[-1]}")
+    return ranks
+
+
+def _slot_views(buf: torch.Tensor, offs, ranks, shape, base: int = 0) -> List[torch.Tensor]:
+    """The cores a library call wrote into its slotted output `buf`: core k starts at offs[k] and is
+    [ranks[base + k], shape[k], ranks[base + k + 1]] (base = i * (N + 1) for tensor i of a batch's rank list)."""
+    out = []
+    for k, n in enumerate(shape):
+        r0, r1 = ranks[base + k], ranks[base + k + 1]
+        out.append(buf[offs[k]: offs[k] + r0 * n * r1].view(r0, n, r1))
+    return out
+
+
+def _ttsvd_layout(shape: Sequence[int], rmax):
+    """The dense TT-SVD's arguments and output layout for `shape` and `rmax`: the i64 shape, the i32 rank caps (a single
+    0 for one mode), each core's offset in the cores buffer and that buffer's capacity in elements.  A shape the
+    library cannot lay out raises ValueError."""
+    N = len(shape)
+    rm = _rmax_list(rmax, max(N - 1, 0))
+    sh, rmc = i64(shape), i32(rm if N > 1 else [0])
+    offs = (C.c_int64 * max(N, 1))()
+    cap = lib().tnb_ttsvd_cores_capacity(N, sh, rmc, offs)
+    if cap < 0:
+        check(_lib.ERR_INVALID)
+    return sh, rmc, offs, cap
 
 
 def launch_count() -> int:
@@ -114,35 +168,11 @@ def ttsvd(data: torch.Tensor, rmax=None, eps: float = 1e-14, batch_mode: bool = 
     """Dense tensor -> list of TT cores [r_{k-1}, I_k, r_k] (tn.Tensor(data, ranks_tt=...), tensor.py:401-408)."""
     _require_cuda(data, "ttsvd")
     data = data.contiguous()
-    code = _dense_code(data.dtype)
-    N = data.dim()
-    shape = list(data.shape)
-    rm = _rmax_list(rmax, max(N - 1, 0))
-    flags = ((0 if use_tensorcore else _lib.FLAG_NO_TENSORCORE) | (_lib.FLAG_BATCH_MODE if batch_mode else 0) |
-             (_lib.FLAG_CONCURRENT if concurrent else 0) | (0 if speculate else _lib.FLAG_NO_SPECULATE))
-    L = lib()
-    sh = i64(shape)
-    rmc = i32(rm) if N > 1 else i32([0])
-    offs = (C.c_int64 * N)()
-    cap = L.tnb_ttsvd_cores_capacity(N, sh, rmc, offs)
-    if cap < 0:
-        check(_lib.ERR_INVALID)
-    wsb = L.tnb_ttsvd_workspace_bytes(code, N, sh, rmc, flags)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED if L.tnb_last_error() else _lib.ERR_INVALID)
-    ws = _ws(wsb, data.device)
-    cores_buf = torch.empty(int(cap), dtype=_core_dtype(data.dtype), device=data.device)
-    ranks = (C.c_int32 * (N + 1))()
-    info = (C.c_double * 32)()
-    with torch.cuda.device(data.device):
-        check(L.tnb_ttsvd(code, _ptr(data), N, sh, rmc, float(eps), flags, _ptr(ws), ws.numel(), _ptr(cores_buf), cap,
-                          ranks, info, _stream()))
-    cores = []
-    for k in range(N):
-        r0, r1 = ranks[k], ranks[k + 1]
-        cores.append(cores_buf[offs[k]: offs[k] + r0 * shape[k] * r1].view(r0, shape[k], r1))
+    plan = TTSVDPlan(data.shape, data.dtype, rmax=rmax, device=data.device, use_tensorcore=use_tensorcore,
+                     concurrent=concurrent, speculate=speculate, batch_mode=batch_mode)
+    cores = plan.run(data, eps)
     if return_info:
-        return cores, _ttsvd_info(info)
+        return cores, _ttsvd_info(plan.info)
     return cores
 
 
@@ -167,27 +197,17 @@ def ttsvd_stream(X_cpu: torch.Tensor, rmax=None, eps: float = 1e-14, chunk_bytes
     dev = torch.device("cuda", torch.cuda.current_device())
     N = X.dim()
     shape = list(X.shape)
-    rm = _rmax_list(rmax, max(N - 1, 0))
+    sh, rmc, offs, cap = _ttsvd_layout(shape, rmax)
     L = lib()
-    sh = i64(shape)
-    rmc = i32(rm) if N > 1 else i32([0])
-    offs = (C.c_int64 * max(N, 1))()
-    cap = L.tnb_ttsvd_cores_capacity(N, sh, rmc, offs)
-    if cap < 0:
-        check(_lib.ERR_INVALID)
     cb = 0 if chunk_bytes is None else int(chunk_bytes)
-    wsb = L.tnb_ttsvd_stream_workspace_bytes(code, N, sh, rmc, cb, 0)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, dev)
+    ws = _workspace(L.tnb_ttsvd_stream_workspace_bytes(code, N, sh, rmc, cb, 0), dev)
     cores_buf = torch.empty(int(cap), dtype=_core_dtype(X.dtype), device=dev)
     ranks = (C.c_int32 * (N + 1))()
     info = (C.c_double * 32)()
     with torch.cuda.device(dev):
         check(L.tnb_ttsvd_stream(code, _ptr(X), N, sh, rmc, float(eps), 0, cb, _ptr(ws), ws.numel(), _ptr(cores_buf), cap,
                                  ranks, info, _stream()))
-    cores = [cores_buf[offs[k]: offs[k] + ranks[k] * shape[k] * ranks[k + 1]].view(ranks[k], shape[k], ranks[k + 1])
-             for k in range(N)]
+    cores = _slot_views(cores_buf, offs, ranks, shape)
     if return_info:
         return cores, dict(_ttsvd_info(info), passes=int(info[24]), chunks=int(info[25]))
     return cores
@@ -222,25 +242,20 @@ class TTSVDPlan:
     """Pre-allocated buffers for repeated decompositions of one shape (bench.py, serving loops)."""
 
     def __init__(self, shape: Sequence[int], dtype: torch.dtype, rmax=None, device="cuda", use_tensorcore: bool = True,
-                 host_io: bool = False, profile: bool = False, concurrent: bool = False, speculate: bool = True):
+                 host_io: bool = False, profile: bool = False, concurrent: bool = False, speculate: bool = True,
+                 batch_mode: bool = False):
         self.shape = [int(s) for s in shape]
         self.N = len(self.shape)
         self.dtype = dtype
         self.device = torch.device(device)
         self.code = _dense_code(dtype)
-        self.rm = _rmax_list(rmax, max(self.N - 1, 0))
         # concurrent: several plans run at once on different streams (TNB_FLAG_CONCURRENT, include/tnb200.h)
         self.flags = ((0 if use_tensorcore else _lib.FLAG_NO_TENSORCORE) | (_lib.FLAG_PROFILE if profile else 0) |
-                      (_lib.FLAG_CONCURRENT if concurrent else 0) | (0 if speculate else _lib.FLAG_NO_SPECULATE))
-        L = lib()
-        self._sh = i64(self.shape)
-        self._rm = i32(self.rm) if self.N > 1 else i32([0])
-        self._offs = (C.c_int64 * self.N)()
-        self.cap = L.tnb_ttsvd_cores_capacity(self.N, self._sh, self._rm, self._offs)
-        wsb = L.tnb_ttsvd_workspace_bytes(self.code, self.N, self._sh, self._rm, self.flags)
-        if self.cap < 0 or wsb == 0:
-            check(_lib.ERR_UNSUPPORTED)
-        self.ws = _ws(wsb, self.device)
+                      (_lib.FLAG_CONCURRENT if concurrent else 0) | (0 if speculate else _lib.FLAG_NO_SPECULATE) |
+                      (_lib.FLAG_BATCH_MODE if batch_mode else 0))
+        self._sh, self._rm, self._offs, self.cap = _ttsvd_layout(self.shape, rmax)
+        self.ws = _workspace(lib().tnb_ttsvd_workspace_bytes(self.code, self.N, self._sh, self._rm, self.flags),
+                             self.device)
         self.cores_buf = torch.empty(int(self.cap), dtype=_core_dtype(dtype), device=self.device)
         self.ranks = (C.c_int32 * (self.N + 1))()
         self.info = (C.c_double * 32)()
@@ -258,7 +273,7 @@ class TTSVDPlan:
             check(lib().tnb_ttsvd(self.code, _ptr(data), self.N, self._sh, self._rm, float(eps), self.flags,
                                   _ptr(self.ws), self.ws.numel(), _ptr(self.cores_buf), self.cap, self.ranks, self.info,
                                   _stream()))
-        return self._views(self.cores_buf)
+        return _slot_views(self.cores_buf, self._offs, self.ranks, self.shape)
 
     def run_host(self, data_host: torch.Tensor, eps: float = 1e-14):
         """End-to-end call on HOST buffers: H2D of the tensor, decomposition, D2H of the cores."""
@@ -267,14 +282,7 @@ class TTSVDPlan:
             check(lib().tnb_ttsvd_host(self.code, _ptr(data_host), self.N, self._sh, self._rm, float(eps), self.flags,
                                        _ptr(self.dev_in), _ptr(self.ws), self.ws.numel(), _ptr(self.cores_buf), self.cap,
                                        _ptr(self.cores_host), self.ranks, self.info, _stream()))
-        return self._views(self.cores_host)
-
-    def _views(self, buf):
-        out = []
-        for k in range(self.N):
-            r0, r1 = self.ranks[k], self.ranks[k + 1]
-            out.append(buf[self._offs[k]: self._offs[k] + r0 * self.shape[k] * r1].view(r0, self.shape[k], r1))
-        return out
+        return _slot_views(self.cores_host, self._offs, self.ranks, self.shape)
 
 
 class TTSVDBatchPlan:
@@ -290,20 +298,13 @@ class TTSVDBatchPlan:
         self.dtype = dtype
         self.device = torch.device(device)
         self.code = _dense_code(dtype)
-        self.rm = _rmax_list(rmax, max(self.N - 1, 0))
         self.flags = (0 if use_tensorcore else _lib.FLAG_NO_TENSORCORE) | (_lib.FLAG_BATCH_MODE if batch_mode else 0)
-        L = lib()
-        self._sh = i64(self.shape)
-        self._rm = i32(self.rm) if self.N > 1 else i32([0])
-        self._offs = (C.c_int64 * self.N)()
-        self.cap = L.tnb_ttsvd_cores_capacity(self.N, self._sh, self._rm, self._offs)
+        self._sh, self._rm, self._offs, self.cap = _ttsvd_layout(self.shape, rmax)
         one = C.c_size_t(0)
-        L.tnb_ttsvd_batch_workspace_bytes(self.code, self.batch, self.N, self._sh, self._rm, self.flags, C.byref(one))
-        if self.cap < 0 or one.value == 0:
-            check(_lib.ERR_UNSUPPORTED)
+        lib().tnb_ttsvd_batch_workspace_bytes(self.code, self.batch, self.N, self._sh, self._rm, self.flags, C.byref(one))
         self.per_tensor_bytes = int(one.value)
         self.inflight = max(1, min(int(inflight), self.batch, 8))
-        self.ws = _ws(self.per_tensor_bytes * self.inflight, self.device)
+        self.ws = _workspace(self.per_tensor_bytes * self.inflight, self.device)
         self.cores_buf = torch.empty(self.batch, int(self.cap), dtype=_core_dtype(dtype), device=self.device)
         self.ranks = (C.c_int32 * (self.batch * (self.N + 1)))()
         self.norms = (C.c_double * self.batch)()
@@ -330,7 +331,8 @@ class TTSVDBatchPlan:
             check(lib().tnb_ttsvd_batch(self.code, ptrs, self.batch, self.N, self._sh, self._rm, float(eps), self.flags,
                                         _ptr(self.ws), self.ws.numel(), self._cores_ptrs, self.cap, self.ranks, self.norms,
                                         self.spec, _stream()))
-        return [self._views(self.cores_buf[i], i) for i in range(self.batch)]
+        return [_slot_views(self.cores_buf[i], self._offs, self.ranks, self.shape, i * (self.N + 1))
+                for i in range(self.batch)]
 
     def run_host(self, tensors_host: torch.Tensor, eps: float = 1e-14):
         """End to end on HOST buffers: `tensors_host` [batch, ...] in (pinned) host memory -> device, decomposition,
@@ -342,15 +344,8 @@ class TTSVDBatchPlan:
         self.run(self.dev_in.view([self.batch] + self.shape), eps)
         self.cores_host.copy_(self.cores_buf, non_blocking=True)
         torch.cuda.current_stream().synchronize()
-        return [self._views(self.cores_host[i], i) for i in range(self.batch)]
-
-    def _views(self, buf, i):
-        out = []
-        base = i * (self.N + 1)
-        for k in range(self.N):
-            r0, r1 = self.ranks[base + k], self.ranks[base + k + 1]
-            out.append(buf[self._offs[k]: self._offs[k] + r0 * self.shape[k] * r1].view(r0, self.shape[k], r1))
-        return out
+        return [_slot_views(self.cores_host[i], self._offs, self.ranks, self.shape, i * (self.N + 1))
+                for i in range(self.batch)]
 
 
 def ttsvd_batch(tensors, rmax=None, eps: float = 1e-14, batch_mode: bool = False, inflight: int = 8,
@@ -381,18 +376,11 @@ def tt_round(cores: Sequence[torch.Tensor], eps: float = 1e-14, rmax=None, batch
     """Tensor.round_tt on device cores (tensor.py:2008-2083). Returns new cores.  speculate=False runs the host-driven
     sweeps even where the speculative one-synchronisation path is eligible (TNB_FLAG_NO_SPECULATE)."""
     N = len(cores)
-    for c in cores:
-        _require_cuda(c, "tt_round")
-        if c.dim() != 3:
-            raise ValueError("tt_round expects TT cores of shape [r, I, r']")
+    rin = _tt_ranks(cores, "tt_round")
     dt = cores[0].dtype
     cores = [c.contiguous() for c in cores]
     code = _dtype_code(cores[0])
     shape = [c.shape[1] for c in cores]
-    rin = [cores[0].shape[0]] + [c.shape[2] for c in cores]
-    for k in range(N - 1):
-        if cores[k].shape[2] != cores[k + 1].shape[0]:
-            raise ValueError("Core ranks do not match")
     rm = _rmax_list(rmax, max(N - 1, 0))
     L = lib()
     sh, rinc = i64(shape), i32(rin)
@@ -401,11 +389,8 @@ def tt_round(cores: Sequence[torch.Tensor], eps: float = 1e-14, rmax=None, batch
     cap = L.tnb_tt_round_cores_capacity(N, sh, rinc, rmc, offs)
     if cap < 0:
         check(_lib.ERR_INVALID)
-    wsb = L.tnb_tt_round_workspace_bytes(code, N, sh, rinc, rmc)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
     dev = cores[0].device
-    ws = _ws(wsb, dev)
+    ws = _workspace(L.tnb_tt_round_workspace_bytes(code, N, sh, rinc, rmc), dev)
     out = torch.empty(int(cap), dtype=dt, device=dev)
     ranks = (C.c_int32 * (N + 1))()
     ptrs = (C.c_void_p * N)(*[c.data_ptr() for c in cores])
@@ -413,11 +398,7 @@ def tt_round(cores: Sequence[torch.Tensor], eps: float = 1e-14, rmax=None, batch
     with torch.cuda.device(dev):
         check(L.tnb_tt_round(code, ptrs, N, sh, rinc, rmc, float(eps), flags, _ptr(ws), ws.numel(), _ptr(out), cap, ranks,
                              _stream()))
-    res = []
-    for k in range(N):
-        r0, r1 = ranks[k], ranks[k + 1]
-        res.append(out[offs[k]: offs[k] + r0 * shape[k] * r1].view(r0, shape[k], r1))
-    return res
+    return _slot_views(out, offs, ranks, shape)
 
 
 def tt_round_batch(batch_cores: Sequence[Sequence[torch.Tensor]], eps: float = 1e-14, rmax=None, batch_mode: bool = False,
@@ -434,26 +415,27 @@ def tt_round_batch(batch_cores: Sequence[Sequence[torch.Tensor]], eps: float = 1
     if B == 0:
         return []
     N = len(batch_cores[0])
-    dt, dev = batch_cores[0][0].dtype, batch_cores[0][0].device
     cs = [[c.contiguous() for c in cores] for cores in batch_cores]
-    shape = [c.shape[1] for c in cs[0]]
-    rin = [cs[0][0].shape[0]] + [c.shape[2] for c in cs[0]]
     for cores in cs:
-        if [c.shape for c in cores] != [c.shape for c in cs[0]]:
-            raise ValueError("tt_round_batch: all tensors must share their core shapes")
-    code = _DT[dt]
+        rin = _tt_ranks(cores, "tt_round_batch")
+        if ([c.shape for c in cores] != [c.shape for c in cs[0]] or cores[0].dtype != cs[0][0].dtype
+                or cores[0].device != cs[0][0].device):
+            raise ValueError("tt_round_batch: all tensors must share their core shapes, dtype and device")
+    dt, dev = cs[0][0].dtype, cs[0][0].device
+    code = _dtype_code(cs[0][0])
+    shape = [c.shape[1] for c in cs[0]]
     rm = _rmax_list(rmax, max(N - 1, 0))
     L = lib()
     sh, rinc = i64(shape), i32(rin)
     rmc = i32(rm) if N > 1 else i32([0])
     offs = (C.c_int64 * N)()
     cap = L.tnb_tt_round_cores_capacity(N, sh, rinc, rmc, offs)
+    if cap < 0:
+        check(_lib.ERR_INVALID)
     one = C.c_size_t(0)
-    total = L.tnb_tt_round_batch_workspace_bytes(code, B, N, sh, rinc, rmc, C.byref(one))
-    if cap < 0 or one.value == 0:
-        check(_lib.ERR_UNSUPPORTED)
+    L.tnb_tt_round_batch_workspace_bytes(code, B, N, sh, rinc, rmc, C.byref(one))
     k = max(1, min(int(inflight), B, 8))
-    ws = _ws(one.value * k, dev)
+    ws = _workspace(one.value * k, dev)
     out = torch.empty(B, int(cap), dtype=dt, device=dev)
     ranks = (C.c_int32 * (B * (N + 1)))()
     spec = (C.c_int32 * B)()
@@ -463,40 +445,34 @@ def tt_round_batch(batch_cores: Sequence[Sequence[torch.Tensor]], eps: float = 1
     with torch.cuda.device(dev):
         check(L.tnb_tt_round_batch(code, pin, B, N, sh, rinc, rmc, float(eps), flags, _ptr(ws), ws.numel(), pout, cap, ranks, spec,
                                    _stream()))
-    res = []
-    for i in range(B):
-        base = i * (N + 1)
-        res.append([out[i, offs[n]: offs[n] + ranks[base + n] * shape[n] * ranks[base + n + 1]].view(ranks[base + n], shape[n], ranks[base + n + 1])
-                    for n in range(N)])
+    res = [_slot_views(out[i], offs, ranks, shape, i * (N + 1)) for i in range(B)]
     if return_info:
         return res, dict(speculative=[int(x) for x in spec])
     return res
 
 
-def _tt_operands(operands):
+def _tt_operands(operands, what: str, boundary: bool = False):
     """operands: list of lists of TT cores [r, I, r'] (same shape, dtype, device) -> pointers / ranks for the C-ABI."""
     K = len(operands)
     N = len(operands[0])
-    dt, dev = operands[0][0].dtype, operands[0][0].device
     ops_c = [[c.contiguous() for c in cores] for cores in operands]
+    ranks = []
+    for cores in ops_c:
+        ranks += _tt_ranks(cores, what, boundary)
+    dt, dev = ops_c[0][0].dtype, ops_c[0][0].device
     shape = [c.shape[1] for c in ops_c[0]]
     for cores in ops_c:
         if len(cores) != N or [c.shape[1] for c in cores] != shape:
             raise ValueError("TT operands must share their shape")
-        for c in cores:
-            _require_cuda(c, "tt_sum")
-            if c.dim() != 3 or c.dtype != dt:
-                raise ValueError("TT operands must be lists of [r, I, r'] cores of one dtype")
-    ranks = []
-    for cores in ops_c:
-        ranks += [cores[0].shape[0]] + [c.shape[2] for c in cores]
+        if cores[0].dtype != dt or cores[0].device != dev:
+            raise ValueError("TT operands must be lists of [r, I, r'] cores of one dtype on one device")
     ptrs = (C.c_void_p * (K * N))(*[c.data_ptr() for cores in ops_c for c in cores])
     return ops_c, K, N, shape, ranks, ptrs, dt, dev
 
 
 def tt_sum(operands, alpha=None):
     """sum_k alpha_k T_k as block TT cores (Tensor.__add__, tensor.py:445-520); no rounding."""
-    ops_c, K, N, shape, ranks, ptrs, dt, dev = _tt_operands(operands)
+    ops_c, K, N, shape, ranks, ptrs, dt, dev = _tt_operands(operands, "tt_sum")
     L = lib()
     rsum = (C.c_int32 * (N + 1))()
     offs = (C.c_int64 * N)()
@@ -507,13 +483,13 @@ def tt_sum(operands, alpha=None):
     al = None if alpha is None else (C.c_double * K)(*[float(a) for a in alpha])
     with torch.cuda.device(dev):
         check(L.tnb_tt_sum(_dtype_code(ops_c[0][0]), ptrs, K, al, N, i64(shape), i32(ranks), _ptr(out), cap, _stream()))
-    return [out[offs[n]: offs[n] + rsum[n] * shape[n] * rsum[n + 1]].view(rsum[n], shape[n], rsum[n + 1]) for n in range(N)]
+    return _slot_views(out, offs, rsum, shape)
 
 
 def tt_sum_round(operands, alpha=None, eps: float = 1e-14, rmax=None, speculate: bool = True):
     """round_tt(sum_k alpha_k T_k) in ONE library call: block cores assembled in the workspace, then the rounding sweeps
     (the `tn.round(function(a, b))` step of tools.reduce, tools.py:460-512).  speculate as for tt_round."""
-    ops_c, K, N, shape, ranks, ptrs, dt, dev = _tt_operands(operands)
+    ops_c, K, N, shape, ranks, ptrs, dt, dev = _tt_operands(operands, "tt_sum_round")
     L = lib()
     rm = _rmax_list(rmax, max(N - 1, 0))
     rmc = i32(rm) if N > 1 else i32([0])
@@ -522,10 +498,7 @@ def tt_sum_round(operands, alpha=None, eps: float = 1e-14, rmax=None, speculate:
     if cap < 0:
         check(_lib.ERR_INVALID)
     code = _dtype_code(ops_c[0][0])
-    wsb = L.tnb_tt_sum_round_workspace_bytes(code, K, N, i64(shape), i32(ranks), rmc)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, dev)
+    ws = _workspace(L.tnb_tt_sum_round_workspace_bytes(code, K, N, i64(shape), i32(ranks), rmc), dev)
     out = torch.empty(int(cap), dtype=dt, device=dev)
     rk = (C.c_int32 * (N + 1))()
     al = None if alpha is None else (C.c_double * K)(*[float(a) for a in alpha])
@@ -533,12 +506,12 @@ def tt_sum_round(operands, alpha=None, eps: float = 1e-14, rmax=None, speculate:
     with torch.cuda.device(dev):
         check(L.tnb_tt_sum_round(code, ptrs, K, al, N, i64(shape), i32(ranks), rmc, float(eps), flags, _ptr(ws), ws.numel(), _ptr(out),
                                  cap, rk, _stream()))
-    return [out[offs[n]: offs[n] + rk[n] * shape[n] * rk[n + 1]].view(rk[n], shape[n], rk[n + 1]) for n in range(N)]
+    return _slot_views(out, offs, rk, shape)
 
 
 def tt_hadamard(a_cores, b_cores):
     """Elementwise product of two TT tensors: Kronecker cores (Tensor.__mul__, tensor.py:560-640)."""
-    ops_c, K, N, shape, ranks, ptrs, dt, dev = _tt_operands([a_cores, b_cores])
+    ops_c, K, N, shape, ranks, ptrs, dt, dev = _tt_operands([a_cores, b_cores], "tt_hadamard")
     ra, rb = ranks[: N + 1], ranks[N + 1:]
     outs = [torch.empty(ra[n] * rb[n], shape[n], ra[n + 1] * rb[n + 1], dtype=dt, device=dev) for n in range(N)]
     pa = (C.c_void_p * N)(*[c.data_ptr() for c in ops_c[0]])
@@ -558,10 +531,8 @@ def tt_hadamard_round(a_cores, b_cores, eps: float = 1e-14, rmax=None, return_in
     input dtype.  return_info adds dict(norm_sq=||a*b||^2, discarded_sq=||a*b - result||^2).  Envelope: a bond Gram of
     I_mu r_{mu+1} up to 46000 and, where it is wider than 256, a kept rank up to 240 (NotImplementedError otherwise):
     eps-only calls at large ranks need rmax.  use_tensorcore=False runs every GEMM on CUDA-core tiles."""
-    ops_c, K, N, shape, ranks, ptrs, dt, dev = _tt_operands([a_cores, b_cores])
+    ops_c, K, N, shape, ranks, ptrs, dt, dev = _tt_operands([a_cores, b_cores], "tt_hadamard_round", boundary=True)
     ra, rb = ranks[: N + 1], ranks[N + 1:]
-    if ra[0] != 1 or ra[N] != 1 or rb[0] != 1 or rb[N] != 1:
-        raise ValueError("tt_hadamard_round: boundary ranks must be 1")
     if any(c.requires_grad for cores in ops_c for c in cores):
         raise ValueError("tt_hadamard_round: cores that require grad are not supported")
     code = _dtype_code(ops_c[0][0])
@@ -573,10 +544,7 @@ def tt_hadamard_round(a_cores, b_cores, eps: float = 1e-14, rmax=None, return_in
     cap = L.tnb_tt_hadamard_round_cores_capacity(N, sh, rac, rbc, rmc, offs)
     if cap < 0:
         check(_lib.ERR_INVALID)
-    wsb = L.tnb_tt_hadamard_round_workspace_bytes(code, N, sh, rac, rbc, rmc)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, dev)
+    ws = _workspace(L.tnb_tt_hadamard_round_workspace_bytes(code, N, sh, rac, rbc, rmc), dev)
     out = torch.empty(int(cap), dtype=dt, device=dev)
     rk = (C.c_int32 * (N + 1))()
     en = (C.c_double * 2)()
@@ -586,7 +554,7 @@ def tt_hadamard_round(a_cores, b_cores, eps: float = 1e-14, rmax=None, return_in
     with torch.cuda.device(dev):
         check(L.tnb_tt_hadamard_round(code, pa, pb, N, sh, rac, rbc, rmc, float(eps), flags, _ptr(ws), ws.numel(), _ptr(out),
                                       cap, rk, en, _stream()))
-    res = [out[offs[n]: offs[n] + rk[n] * shape[n] * rk[n + 1]].view(rk[n], shape[n], rk[n + 1]) for n in range(N)]
+    res = _slot_views(out, offs, rk, shape)
     if return_info:
         return res, dict(norm_sq=float(en[0]), discarded_sq=float(en[1]))
     return res
@@ -630,10 +598,7 @@ def truncated_svd(M: torch.Tensor, delta=None, eps=None, rmax=None, left_ortho=T
         assert rmax >= 1
         rm = int(min(rmax, 2**31 - 1))
     L = lib()
-    wsb = L.tnb_truncated_svd_workspace_bytes(code, m, n)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, M.device)
+    ws = _workspace(L.tnb_truncated_svd_workspace_bytes(code, m, n), M.device)
     k = min(m, n)
     left = torch.empty(m * k, dtype=M.dtype, device=M.device)
     right = torch.empty(k * n, dtype=M.dtype, device=M.device)
@@ -662,10 +627,7 @@ def cp_als(data: torch.Tensor, R: int, max_iter: int = 25, tol: float = 1e-4, re
     cap = L.tnb_cp_als_factors_capacity(N, sh, int(R), offs)
     if cap < 0:
         check(_lib.ERR_INVALID if N >= 2 else _lib.ERR_UNSUPPORTED)
-    wsb = L.tnb_cp_als_workspace_bytes(code, N, sh, int(R))
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, data.device)
+    ws = _workspace(L.tnb_cp_als_workspace_bytes(code, N, sh, int(R)), data.device)
     fac = torch.zeros(int(cap), dtype=data.dtype, device=data.device)
     errs = (C.c_double * max(int(max_iter), 1))()
     iters = (C.c_int32 * 1)()
@@ -843,10 +805,7 @@ def gram(A: torch.Tensor, tensorcore: bool = False) -> torch.Tensor:
         if tensorcore:
             if A.dtype != torch.float32:
                 raise ValueError("tensor-core Gram needs float32 input")
-            wsb = L.tnb_gram_tc_workspace_bytes(rows, n)
-            if wsb == 0:
-                check(_lib.ERR_UNSUPPORTED)
-            ws = _ws(wsb, A.device)
+            ws = _workspace(L.tnb_gram_tc_workspace_bytes(rows, n), A.device)
             check(L.tnb_gram_tc_f32(_ptr(A), rows, n, _ptr(G), _ptr(ws), ws.numel(), _stream()))
         else:
             code = _dtype_code(A)
@@ -874,12 +833,32 @@ def gram_kblocked(B: torch.Tensor, rows: int, n: int) -> torch.Tensor:
     assert B.dtype == torch.float32 and B.is_contiguous() and B.numel() == rows * n
     G = torch.empty(n, n, dtype=torch.float64, device=B.device)
     L = lib()
-    wsb = L.tnb_gram_tc_workspace_bytes(rows, n)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, B.device)
+    ws = _workspace(L.tnb_gram_tc_workspace_bytes(rows, n), B.device)
     with torch.cuda.device(B.device):
         check(L.tnb_gram_tc_kblocked_f32(_ptr(B), rows, n, _ptr(G), _ptr(ws), ws.numel(), _stream()))
+    return G
+
+
+# The 16- and 8-bit tensor-core Gram and projection of each input dtype: (Gram sizing query, Gram entry point,
+# projection entry point, leading arguments).  Both float8 formats share entry points that take the format's code.
+_TC_LOWP = {
+    torch.bfloat16: ("tnb_gram_tc_bf16_workspace_bytes", "tnb_gram_tc_bf16", "tnb_project_tc_bf16", ()),
+    torch.float16: ("tnb_gram_tc_f16_workspace_bytes", "tnb_gram_tc_f16", "tnb_project_tc_f16", ()),
+    **{dt: ("tnb_gram_tc_f8_workspace_bytes", "tnb_gram_tc_f8", "tnb_project_tc_f8", (code,))
+       for dt, code in _DT_F8.items()},
+}
+
+
+def _gram_lowp(A: torch.Tensor) -> torch.Tensor:
+    """gram_bf16 / gram_f16 / gram_f8 on a CUDA matrix of their dtype."""
+    size, gram, _, lead = _TC_LOWP[A.dtype]
+    A = A.contiguous()
+    rows, n = A.shape
+    G = torch.empty(n, n, dtype=torch.float64, device=A.device)
+    L = lib()
+    ws = _workspace(getattr(L, size)(rows, n), A.device)
+    with torch.cuda.device(A.device):
+        check(getattr(L, gram)(*lead, _ptr(A), rows, n, _ptr(G), _ptr(ws), ws.numel(), _stream()))
     return G
 
 
@@ -888,17 +867,7 @@ def gram_bf16(A: torch.Tensor) -> torch.Tensor:
     accumulation): n % 8 == 0 and n = 32 / 64 (rows divisible by 128 / n), 128 or >= 256."""
     _require_cuda(A, "gram_bf16")
     assert A.dtype == torch.bfloat16
-    A = A.contiguous()
-    rows, n = A.shape
-    G = torch.empty(n, n, dtype=torch.float64, device=A.device)
-    L = lib()
-    wsb = L.tnb_gram_tc_bf16_workspace_bytes(rows, n)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, A.device)
-    with torch.cuda.device(A.device):
-        check(L.tnb_gram_tc_bf16(_ptr(A), rows, n, _ptr(G), _ptr(ws), ws.numel(), _stream()))
-    return G
+    return _gram_lowp(A)
 
 
 def gram_f16(A: torch.Tensor) -> torch.Tensor:
@@ -906,17 +875,7 @@ def gram_f16(A: torch.Tensor) -> torch.Tensor:
     products, fp32 accumulation); the shapes of gram_bf16."""
     _require_cuda(A, "gram_f16")
     assert A.dtype == torch.float16
-    A = A.contiguous()
-    rows, n = A.shape
-    G = torch.empty(n, n, dtype=torch.float64, device=A.device)
-    L = lib()
-    wsb = L.tnb_gram_tc_f16_workspace_bytes(rows, n)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, A.device)
-    with torch.cuda.device(A.device):
-        check(L.tnb_gram_tc_f16(_ptr(A), rows, n, _ptr(G), _ptr(ws), ws.numel(), _stream()))
-    return G
+    return _gram_lowp(A)
 
 
 def gram_f8(A: torch.Tensor) -> torch.Tensor:
@@ -924,17 +883,7 @@ def gram_f8(A: torch.Tensor) -> torch.Tensor:
     widened to fp16 in shared memory (exact products, fp32 accumulation); the shapes of gram_bf16 with n % 16 == 0."""
     _require_cuda(A, "gram_f8")
     assert A.dtype in _DT_F8
-    A = A.contiguous()
-    rows, n = A.shape
-    G = torch.empty(n, n, dtype=torch.float64, device=A.device)
-    L = lib()
-    wsb = L.tnb_gram_tc_f8_workspace_bytes(rows, n)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, A.device)
-    with torch.cuda.device(A.device):
-        check(L.tnb_gram_tc_f8(_DT_F8[A.dtype], _ptr(A), rows, n, _ptr(G), _ptr(ws), ws.numel(), _stream()))
-    return G
+    return _gram_lowp(A)
 
 
 def gram_noise_level(dtype: torch.dtype) -> float:
@@ -943,23 +892,27 @@ def gram_noise_level(dtype: torch.dtype) -> float:
     return float(lib().tnb_gram_noise_level(_dense_code(dtype)))
 
 
-def project_bf16(A: torch.Tensor, V: torch.Tensor, inner: int = 0) -> torch.Tensor:
-    """A (rows x n, bfloat16) @ V (n x r, float32) at fp32 accuracy on the tensor cores, float32 result.  inner > 0
-    writes it K-blocked like project_kblocked_out (returned flat)."""
-    _require_cuda(A, "project_bf16")
-    assert A.dtype == torch.bfloat16 and V.dtype == torch.float32
+def _project_lowp(A: torch.Tensor, V: torch.Tensor, inner: int) -> torch.Tensor:
+    """project_bf16 / project_f16 / project_f8 on a CUDA matrix of their dtype and a float32 V."""
+    project, lead = _TC_LOWP[A.dtype][2:]
     A, V = A.contiguous(), V.contiguous()
     rows, n = A.shape
     r = V.shape[1]
     out = torch.empty(rows * r if inner > 0 else (rows, r), dtype=torch.float32, device=A.device)
     L = lib()
-    wsb = L.tnb_project_tc_workspace_bytes(n, r)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, A.device)
+    ws = _workspace(L.tnb_project_tc_workspace_bytes(n, r), A.device)
     with torch.cuda.device(A.device):
-        check(L.tnb_project_tc_bf16(_ptr(A), rows, n, _ptr(V), r, int(inner), _ptr(out), _ptr(ws), ws.numel(), _stream()))
+        check(getattr(L, project)(*lead, _ptr(A), rows, n, _ptr(V), r, int(inner), _ptr(out), _ptr(ws), ws.numel(),
+                                  _stream()))
     return out
+
+
+def project_bf16(A: torch.Tensor, V: torch.Tensor, inner: int = 0) -> torch.Tensor:
+    """A (rows x n, bfloat16) @ V (n x r, float32) at fp32 accuracy on the tensor cores, float32 result.  inner > 0
+    writes it K-blocked like project_kblocked_out (returned flat)."""
+    _require_cuda(A, "project_bf16")
+    assert A.dtype == torch.bfloat16 and V.dtype == torch.float32
+    return _project_lowp(A, V, inner)
 
 
 def project_f16(A: torch.Tensor, V: torch.Tensor, inner: int = 0) -> torch.Tensor:
@@ -968,18 +921,7 @@ def project_f16(A: torch.Tensor, V: torch.Tensor, inner: int = 0) -> torch.Tenso
     flat)."""
     _require_cuda(A, "project_f16")
     assert A.dtype == torch.float16 and V.dtype == torch.float32
-    A, V = A.contiguous(), V.contiguous()
-    rows, n = A.shape
-    r = V.shape[1]
-    out = torch.empty(rows * r if inner > 0 else (rows, r), dtype=torch.float32, device=A.device)
-    L = lib()
-    wsb = L.tnb_project_tc_workspace_bytes(n, r)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, A.device)
-    with torch.cuda.device(A.device):
-        check(L.tnb_project_tc_f16(_ptr(A), rows, n, _ptr(V), r, int(inner), _ptr(out), _ptr(ws), ws.numel(), _stream()))
-    return out
+    return _project_lowp(A, V, inner)
 
 
 def project_f8(A: torch.Tensor, V: torch.Tensor, inner: int = 0) -> torch.Tensor:
@@ -988,19 +930,7 @@ def project_f8(A: torch.Tensor, V: torch.Tensor, inner: int = 0) -> torch.Tensor
     project_kblocked_out (returned flat)."""
     _require_cuda(A, "project_f8")
     assert A.dtype in _DT_F8 and V.dtype == torch.float32
-    A, V = A.contiguous(), V.contiguous()
-    rows, n = A.shape
-    r = V.shape[1]
-    out = torch.empty(rows * r if inner > 0 else (rows, r), dtype=torch.float32, device=A.device)
-    L = lib()
-    wsb = L.tnb_project_tc_workspace_bytes(n, r)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, A.device)
-    with torch.cuda.device(A.device):
-        check(L.tnb_project_tc_f8(_DT_F8[A.dtype], _ptr(A), rows, n, _ptr(V), r, int(inner), _ptr(out), _ptr(ws),
-                                  ws.numel(), _stream()))
-    return out
+    return _project_lowp(A, V, inner)
 
 
 def atb_tensorcore(A: torch.Tensor, B: torch.Tensor, alpha: float = 1.0, D: Optional[torch.Tensor] = None,
@@ -1011,10 +941,7 @@ def atb_tensorcore(A: torch.Tensor, B: torch.Tensor, alpha: float = 1.0, D: Opti
     K, m = A.shape
     n = B.shape[1]
     L = lib()
-    wsb = L.tnb_atb_tc_workspace_bytes(K, m, n)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, A.device)
+    ws = _workspace(L.tnb_atb_tc_workspace_bytes(K, m, n), A.device)
     out = torch.empty(m, n, dtype=torch.float32, device=A.device)
     with torch.cuda.device(A.device):
         check(L.tnb_atb_tc_f32(_ptr(A), K, m, _ptr(B), n, _ptr(out), float(alpha), _ptr(D), float(beta), _ptr(ws),
@@ -1029,10 +956,7 @@ def cheb_filter(G: torch.Tensor, Y0: torch.Tensor, a, bc, g) -> torch.Tensor:
     n, b = Y0.shape
     steps = len(a)
     bufs = [Y0.contiguous().clone(), torch.empty_like(Y0), torch.empty_like(Y0)]
-    wsb = lib().tnb_cheb_filter_workspace_bytes(n, b)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, G.device)
+    ws = _workspace(lib().tnb_cheb_filter_workspace_bytes(n, b), G.device)
     fa, fb, fg = ((C.c_float * steps)(*[float(v) for v in x]) for x in (a, bc, g))
     with torch.cuda.device(G.device):
         check(lib().tnb_cheb_filter_f32(_ptr(G.contiguous()), n, b, _ptr(bufs[0]), _ptr(bufs[1]), _ptr(bufs[2]), steps,
@@ -1050,9 +974,9 @@ def project(A: torch.Tensor, V: torch.Tensor, tensorcore: bool = False) -> torch
     if tensorcore:
         L = lib()
         wsb = L.tnb_project_tc_workspace_bytes(n, r)
-        if wsb == 0 or A.dtype != torch.float32:
+        if A.dtype != torch.float32:
             check(_lib.ERR_UNSUPPORTED)
-        ws = _ws(wsb, A.device)
+        ws = _workspace(wsb, A.device)
         with torch.cuda.device(A.device):
             check(L.tnb_project_tc_f32(_ptr(A), rows, n, _ptr(V), r, _ptr(Cc), _ptr(ws), ws.numel(), _stream()))
         return Cc
@@ -1071,9 +995,9 @@ def project_kblocked_out(A: torch.Tensor, V: torch.Tensor, inner: int) -> torch.
     out = torch.empty(rows * r, dtype=torch.float32, device=A.device)
     L = lib()
     wsb = L.tnb_project_tc_workspace_bytes(n, r)
-    if wsb == 0 or A.dtype != torch.float32:
+    if A.dtype != torch.float32:
         check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, A.device)
+    ws = _workspace(wsb, A.device)
     with torch.cuda.device(A.device):
         check(L.tnb_project_tc_kblocked_out_f32(_ptr(A), rows, n, _ptr(V), r, int(inner), _ptr(out), _ptr(ws), ws.numel(),
                                                 _stream()))
@@ -1088,10 +1012,7 @@ def project_kblocked_in(B: torch.Tensor, rows: int, V: torch.Tensor) -> torch.Te
     assert B.dtype == torch.float32 and B.is_contiguous() and B.numel() == rows * n
     Cc = torch.empty(rows, r, dtype=torch.float32, device=B.device)
     L = lib()
-    wsb = L.tnb_project_tc_workspace_bytes(n, r)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, B.device)
+    ws = _workspace(L.tnb_project_tc_workspace_bytes(n, r), B.device)
     with torch.cuda.device(B.device):
         check(L.tnb_project_tc_kblocked_in_f32(_ptr(B), rows, n, _ptr(V), r, _ptr(Cc), _ptr(ws), ws.numel(), _stream()))
     return Cc
@@ -1104,10 +1025,7 @@ def eigh_jacobi(G: torch.Tensor, return_sweeps: bool = False):
     w = torch.empty(n, dtype=torch.float64, device=G.device)
     V = torch.empty(n, n, dtype=torch.float64, device=G.device)
     L = lib()
-    wsb = L.tnb_eigh_workspace_bytes(n)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, G.device)
+    ws = _workspace(L.tnb_eigh_workspace_bytes(n), G.device)
     with torch.cuda.device(G.device):
         check(L.tnb_eigh_jacobi(_ptr(G), n, _ptr(w), _ptr(V), _ptr(ws), ws.numel(), _stream()))
     if return_sweeps:  # the kernel leaves its sweep count right behind the (256-byte aligned) scratch matrices
@@ -1141,19 +1059,14 @@ def tt_relative_error(data: torch.Tensor, cores: Sequence[torch.Tensor]) -> floa
     cores = [c.contiguous() for c in cores]
     N = data.dim()
     code = _dense_code(data.dtype)
-    if data.dtype in _DT_LOW and any(c.dtype != torch.float32 for c in cores):
+    ranks = _tt_ranks(cores, "tt_relative_error")
+    if data.dtype in _DT_LOW and cores[0].dtype != torch.float32:
         raise ValueError(f"tt_relative_error: {str(data.dtype).replace('torch.', '')} data needs float32 cores")
-    if len(cores) != N or any(c.dim() != 3 for c in cores) or [c.shape[1] for c in cores] != list(data.shape):
+    if len(cores) != N or [c.shape[1] for c in cores] != list(data.shape):
         raise ValueError("tt_relative_error: the cores' mode sizes must match data.shape")
-    if any(cores[k].shape[2] != cores[k + 1].shape[0] for k in range(N - 1)):
-        raise ValueError("tt_relative_error: consecutive core ranks do not match")
-    ranks = [cores[0].shape[0]] + [c.shape[2] for c in cores]
     L = lib()
     sh, rk = i64(list(data.shape)), i32(ranks)
-    wsb = L.tnb_tt_relative_error_workspace_bytes(code, N, sh, rk)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, data.device)
+    ws = _workspace(L.tnb_tt_relative_error_workspace_bytes(code, N, sh, rk), data.device)
     ptrs = (C.c_void_p * N)(*[c.data_ptr() for c in cores])
     res = (C.c_double * 1)()
     with torch.cuda.device(data.device):
@@ -1171,19 +1084,10 @@ def tt_decompress(cores: Sequence[torch.Tensor], dtype: Optional[torch.dtype] = 
     also decompress to bfloat16 or float16 (the float32 result rounded once).  `out`: a preallocated contiguous tensor of
     the result's shape and dtype."""
     cores = list(cores)
-    if not cores or any(c.dim() != 3 for c in cores):
-        raise ValueError("tt_decompress: cores must be 3-D tensors [r, I, r']")
+    ranks = _tt_ranks(cores, "tt_decompress", boundary=True)
     c0 = cores[0]
-    _require_cuda(c0, "tt_decompress")
-    if any(c.dtype != c0.dtype or c.device != c0.device for c in cores):
-        raise ValueError("tt_decompress: cores must share one dtype and one device")
     if any(c.requires_grad for c in cores):
         raise ValueError("tt_decompress: cores that require grad are not supported (use Tensor.torch() without arguments)")
-    ranks = [c0.shape[0]] + [c.shape[2] for c in cores]
-    if ranks[0] != 1 or ranks[-1] != 1:
-        raise ValueError(f"tt_decompress: boundary ranks must be 1, got {ranks[0]} and {ranks[-1]}")
-    if any(a.shape[2] != b.shape[0] for a, b in zip(cores[:-1], cores[1:])):
-        raise ValueError("tt_decompress: core ranks do not match")
     dtype = c0.dtype if dtype is None else dtype
     shape = [c.shape[1] for c in cores]
     if out is None:
@@ -1255,22 +1159,19 @@ def tt_gather_batch(trains, idx, first: int = 0, last: Optional[int] = None, che
         raise ValueError(f"tt_gather: mode range [{first}, {last}) is not inside [0, {N})")
     shape, ranks = None, []
     for cores in trains:
-        if len(cores) != N or any(c.dim() != 3 for c in cores):
+        if len(cores) != N:
             raise ValueError(f"tt_gather: every train must be {N} 3-D cores [r, I, r']")
-        if any(a.shape[2] != b.shape[0] for a, b in zip(cores[:-1], cores[1:])):
-            raise ValueError("tt_gather: core ranks do not match")
+        ranks += _tt_ranks(cores, "tt_gather")
         sh = [c.shape[1] for c in cores]
         if shape is None:
             shape = sh
         elif sh != shape:
             raise ValueError(f"tt_gather: every train must have the shape {shape}, got {sh}")
-        ranks += [cores[0].shape[0]] + [c.shape[2] for c in cores]
     R = N + 1
     ra, rl = ranks[first], ranks[last]
     if any(ranks[t * R + first] != ra or ranks[t * R + last] != rl for t in range(len(trains))):
         raise ValueError("tt_gather: every train must have the same ranks at the ends of the range")
     c0 = trains[0][first]
-    _require_cuda(c0, "tt_gather")
     allc = [c for cores in trains for c in cores[first:last]]
     if any(c.device != c0.device for c in allc):
         raise ValueError("tt_gather: cores must share one CUDA device")
@@ -1306,9 +1207,7 @@ class _GatherPlan:
         sh, rk = i64(self.shape), i32(self.ranks)
         B, N, first, last, P = self.B, self.N, self.first, self.last, self.P
         wsb = L.tnb_tt_gather_workspace_bytes(code, B, N, sh, rk, first, last, P)
-        if wsb == 0:
-            _lib.check(_lib.ERR_UNSUPPORTED)
-        ws = _ws(wsb, c0.device)
+        ws = _workspace(wsb, c0.device)
         out = torch.empty(B, self.ranks[first], P, self.ranks[last], dtype=c0.dtype, device=c0.device)
         with torch.cuda.device(c0.device):
             _lib.check(L.tnb_tt_gather(code, self._ptrs(cs), B, N, sh, rk, first, last, _ptr(self.key), P, _ptr(out),
@@ -1325,9 +1224,7 @@ class _GatherPlan:
         sh, rk = i64(self.shape), i32(self.ranks)
         B, N, first, last, P = self.B, self.N, self.first, self.last, self.P
         wsb = L.tnb_tt_gather_grad_workspace_bytes(code, B, N, sh, rk, first, last, P)
-        if wsb == 0:
-            _lib.check(_lib.ERR_UNSUPPORTED)
-        ws = _ws(wsb, c0.device)
+        ws = _workspace(wsb, c0.device)
         with torch.cuda.device(c0.device):
             _lib.check(L.tnb_tt_gather_grad(code, self._ptrs(cs), B, N, sh, rk, first, last, _ptr(self.key), P,
                                             _ptr(gout), self._ptrs(grads), _ptr(ws), wsb, _stream()))
@@ -1402,24 +1299,11 @@ def tt_multiply(cores: Sequence[torch.Tensor], X: torch.Tensor) -> torch.Tensor:
     L = lib()
     ii, oo, rk = i64(idims), i64(odims), i32(ranks)
     wsb = L.tnb_tt_multiply_workspace_bytes(code, d, ii, oo, rk, b)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, c0.device)
+    ws = _workspace(wsb, c0.device)
     ptrs = (C.c_void_p * d)(*[c.data_ptr() for c in cores])
     with torch.cuda.device(c0.device):
         check(L.tnb_tt_multiply(code, ptrs, d, ii, oo, rk, _ptr(X), b, _ptr(Y), _ptr(ws), wsb, _stream()))
     return Y
-
-
-def _tt_ranks(cores, what: str):
-    if not cores or any(c.dim() != 3 for c in cores):
-        raise ValueError(f"{what}: cores must be 3-D tensors [r, I, r']")
-    ranks = [cores[0].shape[0]] + [c.shape[2] for c in cores]
-    if ranks[0] != 1 or ranks[-1] != 1:
-        raise ValueError(f"{what}: boundary ranks must be 1, got {ranks[0]} and {ranks[-1]}")
-    if any(a.shape[2] != b.shape[0] for a, b in zip(cores[:-1], cores[1:])):
-        raise ValueError(f"{what}: core ranks do not match")
-    return ranks
 
 
 def tt_dot_batch(pairs) -> torch.Tensor:
@@ -1437,14 +1321,13 @@ def tt_dot_batch(pairs) -> torch.Tensor:
         if len(a) != len(b):
             raise NotImplementedError(f"tt_dot: trains of unequal length ({len(a)} and {len(b)} cores) are not supported")
         for cores, rk in ((a, ranks_a), (b, ranks_b)):
-            rk += _tt_ranks(cores, "tt_dot")
+            rk += _tt_ranks(cores, "tt_dot", boundary=True, one_dtype=False)
             sh = [c.shape[1] for c in cores]
             if shape is None:
                 shape = sh
             elif sh != shape:
                 raise ValueError(f"tt_dot: every train must have the shape {shape}, got {sh}")
     c0 = pairs[0][0][0]
-    _require_cuda(c0, "tt_dot")
     allc = [c for a, b in pairs for c in a + b]
     if any(c.device != c0.device for c in allc):
         raise ValueError("tt_dot: cores must share one CUDA device")
@@ -1465,9 +1348,7 @@ def tt_dot_batch(pairs) -> torch.Tensor:
     L = lib()
     sh, ra, rb = i64(shape), i32(ranks_a), i32(ranks_b)
     wsb = L.tnb_tt_dot_workspace_bytes(code, P, N, sh, ra, rb)
-    if wsb == 0:
-        check(_lib.ERR_UNSUPPORTED)
-    ws = _ws(wsb, c0.device)
+    ws = _workspace(wsb, c0.device)
     out = torch.empty(P, dtype=torch.float64, device=c0.device)
     pa = (C.c_void_p * (P * N))(*[c.data_ptr() for c in ca])
     pb = (C.c_void_p * (P * N))(*[c.data_ptr() for c in cb])

@@ -34,8 +34,8 @@ def _streams(data: torch.Tensor, ranks_tt, dev) -> bool:
     if data.is_cuda or data.dim() < 2:
         return False
     shape = list(data.shape)
-    rm = ops._rmax_list(ranks_tt, len(shape) - 1)
-    wsb = ops.lib().tnb_ttsvd_workspace_bytes(ops._dense_code(data.dtype), len(shape), ops.i64(shape), ops.i32(rm), 0)
+    sh, rm, _, _ = ops._ttsvd_layout(shape, ranks_tt)
+    wsb = ops.lib().tnb_ttsvd_workspace_bytes(ops._dense_code(data.dtype), len(shape), sh, rm, 0)
     free, _ = torch.cuda.mem_get_info(dev)
     return ops.stream_instead_of_copy(data.numel() * data.element_size(), int(wsb), int(free))
 
